@@ -33,22 +33,21 @@ _SCALE = float(os.environ.get("B2S_BENCH_SCALE", "1"))  # scaling experiments on
 CONFIGS = {
     2: dict(parts=[("Lift", "Panda", "OSC_POSE", 4096)],
             metric="env-steps/sec (device-timed) Panda-Lift OSC_POSE @4096 envs per GPU",
-            workload="4096 Panda Lift envs, OSC_POSE, fp32, random actions, 1xB200 (BASELINE.json configs[1]); weak-scaled: 4096 envs per GPU"),
+            workload="4096 Panda Lift envs, OSC_POSE, fp32, random actions, 1xH100 (BASELINE.json configs[1]); weak-scaled: 4096 envs per GPU"),
     3: dict(parts=[("Stack", "Sawyer", "JOINT_VELOCITY", 8192)],
             metric="env-steps/sec (device-timed) Sawyer-Stack JOINT_VELOCITY @8192 envs per GPU",
-            workload="8192 Sawyer Stack envs (contact-rich), JOINT_VELOCITY controller, 1xB200 (BASELINE.json configs[2]); weak-scaled"),
+            workload="8192 Sawyer Stack envs (contact-rich), JOINT_VELOCITY controller, 1xH100 (BASELINE.json configs[2]); weak-scaled"),
     4: dict(parts=[("NutAssemblyRound", "Panda", "OSC_POSE", 16384)],
             metric="env-steps/sec (device-timed) Panda-NutAssemblyRound OSC_POSE @16384 envs per GPU",
-            workload="16384 Panda NutAssemblyRound envs (peg-in-hole), OSC_POSE, 1xB200 (BASELINE.json configs[3]); weak-scaled"),
+            workload="16384 Panda NutAssemblyRound envs (peg-in-hole), OSC_POSE, 1xH100 (BASELINE.json configs[3]); weak-scaled"),
     5: dict(parts=[("Lift", "Panda", "OSC_POSE", 2048), ("Stack", "Panda", "OSC_POSE", 2048), ("Door", "Panda", "OSC_POSE", 2048),
                    ("PickPlace", "Panda", "OSC_POSE", 2048)],
             metric="env-steps/sec (device-timed) mixed Lift/Stack/Door/PickPlace @8192 envs per GPU, obs all-gather",
-            workload="65536 mixed Lift/Stack/Door/PickPlace envs sharded across 8xB200 = 4 x 2048 per GPU, NCCL obs all-gather "
+            workload="65536 mixed Lift/Stack/Door/PickPlace envs sharded across 8xH100 = 4 x 2048 per GPU, NCCL obs all-gather "
                      "(BASELINE.json configs[4]); weak-scaled: 8192 envs per GPU"),
 }
-# Static per-environment-substep instruction counts from the ncu captures under profiles/ (warp-level instructions executed),
-# and SURVEY.md section 8d's useful-FLOP estimate: the inputs of roofline.compute
-INST_COUNTS = os.path.join(ROOT, "profiles", "inst_counts.json")
+# --dump-outputs writes at most this many bytes (a seeded sample of environments beyond it)
+DUMP_BYTES = 64 * 1024 * 1024
 
 
 def _peaks():
@@ -56,7 +55,7 @@ def _peaks():
     if os.path.exists(p):
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "measured"
-    return 6650.0, "fallback"
+    return 3350.0, "H100 SXM data sheet (not reached)"
 
 
 def host_threads():
@@ -198,12 +197,6 @@ class CpuArm:
         return n_env * n_steps / dt, dt
 
 
-# measured in the build container with tools/time_reference_on_shim.py (the unmodified reference Python stack stepping on the
-# oracle through oracle/mujoco_shim); /root/reference does not exist on the GPU box, so this row is a recorded number
-REFERENCE_STACK_ROW = {"value": 57.0, "unit": "env-steps/s", "cores": 1, "kind": "reference Python stack on the oracle shim",
-                       "sample": "200 env.step of Lift/Panda OSC_POSE, 1 process, build container (8 cores), recorded - not re-measured here"}
-
-
 def run_reference(args):
     rank = int(os.environ.get("RANK", "0"))
     if rank != 0:
@@ -251,6 +244,24 @@ def device_timeline(part, groups):
         return json.loads(r.stdout.strip().splitlines()[-1])
     except Exception:
         return None
+
+
+def dump_outputs(out_dir, parts, envs):
+    """The arrays the timed path (env_step of every task handle) hands its caller after the last timed step, as
+    <task>_<robot>_<array>.npy in the engine's precision.  Above DUMP_BYTES in all, the same seeded sample of environments is
+    kept for every array (rows in ascending order)."""
+    import numpy as np
+
+    names = ("qpos", "qvel", "qacc", "ctrl", "obs")
+    arrays = {f"{t}_{r}_{nm}": getattr(e.sim, nm) for (t, r, _, _), e in zip(parts, envs) for nm in names}
+    total = sum(a.numel() * a.element_size() for a in arrays.values())
+    os.makedirs(out_dir, exist_ok=True)
+    for key, a in arrays.items():
+        a = a.cpu().numpy()
+        if total > DUMP_BYTES:
+            keep = max(1, len(a) * DUMP_BYTES // total)
+            a = a[np.sort(np.random.default_rng(0).choice(len(a), keep, replace=False))]
+        np.save(os.path.join(out_dir, key + ".npy"), a)
 
 
 def run_gpu(args):
@@ -310,7 +321,7 @@ def run_gpu(args):
     def rand_actions(count):
         return [torch.rand((count, e.num_envs, e.action_dim), generator=gen, device=dev, dtype=dtype) * 2 - 1 for e in envs]
 
-    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device=dev)  # 5x the 50 MB L2 of an H100
 
     def barrier():
         if world > 1:
@@ -346,6 +357,8 @@ def run_gpu(args):
         ev[i][1].record()
     barrier()
     t_wall1 = time.time()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, parts, envs)
     launches = sum(e.sim.launch_count for e in envs) - l0
     ms = sum(a.elapsed_time(b) for a, b in ev)
     t = torch.tensor([ms], dtype=torch.float64, device=dev)
@@ -453,32 +466,9 @@ def run_gpu(args):
         alg_bytes = envs_per_launch * (sub_in + sub_out)
         if tl:
             launch_us, launch_src = tl["kernels"]["tail"]["mean_us"], "%globaltimer stamps of the graph replay (-DB2S_INSTR build, child process)"
-        else:
-            launch_us, launch_src = 0.62 * (ms / K * 1e3) / N_SUBSTEPS / max(1, groups // 2), "estimate: tail share 0.62 of the step (profiles/), 2 groups resident"
+        else:  # no per-kernel timeline: report the whole step
+            kernel, envs_per_launch, alg_bytes = "step_kernel", env0.num_envs, step_bytes
     achieved = alg_bytes / (launch_us * 1e-6) / 1e9
-    traffic = None
-    tp = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(tp):
-        try:
-            with open(tp) as f:
-                traffic = json.load(f).get("dram_bytes_per_launch")
-        except Exception:
-            traffic = None
-    # ---- compute side (SURVEY.md section 8d "report both fractions"): issue slots and useful FP32 work
-    compute = None
-    if os.path.exists(INST_COUNTS):
-        try:
-            with open(INST_COUNTS) as f:
-                ic = json.load(f).get(parts[0][0] + "_" + parts[0][1])
-            sm_mhz = (clk or {}).get("sm_mhz") or 1965.0
-            issue_peak = 148 * 4 * sm_mhz * 1e6                  # warp instructions / s (4 schedulers per SM)
-            fp32_peak = 148 * 128 * 2 * sm_mhz * 1e6             # FLOP/s, non-tensor FP32 (128 FMA lanes per SM)
-            substeps_s = value / world * N_SUBSTEPS * (parts[0][3] / N)
-            compute = {"warp_inst_per_env_substep": ic["warp_inst_per_env_substep"], "issue_slots_frac": ic["warp_inst_per_env_substep"] * substeps_s / issue_peak,
-                       "useful_flop_per_env_step": ic["useful_flop_per_env_step"], "fp32_frac": ic["useful_flop_per_env_step"] * (value / world) / fp32_peak,
-                       "issue_peak_winst_s": issue_peak, "fp32_peak_flops": fp32_peak, "source": ic.get("source")}
-        except Exception:
-            compute = None
     # ---- CPU baseline on a bounded sample (rank 0, N=1 only)
     cpu = None
     if world == 1 and not args.no_cpu_baseline:
@@ -489,8 +479,7 @@ def run_gpu(args):
         cpu = {"value": r, "unit": "env-steps/s", "cores": cores, "kind": "port",
                "sample": f"{arm.n_env} envs x {n_steps} control steps ({dtc:.1f}s) after {args.preroll} untimed pre-roll steps "
                          f"({arm.preroll_s:.1f}s), oracle port (fp64 C) incl. controller, {cores} threads "
-                         f"(affinity {len(os.sched_getaffinity(0))}, cgroup quota {quota})",
-               "reference_python_stack": REFERENCE_STACK_ROW}
+                         f"(affinity {len(os.sched_getaffinity(0))}, cgroup quota {quota})"}
     out = {
         "metric": cfg["metric"], "value": value, "unit": "env-steps/s", "n_gpus": world, "steps": K, "warmup": W,
         "ms_per_step": ms / K, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
@@ -504,16 +493,15 @@ def run_gpu(args):
                           f"before every step (inside the timed region)",
                    "multi_gpu": "env shards independent; NCCL: model broadcast at start" + (", obs all-gather per step (e2e loop)" if args.allgather_obs else "")},
         "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic, "peak_source": how, "kernel": kernel, "launch_us": launch_us, "launch_us_source": launch_src,
+                     "peak_source": how, "kernel": kernel, "launch_us": launch_us, "launch_us_source": launch_src,
                      "envs_per_launch": envs_per_launch, "alg_bytes_per_launch": alg_bytes,
                      "whole_step": {"achieved": achieved_step, "frac": achieved_step / peak, "alg_bytes": step_bytes},
-                     "compute": compute,
                      "timeline": ({"kernels_us": {k: v["mean_us"] for k, v in tl["kernels"].items()}, "gaps_us": tl["gaps_us"],
                                    "phase_kernels_running_hist": tl["phase_kernels_running_hist"],
                                    "solver_mean_niter": tl["solver"]["mean_niter"], "ls_evals_per_solve": tl["solver"]["ls_evals_per_solve"]}
                                   if tl else None),
                      "note": "per-environment state stays in shared memory / L2 between phases: algorithmic HBM traffic is tiny, "
-                             "the kernels are latency / issue bound (DESIGN.md section 5): see `compute`"},
+                             "the kernels are latency / issue bound (DESIGN.md section 5)"},
         "cpu_baseline": cpu,
         "e2e": {"value": e2e_value, "unit": "env-steps/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
         "gpu_launches": int(launches),
@@ -541,6 +529,7 @@ def main():
     ap.add_argument("--preroll", type=int, default=100, help="untimed control steps before the timed region")
     ap.add_argument("--mode", type=int, default=int(os.environ.get("B2S_BENCH_MODE", "1")), help="0 fused kernel, 1 phase-kernel pipeline, 2 unit queue (persistent kernel)")
     ap.add_argument("--allgather-obs", type=int, default=1, help="N>1: all-gather observations over NCCL every e2e step")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step left to its caller as DIR/<name>.npy")
     args = ap.parse_args()
     if args.warmup < 3 and args.impl != "reference":
         args.warmup = 3

@@ -1,4 +1,4 @@
-/* libb2s - C ABI of the B200-native batched rigid-body engine (one environment per warp, sm_100a).
+/* libb2s - C ABI of the H100-native batched rigid-body engine (one environment per warp, sm_90a).
  *
  * Every entry point replaces one call the reference makes into its third-party engine through
  * `robosuite/utils/binding_utils.py` (the `MjSim` shim, SURVEY.md section 8b "Seam 1"), batched over n_env

@@ -1,4 +1,4 @@
-"""B200-native batched manipulation simulator keeping robosuite's make / reset / step / controller_config surface."""
+"""H100-native batched manipulation simulator keeping robosuite's make / reset / step / controller_config surface."""
 import os as _os
 
 __version__ = "0.2.0"

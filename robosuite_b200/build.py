@@ -1,11 +1,11 @@
-"""In-tree build of libb2s.so (hand-written sm_100a CUDA; no JIT cache, the .so travels with the tree)."""
+"""In-tree build of libb2s.so (hand-written CUDA for H100, sm_90a; no JIT cache, the .so travels with the tree)."""
 import os
 import subprocess
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.path.join(_HERE, "libb2s.so")
 SRC = os.path.join(_HERE, "csrc", "b2s_capi.cu")
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17", "-Xcompiler", "-fPIC",
               "-shared"]
 
 

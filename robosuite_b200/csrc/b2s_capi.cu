@@ -47,6 +47,7 @@ struct ArrayInfo { void* ptr; int dtype; int ndim; int64_t shape[4]; };
 
 struct b2s_sim {
   int n_env = 0, device = 0, precision = B2S_F32;
+  int num_sms = 1;  // streaming multiprocessors of `device` (grid sizes of the claim-based launches)
   cudaStream_t stream = 0;
   std::vector<void*> allocs;
   std::map<std::string, ArrayInfo> arrays;
@@ -609,6 +610,10 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
   if (!getenv("B2S_NO_LMEM_FLAG")) keep_local_memory_pool();
   b2s_sim* s = new b2s_sim();
   s->n_env = n_env; s->device = device; s->precision = precision;
+  if (cudaDeviceGetAttribute(&s->num_sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) {
+    b2s_destroy(s);
+    return fail(B2S_ERR_CUDA, "b2s_create: cannot query the multiprocessor count");
+  }
   Blob b{(const char*)blob_host, nbytes};
   try {
     s->nq = b.scalar_i("nq"); s->nv = b.scalar_i("nv"); s->nu = b.scalar_i("nu"); s->nbody = b.scalar_i("nbody");
@@ -798,12 +803,12 @@ template <typename R> static int enqueue_group(b2s_sim* s, DState<R>& st, int ph
     int e0 = (int)((long long)s->n_env * gi / G), e1 = (int)((long long)s->n_env * (gi + 1) / G);
     Grp g{e0, e1 - e0, gi, 0, s->slot};
     int blocks0 = (g.nenv + s->wpb0 - 1) / s->wpb0, blocks5 = (g.nenv + s->wpb5s - 1) / s->wpb5s;
-    int blocksL = std::min((g.nenv + s->wpb5l - 1) / s->wpb5l, 2 * 148);  // large tier: warps claim overflowed environments
+    int blocksL = std::min((g.nenv + s->wpb5l - 1) / s->wpb5l, 2 * s->num_sms);  // large tier: warps claim overflowed environments
     int nA = g.nenv * st.cl_maxa, nG = g.nenv * st.cl_maxg;
     // convex role: one warp per block, items claimed through a counter.  ~1.6 items per environment are queued per substep (Lift), most of
     // them dismissed in a few microseconds: half a block per environment keeps every slow item on its own warp without flooding the
     // block scheduler with thousands of empty blocks per launch (B2S_CVX_BLOCKS overrides)
-    int cvx_blocks = std::max(148, g.nenv / 2);
+    int cvx_blocks = std::max(s->num_sms, g.nenv / 2);
     if (const char* v = getenv("B2S_CVX_BLOCKS")) { int x = atoi(v); if (x > 0) cvx_blocks = x; }
     const bool ctrl_ext = (phases & PH_CTRL_EXT) != 0;
     // B2S_TIMELINE=1 (with B2S_NO_GRAPH=1): timing events between the launches, per-kernel means on stderr (debug aid)

@@ -521,11 +521,11 @@ template <typename R> DEVN int solve(Eng<R> e, int nefc, int ncon, int& warn) {
     }
     R gnorm = r_sqrt(warp_sum(gn));
     __syncwarp();
-    // fp32: cost differences below the rounding noise of the cost itself carry no information
-    const R noise = sizeof(R) == 4 ? R(16) * Lim<R>::eps() * r_abs(cost) : R(0);
+    // fp32 as fp64: the solve stops on the tolerance alone.  An extra exit at the rounding noise of the cost (16 eps |cost|) ended
+    // stiff multi-contact solves early - a nut squeezed between two fingers then turned by a large angle within one substep
     if (iter > 0) {
       R improvement = scale * (prev_cost - cost);
-      if (improvement < m.tolerance || prev_cost - cost < noise || scale * gnorm < m.tolerance) break;
+      if (improvement < m.tolerance || scale * gnorm < m.tolerance) break;
     } else if (scale * gnorm < m.tolerance) break;
     if (iter == m.iterations) break;
     prev_cost = cost;
@@ -626,7 +626,7 @@ template <typename R> DEVN int solve(Eng<R> e, int nefc, int ncon, int& warn) {
     if (d1 >= 0) break;
     // Newton decrement: -d1(0) = grad^T H^-1 grad.  When half of it is below the stopping tolerance this step is the
     // last one: take it and skip the iteration that would only confirm convergence.
-    bool last = R(0.5) * scale * (-d1) < m.tolerance || R(0.5) * (-d1) < noise;
+    bool last = R(0.5) * scale * (-d1) < m.tolerance;
     R gtol = (sizeof(R) == 4 ? R(1e-3) : R(1e-12)) * r_abs(d1);
     alpha = -d1 / d2;
     B2S_LOOP

@@ -9,17 +9,17 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def _gpu_unavailable():
-    """reason string when `gpu`-marked tests cannot run here, else None.  On a GPU box a missing library is a FAILURE, not a skip
+    """reason string when `gpu`-marked tests cannot run here, else None.  On a machine with a GPU a missing library is a FAILURE, not a skip
     (the product path has no CPU fallback and must fail loudly): only the absence of a CUDA device skips."""
     try:
         import torch
 
         if not torch.cuda.is_available():
-            return "no CUDA device (these tests run on the B200 box: pytest -m gpu)"
+            return "no CUDA device (these tests run on an H100: pytest -m gpu)"
     except Exception as e:  # pragma: no cover
         return "torch unavailable: %r" % (e,)
     return None

@@ -12,7 +12,9 @@ import os
 import numpy as np
 import pytest
 
-from tests.util import ROOT, load
+from tests.util import REFERENCE, ROOT, load
+
+HAVE_REFERENCE = bool(REFERENCE) and os.path.isdir(os.path.join(REFERENCE, "robosuite"))
 
 TASKS = ["Lift", "Door", "NutAssemblyRound", "PickPlace", "Stack"]
 
@@ -100,7 +102,7 @@ def test_env_api_matches_reference_stack(task):
     env.close()
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/robosuite"), reason="needs the reference checkout (build container only)")
+@pytest.mark.skipif(not HAVE_REFERENCE, reason="needs a reference robosuite checkout: set ROBOSUITE_REFERENCE")
 def test_reference_stack_runs_on_the_shim_and_reproduces_the_golden_file():
     """regenerate the first two Lift steps with the unmodified reference stack on oracle/mujoco_shim (subprocess: the shim
     shadows the `mujoco` module name) and compare with the committed vectors"""
@@ -127,7 +129,7 @@ def test_reference_stack_runs_on_the_shim_and_reproduces_the_golden_file():
     assert np.abs(got - ref).max() < 1e-12
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/robosuite"), reason="needs the reference checkout (build container only)")
+@pytest.mark.skipif(not HAVE_REFERENCE, reason="needs a reference robosuite checkout: set ROBOSUITE_REFERENCE")
 def test_reference_datacollection_episode_loads_and_replays_on_the_oracle(tmp_path):
     """an episode folder written by the reference's own DataCollectionWrapper (running on the shim) is read by
     robosuite_b200.state_io; its model.xml compiles, its state rows decode, and replaying the recorded actions from the first

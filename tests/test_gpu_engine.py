@@ -130,7 +130,7 @@ def test_rollout_100_f64():
 def test_rollout_100_f32():
     eq, ev = _rollout("f32", 100)
     print("f32 rollout rel err qpos %.3g qvel %.3g" % (eq, ev))
-    # north_star tolerance: <= 1e-4 relative on qpos / qvel over 100 steps (measured on B200: 3.6e-7 / 8.3e-7)
+    # north_star tolerance: <= 1e-4 relative on qpos / qvel over 100 steps (measured on an H100: 3.6e-7 / 8.3e-7)
     assert eq < 1e-4 and ev < 1e-4
 
 
@@ -202,19 +202,19 @@ def test_env_step_pipeline_f64():
 def test_env_step_pipeline_f32():
     eq, ev, et = _env_rollout("f32", 4, mode=1)
     print("f32 env 4 control steps, pipeline + controller kernel: qpos %.3g qvel %.3g tau %.3g" % (eq, ev, et))
-    assert eq < 1e-4 and ev < 1e-4  # measured on B200: 6.2e-7 / 6.4e-6
+    assert eq < 1e-4 and ev < 1e-4  # measured on an H100: 6.2e-7 / 6.4e-6
 
 
 def test_env_step_f32_100_substeps():
     eq, ev, et = _env_rollout("f32", 4)
     print("f32 env 4 control steps (100 substeps): qpos %.3g qvel %.3g tau %.3g" % (eq, ev, et))
-    assert eq < 1e-4 and ev < 1e-4  # measured on B200: 6.2e-7 / 6.4e-6
+    assert eq < 1e-4 and ev < 1e-4  # measured on an H100: 6.2e-7 / 6.4e-6
 
 
 def test_env_step_f32_100_control_steps():
     """stricter reading of '100 steps': 100 env.step = 2500 physics substeps.  The gate is looser for a PHYSICAL reason: closed-loop
     contact dynamics amplify the fp32-vs-fp64 rounding difference (6e-7 after 100 substeps, 2.3e-4 after 2500: ~x400 over 24x more steps,
-    measured on B200); the fp64 build of the same code stays at 1e-8 over the same rollout."""
+    measured on an H100); the fp64 build of the same code stays at 1e-8 over the same rollout."""
     eq, ev, et = _env_rollout("f32", 100, n=4)
     print("f32 env 100 control steps (2500 substeps): qpos %.3g qvel %.3g tau %.3g" % (eq, ev, et))
     assert eq < 5e-3 and ev < 1e-2

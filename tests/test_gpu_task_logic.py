@@ -75,7 +75,7 @@ def test_scripted_episode_free_run_on_device(key):
     print("%s: fp32 device follows the reference record for %d of %d control steps (grasp steps %d, success steps %d)" % (
         key, n_cmp, n_tot, n_grasp, n_succ))
     # the reach + most of the descent (25 control steps = 625 substeps, arm in free space, objects at rest) must track to 1e-3;
-    # measured on B200: Lift 46, Stack 70, NutAssemblyRound 31 (the fingers reach the nut handle at step 32), PickPlace 10 (four
+    # measured on an H100: Lift 70, Stack 70, NutAssemblyRound 45 (the fingers reach the nut handle around step 32), PickPlace 10 (four
     # loose mesh objects settling in the bin amplify fp32 rounding from the first step: the fp64 oracle itself leaves the
     # reference's record at step 15, tests/test_env_golden.py)
     assert n_cmp >= {"PickPlace": 8}.get(key, 25), (key, n_cmp)
@@ -149,7 +149,7 @@ def test_device_task_outputs_lockstep_with_oracle(key):
     assert warn == 0
     # One fp32 control step (25 substeps) from an identical state.  Typical step: 1e-5 or better (median gate).  Worst step of an
     # episode: while the gripper closes on / drags an object the contact forces are stiff and fp32-vs-fp64 rounding is amplified
-    # within the step - measured on B200: Lift 4.7e-4, Stack 3.2e-4, NutAssemblyRound 5e-3, Door 1.5e-2 (handle slipping in the open
+    # within the step - measured on an H100: Lift 1.6e-5, Stack 7.9e-6, NutAssemblyRound 2.6e-4, Door 1.6e-2 (handle slipping in the open
     # gripper), PickPlace O(1) (the gripper ploughs through four loose mesh objects: one of them takes a different bounce).  The
     # gates on the worst step therefore apply to the two tasks whose scripted episode is a clean grasp; flags are gated everywhere.
     # (Door: the open gripper slides along the handle for most of the episode: median 1e-3, p90 2e-3)

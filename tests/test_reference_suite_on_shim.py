@@ -1,4 +1,4 @@
-"""CPU, build container only: the REFERENCE'S OWN test functions (unmodified files under /root/reference/tests, unmodified reference package) run
+"""CPU, with a reference checkout in ROBOSUITE_REFERENCE only: the REFERENCE'S OWN test functions (unmodified files under its tests/, unmodified reference package) run
 on the CPU oracle through oracle/mujoco_shim (tools/run_reference_tests_on_shim.py).  They are behavioural pins of the oracle's PHYSICS by
 the reference's own acceptance criteria: bit-identical open-loop playback (test_action_playback.py), the gripper testers that must
 close on a cube and lift it (test_panda_gripper.py, test_rethink_gripper.py, test_robotiq_*.py, test_jaco_threefinger.py,
@@ -12,9 +12,10 @@ import sys
 
 import pytest
 
-from tests.util import ROOT
+from tests.util import REFERENCE, ROOT
 
-pytestmark = pytest.mark.skipif(not os.path.isdir("/root/reference/tests"), reason="needs /root/reference (build container)")
+pytestmark = pytest.mark.skipif(not REFERENCE or not os.path.isdir(os.path.join(REFERENCE, "tests")),
+                                reason="needs a reference robosuite checkout: set ROBOSUITE_REFERENCE")
 
 
 def _run(names, timeout):

@@ -79,7 +79,7 @@ def test_taking_only_produced_tickets_always_terminates(n_env, n_blocks, wpb):
 
 def test_eager_ticket_taking_terminates_in_the_model_too():
     """the first lockstep version took `wpb` tickets whether produced or not and waited for them in front of the first stage barrier.  On
-    the GPU it stalled until the watchdog in every control step (profiles/r02_summary.md E); in THIS model it terminates, i.e. the stall was
+    the GPU it stalled until the watchdog in every control step; in THIS model it terminates, i.e. the stall was
     not a property of the ticket arithmetic - the shipped kernel removes the wait altogether instead of relying on it"""
     for seed in range(3):
         done, dead, executed = simulate(64, 25, 8, 8, "eager", seed)

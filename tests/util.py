@@ -4,6 +4,8 @@ import os
 import numpy as np
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+# source checkout of the reference robosuite (v1.5.2): the tests that run the reference's own code skip without it
+REFERENCE = os.environ.get("ROBOSUITE_REFERENCE", "")
 PANDA_INIT = np.array([0, np.pi / 16.0, 0.00, -np.pi / 2.0 - np.pi / 3.0, 0.00, np.pi - 0.2, np.pi / 4])
 
 

@@ -32,7 +32,7 @@ TASKS = ["Lift_Panda", "Lift_Sawyer", "Stack_Panda", "Door_Panda", "PickPlace_Pa
 
 
 def load_mjcf(task, assets):
-    """fixture MJCF with the asset prefix of the build container replaced and every texture / textured material attribute removed"""
+    """fixture MJCF with the recorded asset prefix replaced and every texture / textured material attribute removed"""
     xml = open(os.path.join(ROOT, "tests", "golden", "mjcf", task + ".xml")).read()
     xml = re.sub(r"<texture\b[^>]*/>", "", xml)
     xml = re.sub(r'\stexture="[^"]*"', "", xml)

@@ -1,10 +1,10 @@
 """Golden vectors for the environment layer from the REFERENCE'S OWN Python code.
 
-Runs the unmodified robosuite stack (/root/reference) on the CPU oracle through oracle/mujoco_shim (a `mujoco`
+Runs the unmodified robosuite stack (checkout in ROBOSUITE_REFERENCE) on the CPU oracle through oracle/mujoco_shim (a `mujoco`
 look-alike) and records, per task: the composed model's reset state, the action sequence, and after every control step
 the reference's flat observation (`object-state`, `robot0_proprio-state`), reward, and qpos.  tests/test_gpu_env.py replays
 the same states and actions through robosuite_b200 and compares observation layout / values and rewards with what the
-reference code produced.  Runs only in the build container (needs /root/reference); output: tests/golden/env_golden.npz
+reference code produced.  Needs that checkout; output: tests/golden/env_golden.npz
 
 Usage: python tools/gen_env_golden.py
 """
@@ -14,7 +14,7 @@ from unittest.mock import MagicMock
 import numpy as np
 
 ROOT = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..")
-REF = "/root/reference"
+REF = os.environ.get("ROBOSUITE_REFERENCE", "")  # source checkout of the reference robosuite
 
 
 def install():

@@ -5,7 +5,7 @@ import os, re, subprocess, sys, tempfile
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 ptx = os.path.join(tempfile.mkdtemp(), "b2s.ptx")
-subprocess.check_call(["nvcc", "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-std=c++17", "-ptx", "-o", ptx,
+subprocess.check_call(["nvcc", "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-std=c++17", "-ptx", "-o", ptx,
                        os.path.join(ROOT, "robosuite_b200", "csrc", "b2s_capi.cu")])
 txt = open(ptx).read()
 funcs = re.split(r"\n(?=\.(?:visible |weak )?(?:func|entry))", txt)

@@ -1,5 +1,5 @@
-"""Run the REFERENCE'S OWN test functions (unmodified files under /root/reference/tests) with the unmodified reference package on the
-CPU oracle through oracle/mujoco_shim.  Build container only.  usage: python tools/run_reference_tests_on_shim.py [name ...]"""
+"""Run the REFERENCE'S OWN test functions (unmodified files under $ROBOSUITE_REFERENCE/tests) with the unmodified reference package on the
+CPU oracle through oracle/mujoco_shim.  usage: python tools/run_reference_tests_on_shim.py [name ...]"""
 import importlib.util
 import os
 import sys
@@ -10,7 +10,7 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import gen_env_golden as g  # noqa: E402
 
 g.install()
-REF = "/root/reference/tests"
+REF = os.path.join(os.environ.get("ROBOSUITE_REFERENCE", ""), "tests")
 TESTS = {
     "playback": ("test_environments/test_action_playback.py", "test_playback"),
     "panda_gripper": ("test_grippers/test_panda_gripper.py", "test_panda_gripper"),
