@@ -1071,9 +1071,7 @@ template <typename R> static int launch_unit_t(b2s_sim* s, DState<R>& st, int ph
   int rc = bind_constants(s);
   if (rc != B2S_OK) return rc;
   if (getenv("B2S_UNIT_PROF") && !s->uq_prof) s->uq_prof = dev_zeros<unsigned long long>(s, 16);
-  int ubar = 4;
-  if (const char* v = getenv("B2S_UNIT_BARRIERS")) ubar = atoi(v);
-  UnitQ q{s->uq_ring, s->uq_ovf, s->uq_ctr, total, s->uq_nlarge, s->uq_wpb_large, s->uq_stride, s->uq_stride_large, s->uq_prof, ubar};
+  UnitQ q{s->uq_ring, s->uq_ovf, s->uq_ctr, total, s->uq_nlarge, s->uq_wpb_large, s->uq_stride, s->uq_stride_large, s->uq_prof};
   unit_init_kernel<R><<<(total + 255) / 256, 256, 0, s->stream>>>(q, s->n_env);
   unit_kernel<R><<<s->uq_grid, s->uq_wpb * 32, s->uq_smem, s->stream>>>(phases, nsub, action, s->slot, q);
   unit_check_kernel<R><<<8, 256, 0, s->stream>>>(q, s->slot);

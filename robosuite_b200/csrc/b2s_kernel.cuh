@@ -11,6 +11,9 @@ template <typename R> DEV void load_row(R* dst, const R* src, int n, int lane) {
   for (int i = lane; i < n; i += 32) dst[i] = src[i];
 }
 
+// end of an environment's substep(s): state rows, time and warn bits -> global memory (b2s_pipeline.cuh, with the other shared stages)
+template <typename R> DEV void store_state(const Eng<R>& e, int env, R time, int warn);
+
 template <typename R>
 DEVN void export_step1(const Eng<R> e, int env, int ncon) {
   const DModel<R>& m = e.model();
@@ -185,19 +188,11 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
     s.dbg[E * 4] = dbgc[0]; s.dbg[E * 4 + 1] = dbgc[1]; s.dbg[E * 4 + 2] = dbgc[2];
   }
   if (!live) return;
-  // write back
-  for (int i = lane; i < m.nq; i += 32) s.qpos[E * m.nq + i] = e.p(L.qpos)[i];
-  for (int i = lane; i < m.nv; i += 32) {
-    s.qvel[E * m.nv + i] = e.p(L.qvel)[i];
-    s.qacc[E * m.nv + i] = e.p(L.qacc)[i];
-    s.qacc_ws[E * m.nv + i] = e.p(L.qacc_ws)[i];
-  }
   if (phases & PH_CTRL) {
     for (int i = lane; i < m.nu; i += 32) s.ctrl[E * m.nu + i] = e.p(L.ctrl)[i];
     ctrl_store(e, cs, env);
   }
-  warn = warp_or_i(warn);  // some flags (a dropped contact's rows) are raised on the lane that owns the item
-  if (lane == 0) { s.time[env] = time; s.warn[env] |= warn; }
+  store_state(e, env, time, warn);
 }
 
 // masked episode reset without a host round trip: selected environments take their generalized positions from `qpos_new` (a pool of

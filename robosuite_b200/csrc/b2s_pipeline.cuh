@@ -1,6 +1,7 @@
 // Pipeline mode: one substep = phase 0 (kinematics + dynamics + broad phase) | work-list narrow phase (analytic, convex) beside the
 // thread-per-environment controller kernel | tail (contact gather, constraint rows, solve, integrate, observations), exchanging a
-// per-environment workspace row through L2.  Same device functions as the fused kernel; what changes is scheduling and MEMORY:
+// per-environment workspace row through L2.  Same device functions as the fused kernel, and the stage sequences (phase 0, one narrow-
+// phase pair, the tail stages) are defined here once for this pipeline and the unit queue; what changes is scheduling and MEMORY:
 // every kernel has its own compact shared-memory layout (LAY_P0 / LAY_TS / LAY_TL), so 24-28 warps are resident per SM instead of
 // the 14 the one-size-fits-all layout allowed, and the tail kernel runs in two capacity tiers: the small tier holds the contact /
 // row counts almost every environment has, the few that need more are re-run by the large tier (same results, no truncation).
@@ -120,17 +121,11 @@ DEV unsigned long long gtimer() { unsigned long long t; asm volatile("mov.u64 %0
 // the role with the longest single work item (a deep EPA) is scheduled first.  Every block is one warp.
 struct P1Cfg { int nG, nC, sub; };
 
-// analytic pairs: ONE THREAD per candidate pair of any environment (32 different pairs per warp)
-template <typename R> DEV void narrow_analytic_block(const Grp& g, int rb) {
-  const DModel<R>& m = cmodel<R>(g.slot);
-  const DState<R>& s = cstate<R>(g.slot);
-  const WSLayout& RL = c_lay[g.slot][LAY_ROW];
-  int tid = rb * 32 + threadIdx.x;
-  if (tid >= CLC(s, g)[0]) return;
-  tid += g.env0 * s.cl_maxa;  // this group's slice of the candidate list / output slots
-  int code = s.cl_listA[tid];
-  int env = code >> 12, pidx = code & 4095;
-  const R* row = s.wsg + (size_t)env * RL.total;
+// ---- one narrow-phase pair of an environment, for the phase-1 roles and the unit queue alike: geoms in type order (what the fused
+// collide produces), shapes from the environment's workspace row, contact count + records -> the output record `out`
+template <typename R> DEV void narrow_pair_analytic(int slot, const R* row, int pidx, R* out) {
+  const DModel<R>& m = cmodel<R>(slot);
+  const WSLayout& RL = c_lay[slot][LAY_ROW];
   int g1 = m.pair_geom[2 * pidx], g2 = m.pair_geom[2 * pidx + 1];
   if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
   Shape<R> A, B;
@@ -138,9 +133,63 @@ template <typename R> DEV void narrow_analytic_block(const Grp& g, int rb) {
   shape_from(m, g2, row + RL.gpos, row + RL.gmat, B);
   R buf[8 * CREC];
   int n = narrow_analytic(A, B, buf);
-  R* out = s.cl_outA + (size_t)tid * CL_RECA;
   out[0] = R(n);
   for (int k = 0; k < n * CREC; k++) out[1 + k] = buf[k];
+}
+
+// the whole warp on one convex pair: `scratch` holds the EPA polytope, `stage` (stage_cap words, or nullptr) the staged hull vertices.
+// item_stats: -DB2S_INSTR per-item cost histogram and slow-item log (the phase-1 convex role)
+template <typename R>
+DEV void narrow_pair_convex(int slot, int env, const R* row, int pidx, R* out, R* scratch, R* stage, int stage_cap, int lane, bool item_stats) {
+  const DModel<R>& m = cmodel<R>(slot);
+  const DState<R>& s = cstate<R>(slot);
+  const WSLayout& RL = c_lay[slot][LAY_ROW];
+  int g1 = m.pair_geom[2 * pidx], g2 = m.pair_geom[2 * pidx + 1];
+  if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
+  Shape<R> A, B;
+  shape_from(m, g1, row + RL.gpos, row + RL.gmat, A);
+  shape_from(m, g2, row + RL.gpos, row + RL.gmat, B);
+  R buf[CREC];
+#ifdef B2S_INSTR
+  long long it0 = clock64();
+#endif
+  int n = convex_convex(A, B, buf, 1, scratch, lane, s.gjk_cache ? s.gjk_cache + ((size_t)env * m.npair + pidx) * 3 : (R*)nullptr,
+                        EPA_PIPE_MAXV, EPA_PIPE_MAXF, stage, stage_cap);
+#ifdef B2S_INSTR
+  if (item_stats && lane == 0 && s.stats) {  // bucket k = cycles in [2^(k+8), 2^(k+9)), by shape types (mesh-mesh / other)
+    long long dt = clock64() - it0;
+    int k = 0;
+    while (k < 11 && (dt >> (k + 9)) > 0) k++;
+    atomicAdd(s.stats + 500 - 12 * ((A.type == G_MESH && B.type == G_MESH) ? 2 : 1) + k, 1);
+    if (n > 0) atomicAdd(s.stats + 18, 1);
+    if (dt > (1 << 19) && s.slowlog) {  // items above 524 k cycles (~270 us): what are they?
+      int j = atomicAdd(s.stats + 20, 1);
+      if (j < 64) {
+        const int* sp = reinterpret_cast<const int*>(scratch + 9 * EPA_PIPE_MAXV + 4 * EPA_PIPE_MAXF) + EPA_PIPE_MAXF + 64;
+        int* o = s.slowlog + 12 * j;
+        o[0] = (int)dt; o[1] = A.type; o[2] = B.type; o[3] = A.nvert; o[4] = B.nvert; o[5] = sp[0]; o[6] = sp[1]; o[7] = sp[2]; o[8] = sp[3];
+        o[9] = sp[4]; o[10] = g1; o[11] = g2;
+      }
+    }
+  }
+#endif
+  if (lane == 0) {
+    out[0] = R(n);
+    for (int k = 0; k < CREC; k++) out[1 + k] = n ? buf[k] : R(0);
+  }
+  __syncwarp();
+}
+
+// analytic pairs: ONE THREAD per candidate pair of any environment (32 different pairs per warp)
+template <typename R> DEV void narrow_analytic_block(const Grp& g, int rb) {
+  const DState<R>& s = cstate<R>(g.slot);
+  const WSLayout& RL = c_lay[g.slot][LAY_ROW];
+  int tid = rb * 32 + threadIdx.x;
+  if (tid >= CLC(s, g)[0]) return;
+  tid += g.env0 * s.cl_maxa;  // this group's slice of the candidate list / output slots
+  int code = s.cl_listA[tid];
+  int env = code >> 12;
+  narrow_pair_analytic(g.slot, s.wsg + (size_t)env * RL.total, code & 4095, s.cl_outA + (size_t)tid * CL_RECA);
 }
 
 // convex pairs: ONE WARP per candidate pair (mesh support scans split over the lanes).  The block owns one EPA polytope and the
@@ -160,43 +209,9 @@ template <typename R> DEV void narrow_convex_block(const Grp& g, unsigned char* 
     if (item >= cnt) break;
     int wid = item + g.env0 * s.cl_maxg;
     int code = s.cl_listG[wid];
-    int env = code >> 12, pidx = code & 4095;
-    const R* row = s.wsg + (size_t)env * RL.total;
-    int g1 = m.pair_geom[2 * pidx], g2 = m.pair_geom[2 * pidx + 1];
-    if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
-    Shape<R> A, B;
-    shape_from(m, g1, row + RL.gpos, row + RL.gmat, A);
-    shape_from(m, g2, row + RL.gpos, row + RL.gmat, B);
-    R buf[CREC];
-#ifdef B2S_INSTR
-    long long it0 = clock64();
-#endif
-    int n = convex_convex(A, B, buf, 1, scratch, lane, s.gjk_cache ? s.gjk_cache + ((size_t)env * m.npair + pidx) * 3 : (R*)nullptr,
-                          EPA_PIPE_MAXV, EPA_PIPE_MAXF, m.stage_cap > 0 ? scratch + EPA_PIPE_WORDS : (R*)nullptr, m.stage_cap);
-#ifdef B2S_INSTR
-    if (lane == 0 && s.stats) {  // per-item cost histogram: bucket k = cycles in [2^(k+8), 2^(k+9)), by shape types (mesh-mesh / other)
-      long long dt = clock64() - it0;
-      int k = 0;
-      while (k < 11 && (dt >> (k + 9)) > 0) k++;
-      atomicAdd(s.stats + 500 - 12 * ((A.type == G_MESH && B.type == G_MESH) ? 2 : 1) + k, 1);
-      if (n > 0) atomicAdd(s.stats + 18, 1);
-      if (dt > (1 << 19) && s.slowlog) {  // items above 524 k cycles (~270 us): what are they?
-        int slot = atomicAdd(s.stats + 20, 1);
-        if (slot < 64) {
-          const int* sp = reinterpret_cast<const int*>(scratch + 9 * EPA_PIPE_MAXV + 4 * EPA_PIPE_MAXF) + EPA_PIPE_MAXF + 64;
-          int* o = s.slowlog + 12 * slot;
-          o[0] = (int)dt; o[1] = A.type; o[2] = B.type; o[3] = A.nvert; o[4] = B.nvert; o[5] = sp[0]; o[6] = sp[1]; o[7] = sp[2]; o[8] = sp[3];
-          o[9] = sp[4]; o[10] = g1; o[11] = g2;
-        }
-      }
-    }
-#endif
-    R* out = s.cl_outG + (size_t)wid * 8;
-    if (lane == 0) {
-      out[0] = R(n);
-      for (int k = 0; k < CREC; k++) out[1 + k] = n ? buf[k] : R(0);
-    }
-    __syncwarp();
+    int env = code >> 12;
+    narrow_pair_convex(g.slot, env, s.wsg + (size_t)env * RL.total, code & 4095, s.cl_outG + (size_t)wid * 8, scratch,
+                       m.stage_cap > 0 ? scratch + EPA_PIPE_WORDS : (R*)nullptr, m.stage_cap, lane, true);
   }
 }
 
@@ -283,45 +298,18 @@ template <typename R> DEVN int gather_contacts(Eng<R> e, int env, int& warn) {
   return total;
 }
 
-// Launch bounds (threads per block, resident blocks per SM the register allocation is sized for).  (256, 2) = 128 registers per
-// thread: with (256, 3) = 80 registers the heavily spilling build mis-executed solve() on 21-dof models (a corrupted workspace
-// pointer; compute-sanitizer: tools/run8.sh) - the same family of nvcc 12.9 stack-slot problems as DESIGN.md section 3 records.
-// The kernels are latency bound at 4096 environments (every environment's warp is resident either way), so the lost occupancy
-// costs nothing measurable (lb256x2 was the fastest variant of tools/run7.sh).
-#ifndef B2S_LB0_THREADS
-#define B2S_LB0_THREADS 256  // phase 0
-#define B2S_LB0_BLOCKS 2
-#endif
-#ifndef B2S_LB5_THREADS
-#define B2S_LB5_THREADS 256  // tail kernel
-#define B2S_LB5_BLOCKS 2
-#endif
+// ---- the stages of one environment-substep.  The phase kernels and the unit queue both run these; they differ only in how they hand
+// environments to warps.  Each stage is inlined into its caller (the inline boundaries decide register allocation and FMA contraction).
 
-// ---- phase 0: kinematics, velocity stage + RNE bias, CRB -> M, broad phase -> global candidate work lists
-template <typename R>
-__global__ void __launch_bounds__(B2S_LB0_THREADS, B2S_LB0_BLOCKS) phase0_kernel(int phases, Grp g) {
-  const DModel<R>& m = cmodel<R>(g.slot);
-  const DState<R>& s = cstate<R>(g.slot);
-  const WSLayout& L = c_lay[g.slot][LAY_P0];
-  const WSLayout& RL = c_lay[g.slot][LAY_ROW];
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  R* smem = reinterpret_cast<R*>(smem_raw);
-  int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
-  int env = blockIdx.x * wpb + warp;
-  INSTR_BEGIN(s, g, 0)
-#ifdef B2S_INSTR
-  long long instr_t0 = clock64();
-#endif
-  if (env >= g.nenv) return;
-  env += g.env0;
-  Eng<R> e(smem + (size_t)warp * L.total, lane, g.slot, LAY_P0);
+// phase 0 up to the broad phase: state rows in, kinematics, velocity stage + RNE bias, CRB -> M, collision candidates (in the
+// layout's scratch: analytic, then convex at +96) clamped to the candidate-list capacities.  Returns the warn bits.
+template <typename R> DEV int phase0_env(Eng<R>& e, int env, int& na, int& ng) {
+  const DModel<R>& m = e.model();
+  const DState<R>& s = e.state();
+  const WSLayout& L = e.lay();
+  const int lane = e.lane;
+  const size_t E = env;
   e.env = env;
-#ifdef B2S_ZERO_SMEM
-  for (int i = lane; i < L.total; i += 32) e.ws[i] = 0;
-  __syncwarp();
-#endif
-  size_t E = env;
-  R* row = s.wsg + E * RL.total;
   load_row(e.p(L.qpos), s.qpos + E * m.nq, m.nq, lane);
   load_row(e.p(L.qvel), s.qvel + E * m.nv, m.nv, lane);
   __syncwarp();
@@ -334,13 +322,173 @@ __global__ void __launch_bounds__(B2S_LB0_THREADS, B2S_LB0_BLOCKS) phase0_kernel
   }
   e.velocity();
   e.crb();
-  // collision candidates of this environment -> global work lists (slots by warp-aggregated atomics)
-  int* cand = reinterpret_cast<int*>(e.p(L.scratch));
-  int* cand_g = cand + 96;
-  int na, ng, warn = was_reset;
-  cull_pairs(e, cand, cand_g, s.cl_maxa, s.cl_maxg, na, ng);
+  int* cand = e.pi(L.scratch);
+  int warn = was_reset;
+  cull_pairs(e, cand, cand + 96, s.cl_maxa, s.cl_maxg, na, ng);
   if (na > s.cl_maxa) { na = s.cl_maxa; warn |= 4; }
   if (ng > s.cl_maxg) { ng = s.cl_maxg; warn |= 4; }
+  return warn;
+}
+
+// end of phase 0: the environment's candidate table (pair index and output slot: analytic candidate i -> baseA + i, convex i -> baseG + i),
+// the warn word of the row header, phase 0's workspace regions -> the row.  worklist: the candidates also go to the group's work lists.
+template <typename R> DEV void phase0_publish(const Eng<R>& e, int env, int na, int ng, int warn, int baseA, int baseG, bool worklist) {
+  const DState<R>& s = e.state();
+  const WSLayout& L = e.lay();
+  const WSLayout& RL = c_lay[e.slot][LAY_ROW];
+  const int lane = e.lane;
+  const size_t E = env;
+  const int* cand = e.pi(L.scratch);
+  const int* cand_g = cand + 96;
+  int* tab = s.cl_env + E * CL_ENVW(s);
+  if (lane == 0) { tab[0] = na; tab[1] = ng; }
+  for (int i = lane; i < na; i += 32) {
+    if (worklist) s.cl_listA[baseA + i] = (env << 12) | cand[i];
+    tab[2 + 2 * i] = cand[i]; tab[3 + 2 * i] = baseA + i;
+  }
+  for (int i = lane; i < ng; i += 32) {
+    if (worklist) s.cl_listG[baseG + i] = (env << 12) | cand_g[i];
+    tab[2 + 2 * (s.cl_maxa + i)] = cand_g[i]; tab[3 + 2 * (s.cl_maxa + i)] = baseG + i;
+  }
+  R* row = s.wsg + E * RL.total;
+  if (lane == 0) reinterpret_cast<int*>(row + RL.hdr)[2] = warn;
+  __syncwarp();
+  ws_store(e, row, c_pio[e.slot][PIO_P0]);
+}
+
+// The tail stages take the engine of the tier's layout (LAY_TS / LAY_TL).
+// Rows: workspace regions and state rows in, contacts gathered from the narrow-phase outputs, constraint rows, and whether the
+// environment fits this tier (if not, nothing of its state has been touched).  Returns the packed word below; nefc <= the layout's row
+// capacity, far below 2^14 in any layout that fits shared memory.
+#define TAIL_NCON(pk) ((pk) & 255)
+#define TAIL_WARN(pk) (((pk) >> 8) & 255)
+#define TAIL_NEFC(pk) (((pk) >> 16) & 0x3fff)
+#define TAIL_OVF(pk) ((pk) >> 30)
+template <typename R> DEV int tail_rows(Eng<R>& e, int env, unsigned long long* bar, unsigned& parity) {
+  const DModel<R>& m = e.model();
+  const DState<R>& s = e.state();
+  const WSLayout& L = e.lay();
+  const WSLayout& RL = c_lay[e.slot][LAY_ROW];
+  const int lane = e.lane;
+  const bool tiered = L.mc < m.maxcon || L.me < m.maxefc;
+  const size_t E = env;
+  const R* row = s.wsg + E * RL.total;
+  const int warn = reinterpret_cast<const int*>(row + RL.hdr)[2];  // phase 0: divergence reset, candidate-list overflow
+  ws_load(e, row, c_pio[e.slot][e.lid == LAY_TL ? PIO_TL : PIO_TS], bar, parity);
+  load_row(e.p(L.qpos), s.qpos + E * m.nq, m.nq, lane);
+  load_row(e.p(L.qvel), s.qvel + E * m.nv, m.nv, lane);
+  load_row(e.p(L.ctrl), s.ctrl + E * m.nu, m.nu, lane);
+  load_row(e.p(L.qacc_ws), s.qacc_ws + E * m.nv, m.nv, lane);
+  __syncwarp();
+  int wl = 0;
+  const int ncon = gather_contacts(e, env, wl);
+  const int nefc = (tiered && (wl & 4)) ? 0 : make_constraint(e, ncon, wl);
+  wl = warp_or_i(wl);  // make_constraint flags a dropped contact on the lane that owns it: the verdict must be warp-uniform
+  const int ovf = (tiered && (wl & 12)) ? 1 : 0;
+  return (ncon & 255) | (((warn | wl) & 255) << 8) | ((nefc & 0x3fff) << 16) | (ovf << 30);
+}
+
+// Controller run inside the tail (JV / joint controllers; OSC when it is not a phase-1 role): ctrl -> global memory
+template <typename R> DEV void tail_ctrl(Eng<R>& e, int env, int sub, const R* action) {
+  const DModel<R>& m = e.model();
+  const DState<R>& s = e.state();
+  const WSLayout& L = e.lay();
+  const size_t E = env;
+  CtrlState<R> cs;
+  ctrl_load(e, cs, env);
+  ctrl_run(e, cs, env, sub == 0 ? action : (const R*)nullptr);
+  for (int i = e.lane; i < m.nu; i += 32) s.ctrl[E * m.nu + i] = e.p(L.ctrl)[i];
+  if (sub == 0) ctrl_store(e, cs, env);
+  __syncwarp();
+}
+
+// Dynamics, in two parts (the unit queue puts a block barrier between them): actuation + smooth acceleration, then the Newton solve.
+// Both return warn bits.
+template <typename R> DEV int tail_accel(Eng<R>& e) {
+  e.actuation((R*)nullptr);
+  return e.acceleration() ? 1 : 0;
+}
+template <typename R> DEV int tail_newton(Eng<R>& e, int nefc, int ncon) {
+  int warn = 0;
+  solve(e, nefc, ncon, warn);
+  return warn;
+}
+
+// Write-back, also the end of the fused step_kernel: state rows, time and the warn bits of the whole warp -> global memory
+template <typename R> DEV void store_state(const Eng<R>& e, int env, R time, int warn) {
+  const DModel<R>& m = e.model();
+  const DState<R>& s = e.state();
+  const WSLayout& L = e.lay();
+  const int lane = e.lane;
+  const size_t E = env;
+  for (int i = lane; i < m.nq; i += 32) s.qpos[E * m.nq + i] = e.p(L.qpos)[i];
+  for (int i = lane; i < m.nv; i += 32) {
+    s.qvel[E * m.nv + i] = e.p(L.qvel)[i];
+    s.qacc[E * m.nv + i] = e.p(L.qacc)[i];
+    s.qacc_ws[E * m.nv + i] = e.p(L.qacc_ws)[i];
+  }
+  warn = warp_or_i(warn);  // some flags (a dropped contact's rows) are raised on the lane that owns the item
+  if (lane == 0) { s.time[env] = time; s.warn[env] |= warn; }
+  __syncwarp();
+}
+
+// Finish: Euler, on the last substep of a control step the observation and task rows, state write-back.
+template <typename R>
+DEV void tail_finish(Eng<R>& e, int env, int sub, int nsub, int phases, int ncon, int warn, unsigned long long* bar, unsigned& parity) {
+  const DState<R>& s = e.state();
+  R time = s.time[env];
+  if (!(phases & PH_NOINTEGRATE)) {
+    { int eb = e.euler(&time); if (eb & 32) warn |= 32; else if (eb) warn |= 2; }
+  }
+  if ((phases & PH_OBS) && e.ccfg().obs_dim > 0 && sub == nsub - 1) {
+    // The reference's observables sample on the LAST substep of a control step: reset()'s forced update already
+    // advances their period timer by one model timestep (utils/observables.py:214-259, environments/base.py:418-427),
+    // so the period closes after substep 24 and the next update - substep 25 - takes the sample.
+    // Body / site poses of this substep's step1 arrive now, over the (dead) constraint Jacobian.
+    ws_load(e, s.wsg + (size_t)env * c_lay[e.slot][LAY_ROW].total, c_pio[e.slot][e.lid == LAY_TL ? PIO_TL_LATE : PIO_TS_LATE], bar, parity);
+    write_obs(e, env, (phases & PH_NOINTEGRATE) != 0);
+    write_task(e, env, ncon);
+  }
+  store_state(e, env, time, warn);
+}
+
+// Launch bounds (threads per block, resident blocks per SM the register allocation is sized for).  (256, 2) = 128 registers per
+// thread: with (256, 3) = 80 registers the heavily spilling build mis-executed solve() on 21-dof models (a corrupted workspace
+// pointer, found with compute-sanitizer) - the same family of nvcc 12.9 stack-slot problems as DESIGN.md section 3 records.
+// The kernels are latency bound at 4096 environments (every environment's warp is resident either way), so the lost occupancy
+// costs nothing measurable (256 x 2 was the fastest of the launch-bound variants measured).
+#ifndef B2S_LB0_THREADS
+#define B2S_LB0_THREADS 256  // phase 0
+#define B2S_LB0_BLOCKS 2
+#endif
+#ifndef B2S_LB5_THREADS
+#define B2S_LB5_THREADS 256  // tail kernel
+#define B2S_LB5_BLOCKS 2
+#endif
+
+// ---- phase 0: kinematics, velocity stage + RNE bias, CRB -> M, broad phase -> global candidate work lists
+template <typename R>
+__global__ void __launch_bounds__(B2S_LB0_THREADS, B2S_LB0_BLOCKS) phase0_kernel(int phases, Grp g) {
+  const DState<R>& s = cstate<R>(g.slot);
+  const WSLayout& L = c_lay[g.slot][LAY_P0];
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  R* smem = reinterpret_cast<R*>(smem_raw);
+  int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  int env = blockIdx.x * wpb + warp;
+  INSTR_BEGIN(s, g, 0)
+#ifdef B2S_INSTR
+  long long instr_t0 = clock64();
+#endif
+  if (env >= g.nenv) return;
+  env += g.env0;
+  Eng<R> e(smem + (size_t)warp * L.total, lane, g.slot, LAY_P0);
+#ifdef B2S_ZERO_SMEM
+  for (int i = lane; i < L.total; i += 32) e.ws[i] = 0;
+  __syncwarp();
+#endif
+  int na, ng;
+  const int warn = phase0_env(e, env, na, ng);
+  // output slots of the candidates: appended to the group's work lists (slots by warp-aggregated atomics)
   int baseA = 0, baseG = 0;
   if (lane == 0) {
     if (na) baseA = g.env0 * s.cl_maxa + atomicAdd(CLC(s, g), na);
@@ -348,15 +496,9 @@ __global__ void __launch_bounds__(B2S_LB0_THREADS, B2S_LB0_BLOCKS) phase0_kernel
   }
   baseA = __shfl_sync(B2S_FULL, baseA, 0);
   baseG = __shfl_sync(B2S_FULL, baseG, 0);
-  int* tab = s.cl_env + E * CL_ENVW(s);
-  if (lane == 0) { tab[0] = na; tab[1] = ng; }
-  for (int i = lane; i < na; i += 32) { s.cl_listA[baseA + i] = (env << 12) | cand[i]; tab[2 + 2 * i] = cand[i]; tab[3 + 2 * i] = baseA + i; }
-  for (int i = lane; i < ng; i += 32) { s.cl_listG[baseG + i] = (env << 12) | cand_g[i]; tab[2 + 2 * (s.cl_maxa + i)] = cand_g[i]; tab[3 + 2 * (s.cl_maxa + i)] = baseG + i; }
-  if (lane == 0) reinterpret_cast<int*>(row + RL.hdr)[2] = warn;
-  __syncwarp();
-  ws_store(e, row, c_pio[g.slot][PIO_P0]);
+  phase0_publish(e, env, na, ng, warn, baseA, baseG, true);
 #ifdef B2S_INSTR
-  if (lane == 0 && s.cyc) s.cyc[(E * 32 + (g.sub & 31)) * 2] = (float)(clock64() - instr_t0);
+  if (lane == 0 && s.cyc) s.cyc[((size_t)env * 32 + (g.sub & 31)) * 2] = (float)(clock64() - instr_t0);
 #endif
   INSTR_END(s, g, 0)
 }
@@ -366,14 +508,9 @@ __global__ void __launch_bounds__(B2S_LB0_THREADS, B2S_LB0_BLOCKS) phase0_kernel
 // the group's overflow list untouched.  tier 1: warps claim the overflowed environments and run them with the full-capacity layout.
 template <typename R>
 __global__ void __launch_bounds__(B2S_LB5_THREADS, B2S_LB5_BLOCKS) tail_kernel(int phases, int nsub, const R* action, Grp g, int tier) {
-  const DModel<R>& m = cmodel<R>(g.slot);
   const DState<R>& s = cstate<R>(g.slot);
   const int lid = tier ? LAY_TL : LAY_TS;
   const WSLayout& L = c_lay[g.slot][lid];
-  const WSLayout& RL = c_lay[g.slot][LAY_ROW];
-  const PhaseIO& io = c_pio[g.slot][tier ? PIO_TL : PIO_TS];
-  const PhaseIO& io_late = c_pio[g.slot][tier ? PIO_TL_LATE : PIO_TS_LATE];
-  const CtrlCfgDev& cc = c_cc[g.slot];
   extern __shared__ __align__(16) unsigned char smem_raw[];
   R* smem = reinterpret_cast<R*>(smem_raw);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpb = blockDim.x >> 5, sub = g.sub;
@@ -388,7 +525,6 @@ __global__ void __launch_bounds__(B2S_LB5_THREADS, B2S_LB5_BLOCKS) tail_kernel(i
   __syncwarp();
 #endif
   int* clc = CLC(s, g);
-  const bool tiered = L.mc < m.maxcon || L.me < m.maxefc;
   for (int iter = 0;; iter++) {
     int env;
     if (tier == 0) {
@@ -406,60 +542,20 @@ __global__ void __launch_bounds__(B2S_LB5_THREADS, B2S_LB5_BLOCKS) tail_kernel(i
 #ifdef B2S_INSTR
     long long instr_t0 = clock64();
 #endif
-    const size_t E = env;
-    const R* row = s.wsg + E * RL.total;
-    int warn = reinterpret_cast<const int*>(row + RL.hdr)[2];  // phase 0: candidate-list overflow
-    ws_load(e, row, io, &mbar[warp], parity);
-    load_row(e.p(L.qpos), s.qpos + E * m.nq, m.nq, lane);
-    load_row(e.p(L.qvel), s.qvel + E * m.nv, m.nv, lane);
-    load_row(e.p(L.ctrl), s.ctrl + E * m.nu, m.nu, lane);
-    load_row(e.p(L.qacc_ws), s.qacc_ws + E * m.nv, m.nv, lane);
-    __syncwarp();
-    int wl = 0;
-    int ncon = gather_contacts(e, env, wl);
-    int nefc = (tiered && (wl & 4)) ? 0 : make_constraint(e, ncon, wl);
-    wl = warp_or_i(wl);  // make_constraint flags a dropped contact on the lane that owns it: the decision below must be warp-uniform
-    if (tiered && (wl & 12)) {  // does not fit this tier: nothing of the environment's state has been touched yet
+    const int pk = tail_rows(e, env, &mbar[warp], parity);
+    if (TAIL_OVF(pk)) {  // does not fit this tier: nothing of the environment's state has been touched yet
       if (lane == 0) s.ovf_list[g.env0 + atomicAdd(clc + 2, 1)] = env;
       __syncwarp();
       continue;
     }
-    warn |= wl;
-    if ((phases & PH_CTRL) && !(phases & PH_CTRL_EXT)) {
-      CtrlState<R> cs;
-      ctrl_load(e, cs, env);
-      ctrl_run(e, cs, env, sub == 0 ? action : (const R*)nullptr);
-      for (int i = lane; i < m.nu; i += 32) s.ctrl[E * m.nu + i] = e.p(L.ctrl)[i];
-      if (sub == 0) ctrl_store(e, cs, env);
-      __syncwarp();
-    }
-    R time = s.time[env];
-    e.actuation((R*)nullptr);
-    if (e.acceleration()) warn |= 1;
-    solve(e, nefc, ncon, warn);
-    if (!(phases & PH_NOINTEGRATE)) {
-      { int eb = e.euler(&time); if (eb & 32) warn |= 32; else if (eb) warn |= 2; }
-    }
-    if ((phases & PH_OBS) && cc.obs_dim > 0 && sub == nsub - 1) {
-      // The reference's observables sample on the LAST substep of a control step: reset()'s forced update already
-      // advances their period timer by one model timestep (utils/observables.py:214-259, environments/base.py:418-427),
-      // so the period closes after substep 24 and the next update - substep 25 - takes the sample.
-      // Body / site poses of this substep's step1 arrive now, over the (dead) constraint Jacobian.
-      ws_load(e, row, io_late, &mbar[warp], parity);
-      write_obs(e, env, (phases & PH_NOINTEGRATE) != 0);
-      write_task(e, env, ncon);
-    }
-    for (int i = lane; i < m.nq; i += 32) s.qpos[E * m.nq + i] = e.p(L.qpos)[i];
-    for (int i = lane; i < m.nv; i += 32) {
-      s.qvel[E * m.nv + i] = e.p(L.qvel)[i];
-      s.qacc[E * m.nv + i] = e.p(L.qacc)[i];
-      s.qacc_ws[E * m.nv + i] = e.p(L.qacc_ws)[i];
-    }
-    warn = warp_or_i(warn);
-    if (lane == 0) { s.time[env] = time; s.warn[env] |= warn; }
-    __syncwarp();
+    const int ncon = TAIL_NCON(pk), nefc = TAIL_NEFC(pk);
+    int warn = TAIL_WARN(pk);
+    if ((phases & PH_CTRL) && !(phases & PH_CTRL_EXT)) tail_ctrl(e, env, sub, action);
+    warn |= tail_accel(e);
+    warn |= tail_newton(e, nefc, ncon);
+    tail_finish(e, env, sub, nsub, phases, ncon, warn, &mbar[warp], parity);
 #ifdef B2S_INSTR
-    if (lane == 0 && s.cyc) s.cyc[(E * 32 + (sub & 31)) * 2 + 1] = (float)(clock64() - instr_t0);
+    if (lane == 0 && s.cyc) s.cyc[((size_t)env * 32 + (sub & 31)) * 2 + 1] = (float)(clock64() - instr_t0);
     if (lane == 0 && s.stats) { atomicAdd(s.stats + 32 + min(ncon, 128), 1); atomicAdd(s.stats + 176 + min(nefc, 320), 1); if (tier) atomicAdd(s.stats + 19, 1); }
 #endif
   }

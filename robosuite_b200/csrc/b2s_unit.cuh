@@ -4,8 +4,8 @@
 // slowest environment (a deep EPA, a 9-iteration Newton solve), so a group's chain costs max(P0) + max(narrow) + max(tail) per substep
 // although the mean environment needs a quarter of that, and the GPU idles in the bubbles.  Here the schedulable unit is ONE SUBSTEP OF
 // ONE ENVIRONMENT: resident warps pull units from a ticket ring in global memory, run kinematics / dynamics / broad phase, the
-// environment's own narrow phase, constraint rows, controller, Newton solve, integration (the very device functions of the other two
-// modes, with their per-phase shared-memory layouts placed in the warp's one workspace area), and push the environment back for its
+// environment's own narrow phase, constraint rows, controller, Newton solve, integration (the very stage functions of the pipeline,
+// with their per-phase shared-memory layouts placed in the warp's one workspace area), and push the environment back for its
 // next substep.  Nothing waits for anybody else's slow item: an expensive environment delays only itself, and the ring hands the next
 // ready environment to whichever warp is free (FIFO, so all environments advance at the same rate).
 //
@@ -26,8 +26,6 @@ struct UnitQ {
   int total, n_large, wpb_large;
   int stride, stride_large;  // words of shared memory per warp: small role / large role
   unsigned long long* prof;  // B2S_UNIT_PROF: [16] clock64 cycles per stage summed over the blocks' rounds (thread 0 of every block), [15] = rounds
-  int barriers;              // small role: -1 free-running warps, 0 the block starts its round of units together, 1..4 block
-                             // barriers between the stages of a round as well (EXPERIMENTAL: stalls, see DESIGN.md)
 };
 
 DEV int ld_acquire_gpu(const int* p) { int v; asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
@@ -49,233 +47,60 @@ template <typename R> __global__ void unit_check_kernel(UnitQ q, int slot) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < s.n_env; i += gridDim.x * blockDim.x) s.warn[i] |= 64;
 }
 
-// steps 1: kinematics, velocity stage + RNE bias, CRB -> M, broad phase; candidate table of the environment; poses etc. -> workspace row
+// ---- the stages of a unit: the shared stage functions of b2s_pipeline.cuh as separately compiled (noinline) functions.  The lockstep
+// rounds of the small role put block barriers between them, and a kernel body that inlines all of it is the kind of function nvcc 12.9
+// has mis-allocated before (DESIGN.md section 3).
+
+// phase 0; the environment owns fixed output slots: analytic candidate i -> env * cl_maxa + i, convex candidate i -> env * cl_maxg + i
 template <typename R> DEVN int unit_phase0(R* area, int lane, int slot, int env) {
-  const DModel<R>& m = cmodel<R>(slot);
   const DState<R>& s = cstate<R>(slot);
-  const WSLayout& L = c_lay[slot][LAY_P0];
-  const WSLayout& RL = c_lay[slot][LAY_ROW];
   Eng<R> e(area, lane, slot, LAY_P0);
-  e.env = env;
-  size_t E = env;
-  R* row = s.wsg + E * RL.total;
-  load_row(e.p(L.qpos), s.qpos + E * m.nq, m.nq, lane);
-  load_row(e.p(L.qvel), s.qvel + E * m.nv, m.nv, lane);
-  __syncwarp();
-  const int was_reset = e.kinematics();
-  if (was_reset) {  // diverged state reset to the model defaults (mj_checkPos / mj_checkVel): the tail reads the state from global memory
-    for (int i = lane; i < m.nq; i += 32) s.qpos[E * m.nq + i] = e.p(L.qpos)[i];
-    for (int i = lane; i < m.nv; i += 32) { s.qvel[E * m.nv + i] = 0; s.qacc[E * m.nv + i] = 0; s.qacc_ws[E * m.nv + i] = 0; }
-    if (lane == 0) s.time[env] = 0;
-    __syncwarp();
-  }
-  e.velocity();
-  e.crb();
-  int* cand = reinterpret_cast<int*>(e.p(L.scratch));
-  int* cand_g = cand + 96;
-  int na, ng, warn = was_reset;
-  cull_pairs(e, cand, cand_g, s.cl_maxa, s.cl_maxg, na, ng);
-  if (na > s.cl_maxa) { na = s.cl_maxa; warn |= 4; }
-  if (ng > s.cl_maxg) { ng = s.cl_maxg; warn |= 4; }
-  // the environment owns fixed output slots: analytic candidate i -> env * cl_maxa + i, convex candidate i -> env * cl_maxg + i
-  int* tab = s.cl_env + E * CL_ENVW(s);
-  if (lane == 0) { tab[0] = na; tab[1] = ng; }
-  for (int i = lane; i < na; i += 32) { tab[2 + 2 * i] = cand[i]; tab[3 + 2 * i] = env * s.cl_maxa + i; }
-  for (int i = lane; i < ng; i += 32) { tab[2 + 2 * (s.cl_maxa + i)] = cand_g[i]; tab[3 + 2 * (s.cl_maxa + i)] = env * s.cl_maxg + i; }
-  if (lane == 0) reinterpret_cast<int*>(row + RL.hdr)[2] = warn;
-  __syncwarp();
-  ws_store(e, row, c_pio[slot][PIO_P0]);
+  int na, ng;
+  const int warn = phase0_env(e, env, na, ng);
+  phase0_publish(e, env, na, ng, warn, env * s.cl_maxa, env * s.cl_maxg, false);
   return na | (ng << 16);
 }
 
 // narrow phase of ONE environment by its own warp: analytic pairs one per lane, convex pairs one after the other with the warp's whole
 // workspace area as EPA polytope + vertex staging scratch (phase 0's regions are in the global row by now)
 template <typename R> DEVN void unit_narrow(R* area, int area_words, int lane, int slot, int env, int na, int ng) {
-  const DModel<R>& m = cmodel<R>(slot);
   const DState<R>& s = cstate<R>(slot);
-  const WSLayout& RL = c_lay[slot][LAY_ROW];
   size_t E = env;
-  const R* row = s.wsg + E * RL.total;
+  const R* row = s.wsg + E * c_lay[slot][LAY_ROW].total;
   const int* tab = s.cl_env + E * CL_ENVW(s);
   for (int base = 0; base < na; base += 32) {
     int i = base + lane;
-    if (i < na) {
-      int pidx = tab[2 + 2 * i];
-      int g1 = m.pair_geom[2 * pidx], g2 = m.pair_geom[2 * pidx + 1];
-      if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
-      Shape<R> A, B;
-      shape_from(m, g1, row + RL.gpos, row + RL.gmat, A);
-      shape_from(m, g2, row + RL.gpos, row + RL.gmat, B);
-      R buf[8 * CREC];
-      int n = narrow_analytic(A, B, buf);
-      R* out = s.cl_outA + ((size_t)env * s.cl_maxa + i) * CL_RECA;
-      out[0] = R(n);
-      for (int k = 0; k < n * CREC; k++) out[1 + k] = buf[k];
-    }
+    if (i < na) narrow_pair_analytic(slot, row, tab[2 + 2 * i], s.cl_outA + (E * s.cl_maxa + i) * CL_RECA);
   }
   __syncwarp();
   const int stage_cap = area_words - EPA_PIPE_WORDS;
-  for (int i = 0; i < ng; i++) {
-    int pidx = tab[2 + 2 * (s.cl_maxa + i)];
-    int g1 = m.pair_geom[2 * pidx], g2 = m.pair_geom[2 * pidx + 1];
-    if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
-    Shape<R> A, B;
-    shape_from(m, g1, row + RL.gpos, row + RL.gmat, A);
-    shape_from(m, g2, row + RL.gpos, row + RL.gmat, B);
-    R buf[CREC];
-    int n = convex_convex(A, B, buf, 1, area, lane, s.gjk_cache ? s.gjk_cache + ((size_t)env * m.npair + pidx) * 3 : (R*)nullptr,
-                          EPA_PIPE_MAXV, EPA_PIPE_MAXF, stage_cap >= 64 ? area + EPA_PIPE_WORDS : (R*)nullptr, stage_cap >= 64 ? stage_cap : 0);
-    R* out = s.cl_outG + ((size_t)env * s.cl_maxg + i) * 8;
-    if (lane == 0) {
-      out[0] = R(n);
-      for (int k = 0; k < CREC; k++) out[1 + k] = n ? buf[k] : R(0);
-    }
-    __syncwarp();
-  }
+  for (int i = 0; i < ng; i++)
+    narrow_pair_convex(slot, env, row, tab[2 + 2 * (s.cl_maxa + i)], s.cl_outG + (E * s.cl_maxg + i) * 8, area,
+                       stage_cap >= 64 ? area + EPA_PIPE_WORDS : (R*)nullptr, stage_cap >= 64 ? stage_cap : 0, lane, false);
   __syncwarp();
 }
 
-// contact gather, constraint rows, controller, actuation, Newton solve, Euler, observation / task rows of substep `sub`.
-// Returns 0 when the unit is finished, 1 when the environment does not fit this tier (nothing of its state has been touched).
-template <typename R>
-DEV int unit_tail(R* area, int lane, int slot, int lid, int env, int sub, int nsub, int phases, const R* action, unsigned long long* bar, unsigned& parity) {
-  const DModel<R>& m = cmodel<R>(slot);
-  const DState<R>& s = cstate<R>(slot);
-  const WSLayout& L = c_lay[slot][lid];
-  const WSLayout& RL = c_lay[slot][LAY_ROW];
-  const PhaseIO& io = c_pio[slot][lid == LAY_TL ? PIO_TL : PIO_TS];
-  const PhaseIO& io_late = c_pio[slot][lid == LAY_TL ? PIO_TL_LATE : PIO_TS_LATE];
-  const CtrlCfgDev& cc = c_cc[slot];
-  Eng<R> e(area, lane, slot, lid);
-  const bool tiered = L.mc < m.maxcon || L.me < m.maxefc;
-  const size_t E = env;
-  const R* row = s.wsg + E * RL.total;
-  int warn = reinterpret_cast<const int*>(row + RL.hdr)[2];
-  ws_load(e, row, io, bar, parity);
-  load_row(e.p(L.qpos), s.qpos + E * m.nq, m.nq, lane);
-  load_row(e.p(L.qvel), s.qvel + E * m.nv, m.nv, lane);
-  load_row(e.p(L.ctrl), s.ctrl + E * m.nu, m.nu, lane);
-  load_row(e.p(L.qacc_ws), s.qacc_ws + E * m.nv, m.nv, lane);
-  __syncwarp();
-  int wl = 0;
-  int ncon = gather_contacts(e, env, wl);
-  int nefc = (tiered && (wl & 4)) ? 0 : make_constraint(e, ncon, wl);
-  wl = warp_or_i(wl);
-  if (tiered && (wl & 12)) return 1;
-  warn |= wl;
-  if (phases & PH_CTRL) {
-    CtrlState<R> cs;
-    ctrl_load(e, cs, env);
-    ctrl_run(e, cs, env, sub == 0 ? action : (const R*)nullptr);
-    for (int i = lane; i < m.nu; i += 32) s.ctrl[E * m.nu + i] = e.p(L.ctrl)[i];
-    if (sub == 0) ctrl_store(e, cs, env);
-    __syncwarp();
-  }
-  R time = s.time[env];
-  e.actuation((R*)nullptr);
-  if (e.acceleration()) warn |= 1;
-  solve(e, nefc, ncon, warn);
-  if (!(phases & PH_NOINTEGRATE)) {
-    { int eb = e.euler(&time); if (eb & 32) warn |= 32; else if (eb) warn |= 2; }
-  }
-  if ((phases & PH_OBS) && cc.obs_dim > 0 && sub == nsub - 1) {
-    ws_load(e, row, io_late, bar, parity);
-    write_obs(e, env, (phases & PH_NOINTEGRATE) != 0);
-    write_task(e, env, ncon);
-  }
-  for (int i = lane; i < m.nq; i += 32) s.qpos[E * m.nq + i] = e.p(L.qpos)[i];
-  for (int i = lane; i < m.nv; i += 32) {
-    s.qvel[E * m.nv + i] = e.p(L.qvel)[i];
-    s.qacc[E * m.nv + i] = e.p(L.qacc)[i];
-    s.qacc_ws[E * m.nv + i] = e.p(L.qacc_ws)[i];
-  }
-  warn = warp_or_i(warn);
-  if (lane == 0) { s.time[env] = time; s.warn[env] |= warn; }
-  __syncwarp();
-  return 0;
-}
-
-// ---- the tail of a unit as separately compiled (noinline) stages: the lockstep rounds of the small role put block barriers between
-// them, and a kernel body that inlines all of it is the kind of function nvcc 12.9 has mis-allocated before (DESIGN.md section 3)
-// packed result of stage A: ncon (8 bits) | nefc (10 bits) << 8 | warn (8 bits) << 20 | does-not-fit-this-tier << 30
-template <typename R>
-DEVN int unit_tail_a(R* area, int lane, int slot, int env, unsigned long long* bar, unsigned& parity) {
-  const DModel<R>& m = cmodel<R>(slot);
-  const DState<R>& s = cstate<R>(slot);
-  const WSLayout& L = c_lay[slot][LAY_TS];
-  const WSLayout& RL = c_lay[slot][LAY_ROW];
+// the tail of a small-tier unit (the packed word of tail_rows, the warn bits of the dynamics)
+template <typename R> DEVN int unit_tail_a(R* area, int lane, int slot, int env, unsigned long long* bar, unsigned& parity) {
   Eng<R> e(area, lane, slot, LAY_TS);
-  const bool tiered = L.mc < m.maxcon || L.me < m.maxefc;
-  const size_t E = env;
-  const R* row = s.wsg + E * RL.total;
-  int warn = reinterpret_cast<const int*>(row + RL.hdr)[2];
-  ws_load(e, row, c_pio[slot][PIO_TS], bar, parity);
-  load_row(e.p(L.qpos), s.qpos + E * m.nq, m.nq, lane);
-  load_row(e.p(L.qvel), s.qvel + E * m.nv, m.nv, lane);
-  load_row(e.p(L.ctrl), s.ctrl + E * m.nu, m.nu, lane);
-  load_row(e.p(L.qacc_ws), s.qacc_ws + E * m.nv, m.nv, lane);
-  __syncwarp();
-  int wl = 0;
-  int ncon = gather_contacts(e, env, wl);
-  int nefc = (tiered && (wl & 4)) ? 0 : make_constraint(e, ncon, wl);
-  wl = warp_or_i(wl);
-  int ovf = (tiered && (wl & 12)) ? 1 : 0;
-  warn = warp_or_i(warn | wl) & 255;
-  return (ncon & 255) | ((nefc & 1023) << 8) | (warn << 20) | (ovf << 30);
+  return tail_rows(e, env, bar, parity);
 }
 template <typename R> DEVN void unit_tail_ctrl(R* area, int lane, int slot, int env, int sub, const R* action) {
-  const DModel<R>& m = cmodel<R>(slot);
-  const DState<R>& s = cstate<R>(slot);
-  const WSLayout& L = c_lay[slot][LAY_TS];
   Eng<R> e(area, lane, slot, LAY_TS);
-  const size_t E = env;
-  CtrlState<R> cs;
-  ctrl_load(e, cs, env);
-  ctrl_run(e, cs, env, sub == 0 ? action : (const R*)nullptr);
-  for (int i = lane; i < m.nu; i += 32) s.ctrl[E * m.nu + i] = e.p(L.ctrl)[i];
-  if (sub == 0) ctrl_store(e, cs, env);
-  __syncwarp();
+  tail_ctrl(e, env, sub, action);
 }
 template <typename R> DEVN int unit_tail_acc(R* area, int lane, int slot) {
   Eng<R> e(area, lane, slot, LAY_TS);
-  e.actuation((R*)nullptr);
-  int w = e.acceleration() ? 1 : 0;
-  return warp_or_i(w);
+  return tail_accel(e);
 }
 template <typename R> DEVN int unit_tail_solve(R* area, int lane, int slot, int nefc, int ncon) {
   Eng<R> e(area, lane, slot, LAY_TS);
-  int warn = 0;
-  solve(e, nefc, ncon, warn);
-  return warp_or_i(warn);
+  return tail_newton(e, nefc, ncon);
 }
 template <typename R>
 DEVN void unit_tail_end(R* area, int lane, int slot, int env, int sub, int nsub, int phases, int ncon, int warn, unsigned long long* bar, unsigned& parity) {
-  const DModel<R>& m = cmodel<R>(slot);
-  const DState<R>& s = cstate<R>(slot);
-  const WSLayout& L = c_lay[slot][LAY_TS];
-  const WSLayout& RL = c_lay[slot][LAY_ROW];
-  const CtrlCfgDev& cc = c_cc[slot];
   Eng<R> e(area, lane, slot, LAY_TS);
-  const size_t E = env;
-  const R* row = s.wsg + E * RL.total;
-  R time = s.time[env];
-  if (!(phases & PH_NOINTEGRATE)) {
-    { int eb = e.euler(&time); if (eb & 32) warn |= 32; else if (eb) warn |= 2; }
-  }
-  if ((phases & PH_OBS) && cc.obs_dim > 0 && sub == nsub - 1) {
-    ws_load(e, row, c_pio[slot][PIO_TS_LATE], bar, parity);
-    write_obs(e, env, (phases & PH_NOINTEGRATE) != 0);
-    write_task(e, env, ncon);
-  }
-  for (int i = lane; i < m.nq; i += 32) s.qpos[E * m.nq + i] = e.p(L.qpos)[i];
-  for (int i = lane; i < m.nv; i += 32) {
-    s.qvel[E * m.nv + i] = e.p(L.qvel)[i];
-    s.qacc[E * m.nv + i] = e.p(L.qacc)[i];
-    s.qacc_ws[E * m.nv + i] = e.p(L.qacc_ws)[i];
-  }
-  warn = warp_or_i(warn);
-  if (lane == 0) { s.time[env] = time; s.warn[env] |= warn; }
-  __syncwarp();
+  tail_finish(e, env, sub, nsub, phases, ncon, warn, bar, parity);
 }
 
 // the unit is finished: hand the environment to whoever takes the next ticket (or count it as done after its last substep)
@@ -294,8 +119,8 @@ DEV void unit_finish(const UnitQ& q, int n_env, int env, int sub, int nsub, int 
 
 
 // One block of 16 warps per SM: what counts is that an SM executes ONE code region at a time (the hot code is ~10x the instruction
-// cache).  Measured on 4096 Lift environments (tools/run30.sh): 16 warps x 1 block 306 k env-steps/s, 8 warps x 2 blocks 248 k,
-// 8 warps x 1 block 210 k, 4 warps x 4 blocks 158 k, free-running warps 80 k.
+// cache).  Measured on 4096 Lift environments: 16 warps x 1 block 306 k env-steps/s, 8 warps x 2 blocks 248 k, 8 warps x 1 block 210 k,
+// 4 warps x 4 blocks 158 k, free-running warps (no block barriers) 80 k.
 #ifndef B2S_LBU_THREADS
 #define B2S_LBU_THREADS 512
 #define B2S_LBU_BLOCKS 1
@@ -334,7 +159,14 @@ __global__ void __launch_bounds__(B2S_LBU_THREADS, B2S_LBU_BLOCKS) unit_kernel(i
       __syncwarp();
       fence_proxy_async_all();  // the row was written through the async proxy of another SM
       const int env = code % n_env, sub = code / n_env;
-      unit_tail<R>(area, lane, slot, LAY_TL, env, sub, nsub, phases, action, &mbar[warp], parity);
+      Eng<R> e(area, lane, slot, LAY_TL);
+      const int pk = tail_rows(e, env, &mbar[warp], parity);  // the full-capacity layout holds every environment: no overflow
+      const int ncon = TAIL_NCON(pk);
+      int warn = TAIL_WARN(pk);
+      if (phases & PH_CTRL) tail_ctrl(e, env, sub, action);
+      warn |= tail_accel(e);
+      warn |= tail_newton(e, TAIL_NEFC(pk), ncon);
+      tail_finish(e, env, sub, nsub, phases, ncon, warn, &mbar[warp], parity);
       unit_finish(q, n_env, env, sub, nsub, lane);
     }
     return;
@@ -347,46 +179,37 @@ __global__ void __launch_bounds__(B2S_LBU_THREADS, B2S_LBU_BLOCKS) unit_kernel(i
   const int wpb = blockDim.x >> 5;
   __shared__ int sh_t0, sh_k;
   R* area = smem + (size_t)warp * q.stride;
-#define UBAR(level) if (q.barriers >= (level)) __syncthreads();
 #define UTICK(k) if (q.prof != nullptr && threadIdx.x == 0) { long long tn_ = clock64(); atomicAdd(q.prof + (k), (unsigned long long)(tn_ - tprev)); tprev = tn_; }
   long long tprev = clock64();
   for (;;) {
-    int t;
-    if (q.barriers >= 0) {
-      // the block takes up to `wpb` tickets that are ALREADY PRODUCED (head < tail).  The first lockstep version took `wpb` tickets
-      // whether they existed or not and waited for the missing ones in front of the first stage barrier: every control step stalled until
-      // the watchdog on the GPU (the ticket arithmetic itself terminates: tests/test_unit_queue_protocol.py).  No wait inside a round now.
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        int t0v = 0x7fffffff, k = 0, spins = 0;
-        for (;;) {
-          if (ld_relaxed_gpu(q.ctr + 7) != 0) break;
-          const int H = ld_relaxed_gpu(q.ctr);
-          if (H >= q.total) break;
-          const int P = ld_acquire_gpu(q.ctr + 1);
-          if (H < P) {
-            k = min(wpb, P - H);
-            if (atomicCAS(q.ctr, H, H + k) == H) { t0v = H; break; }
-            k = 0;
-            continue;
-          }
-          __nanosleep(100);
-          if (++spins > (1 << 22)) { atomicCAS(q.ctr + 7, 0, 2); break; }
+    // the block takes up to `wpb` tickets that are ALREADY PRODUCED (head < tail).  The first lockstep version took `wpb` tickets
+    // whether they existed or not and waited for the missing ones in front of the first stage barrier: every control step stalled until
+    // the watchdog on the GPU (the ticket arithmetic itself terminates: tests/test_unit_queue_protocol.py).  No wait inside a round now.
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      int t0v = 0x7fffffff, k = 0, spins = 0;
+      for (;;) {
+        if (ld_relaxed_gpu(q.ctr + 7) != 0) break;
+        const int H = ld_relaxed_gpu(q.ctr);
+        if (H >= q.total) break;
+        const int P = ld_acquire_gpu(q.ctr + 1);
+        if (H < P) {
+          k = min(wpb, P - H);
+          if (atomicCAS(q.ctr, H, H + k) == H) { t0v = H; break; }
+          k = 0;
+          continue;
         }
-        sh_t0 = t0v; sh_k = k;
+        __nanosleep(100);
+        if (++spins > (1 << 22)) { atomicCAS(q.ctr + 7, 0, 2); break; }
       }
-      __syncthreads();
-      const int t0 = sh_t0;
-      if (t0 == 0x7fffffff) break;
-      UTICK(0)
-      if (q.prof != nullptr && threadIdx.x == 0) atomicAdd(q.prof + 15, 1ull);
-      t = warp < sh_k ? t0 + warp : q.total;
-    } else {  // free-running warps (no block synchronisation at all): one ticket per warp
-      t = 0;
-      if (lane == 0) t = ld_relaxed_gpu(q.ctr + 7) != 0 ? 0x7fffffff : atomicAdd(q.ctr, 1);
-      t = __shfl_sync(B2S_FULL, t, 0);
-      if (t >= q.total) break;
+      sh_t0 = t0v; sh_k = k;
     }
+    __syncthreads();
+    const int t0 = sh_t0;
+    if (t0 == 0x7fffffff) break;
+    UTICK(0)
+    if (q.prof != nullptr && threadIdx.x == 0) atomicAdd(q.prof + 15, 1ull);
+    const int t = warp < sh_k ? t0 + warp : q.total;
     bool live = t < q.total;
     int code = 0;
     if (live) {
@@ -407,20 +230,20 @@ __global__ void __launch_bounds__(B2S_LBU_THREADS, B2S_LBU_BLOCKS) unit_kernel(i
       if (code < 0) { live = false; code = 0; }
     }
     const int env = code % n_env, sub = code / n_env;
-    UBAR(1)
+    __syncthreads();
     UTICK(1)
     int nn = 0;
     if (live) nn = unit_phase0<R>(area, lane, slot, env);
-    UBAR(2)
+    __syncthreads();
     UTICK(2)
     if (live) unit_narrow<R>(area, q.stride, lane, slot, env, nn & 0xffff, nn >> 16);
-    UBAR(1)
+    __syncthreads();
     UTICK(3)
     int warn = 0, ncon = 0, nefc = 0;
     if (live) {
       const int pk = unit_tail_a<R>(area, lane, slot, env, &mbar[warp], parity);
-      ncon = pk & 255; nefc = (pk >> 8) & 1023; warn = (pk >> 20) & 255;
-      if (pk >> 30) {  // does not fit the small tier: to the large-role warps, nothing of the state has been touched
+      ncon = TAIL_NCON(pk); nefc = TAIL_NEFC(pk); warn = TAIL_WARN(pk);
+      if (TAIL_OVF(pk)) {  // does not fit the small tier: to the large-role warps, nothing of the state has been touched
         if (lane == 0) {
           __threadfence();
           int p = atomicAdd(q.ctr + 4, 1);
@@ -430,16 +253,16 @@ __global__ void __launch_bounds__(B2S_LBU_THREADS, B2S_LBU_BLOCKS) unit_kernel(i
         live = false;
       }
     }
-    UBAR(3)
+    __syncthreads();
     UTICK(4)
     if (live && (phases & PH_CTRL)) unit_tail_ctrl<R>(area, lane, slot, env, sub, action);
-    UBAR(3)
+    __syncthreads();
     UTICK(5)
     if (live) warn |= unit_tail_acc<R>(area, lane, slot);
-    UBAR(4)
+    __syncthreads();
     UTICK(6)
     if (live) warn |= unit_tail_solve<R>(area, lane, slot, nefc, ncon);
-    UBAR(4)
+    __syncthreads();
     UTICK(7)
     if (live) {
       unit_tail_end<R>(area, lane, slot, env, sub, nsub, phases, ncon, warn, &mbar[warp], parity);
@@ -447,6 +270,5 @@ __global__ void __launch_bounds__(B2S_LBU_THREADS, B2S_LBU_BLOCKS) unit_kernel(i
     }
     UTICK(8)
   }
-#undef UBAR
 #undef UTICK
 }
