@@ -119,6 +119,27 @@ int b2s_reset_envs(b2s_sim* sim, const uint8_t* env_mask, const void* qpos_new);
  * pose: override them too (pose = parent pose * local pose).  At most 4 bodies per handle. */
 int b2s_body_pose_override(b2s_sim* sim, int body_id);
 
+/* Per-environment model values (domain randomisation; the reference draws e.g. Lift's cube size per model build,
+ * environments/manipulation/lift.py:311-314).  Declares a per-environment copy of `field` for object `id`: afterwards the array
+ * "<field>:<id>" (fetch it with b2s_array) holds one value per environment, initialised to the model's, and every step reads it.
+ *   "geom_size"     [n_env, 3]  colliding sphere / capsule / ellipsoid / cylinder / box geoms
+ *   "geom_friction" [n_env, 3]  same geoms
+ *   "body_mass"     [n_env]     moving bodies
+ *   "body_inertia"  [n_env, 3]  moving bodies: principal moments in the model's inertial frame (body_ipos / body_iquat stay shared)
+ * A declared geom also gets "geom_rbound:<id>" [n_env] and "geom_aabb:<id>" [n_env, 6]; the first declaration of a handle creates
+ * "dof_invweight0" [n_env, nv], "body_invweight0" [n_env, nbody, 2] and "meaninertia" [n_env].  These DERIVED constants start at the
+ * model's values and are STALE after a change until b2s_set_const or b2s_reset / b2s_reset_envs (which run the same pass for their
+ * masked environments whenever the handle has overrides) recomputes them.  Returns B2S_ERR_ARG for an unknown field or an id out of
+ * range, B2S_ERR_UNSUPPORTED for meshes, planes, non-colliding geoms, the world body and bodies welded to it, and beyond 8 geoms or
+ * 8 bodies per handle.  Declaring again returns B2S_OK and changes nothing. */
+int b2s_model_override(b2s_sim* sim, const char* field, int id);
+/* The set-constants pass for the masked environments (env_mask: n_env device bytes, NULL = all), one warp each, on the handle's
+ * stream: kinematics and composite inertia at qpos0 (world-pose overrides honoured) -> dof_invweight0, body_invweight0, meaninertia
+ * (the compiler's definitions), and the bounding radius / box of every overridden geom from its size.  Environments whose override
+ * values are non-finite or non-positive, or whose moments violate the triangle inequality, get warn bit 128.  No-op on a handle
+ * without overrides. */
+int b2s_set_const(b2s_sim* sim, const uint8_t* env_mask);
+
 /* Observation program = MujocoEnv._get_observations flattened (environments/base.py:429-465): one (op, a, b) entry
  * per output scalar (ops: enum OB_* in csrc/b2s_types.cuh; OB_REL_*_LAG entries read the previous sample, as the reference's
  * sensor ordering does: manipulation_env.py:268-329).  Creates the device arrays "obs" [n_env, obs_dim] and "obs_fresh" [n_env]

@@ -93,7 +93,14 @@ struct b2s_sim {
   unsigned long long* uq_prof = nullptr;
   std::vector<double> xpos0_h, xquat0_h;  // world poses of the bodies welded to the world (model constants)
   std::vector<int> body_weldid_h;
+  // model values that b2s_model_override copies per environment, and the host-computed constants derived from them
+  std::vector<int> geom_type_h;
+  std::vector<double> geom_size_h, geom_friction_h, geom_rbound_h, geom_aabb_h, body_mass_h, body_inertia_h, dof_iw_h, body_iw_h;
+  double meaninertia_h = 1;
+  int sc_words = 0;  // set-constants pass: words of shared memory per warp (0 until its first launch)
 };
+
+static int launch_set_const(b2s_sim* s, const uint8_t* mask);  // the set-constants pass (no-op without model overrides)
 
 template <typename T> static T* dev_upload(b2s_sim* s, const std::vector<T>& h) {
   T* d = nullptr;
@@ -262,6 +269,14 @@ template <typename R> static void build_model(b2s_sim* s, const Blob& b, DModel<
   m.body_xpos0 = up_vec<R>(s, xpos0); m.body_xquat0 = up_vec<R>(s, xquat0);
   s->xpos0_h = xpos0; s->xquat0_h = xquat0;
   { const int* wd = b.i32("body_weldid"); s->body_weldid_h.assign(wd, wd + nb); }
+  {
+    auto host = [&](const char* name, std::vector<double>& v) { int64_t n = 0; const double* p = b.f64(name, &n); v.assign(p, p + n); };
+    host("geom_size", s->geom_size_h); host("geom_friction", s->geom_friction_h); host("geom_rbound", s->geom_rbound_h);
+    host("geom_aabb", s->geom_aabb_h); host("body_mass", s->body_mass_h); host("body_inertia", s->body_inertia_h);
+    host("dof_invweight0", s->dof_iw_h); host("body_invweight0", s->body_iw_h);
+    s->meaninertia_h = b.scalar_f("stat_meaninertia");
+    const int* gt = b.i32("geom_type"); s->geom_type_h.assign(gt, gt + ng);
+  }
   m.jnt_type = up_i(s, b, "jnt_type"); m.jnt_qposadr = up_i(s, b, "jnt_qposadr"); m.jnt_dofadr = up_i(s, b, "jnt_dofadr");
   m.jnt_bodyid = up_i(s, b, "jnt_bodyid"); m.jnt_limited = up_i(s, b, "jnt_limited");
   m.jnt_pos = up_f<R>(s, b, "jnt_pos"); m.jnt_axis = up_f<R>(s, b, "jnt_axis"); m.jnt_range = up_f<R>(s, b, "jnt_range");
@@ -1150,7 +1165,7 @@ int b2s_reset(b2s_sim* s, const uint8_t* mask) {
   clear_warm_start(s, mask);
   s->launches++;
   CUDA_TRY(cudaGetLastError());
-  return B2S_OK;
+  return launch_set_const(s, mask);
 }
 
 int b2s_forward(b2s_sim* s) { return s ? launch(s, PH_STEP1 | PH_STEP2 | PH_NOINTEGRATE | PH_EXPORT | (s->has_obs ? PH_OBS : 0), 1) : fail(B2S_ERR_ARG, "null handle"); }
@@ -1281,6 +1296,7 @@ int b2s_reset_envs(b2s_sim* s, const uint8_t* mask, const void* qpos_new) {
   else reset_envs_kernel<double><<<blocks, threads, 0, s->stream>>>(mask, (const double*)qpos_new, s->slot);
   s->launches++;
   CUDA_TRY(cudaGetLastError());
+  { int rc = launch_set_const(s, mask); if (rc != B2S_OK) return rc; }  // after the warn bits were cleared: bit 128 survives
   int rc = launch(s, PH_STEP1 | PH_STEP2 | PH_NOINTEGRATE | PH_EXPORT | (s->has_obs ? PH_OBS : 0), 1, nullptr, mask);
   if (rc != B2S_OK) return rc;
   if (s->has_ctrl) return b2s_ctrl_reset(s, mask);
@@ -1307,7 +1323,109 @@ template <typename R> static int body_pose_override_t(b2s_sim* s, DState<R>& st,
   s->dirty = 1;
   return B2S_OK;
 }
+// ---- per-environment model values (b2s_model_override) and the set-constants pass
+static bool has_model_overrides(const b2s_sim* s) { return s->precision == B2S_F32 ? s->sf.dof_iw != nullptr : s->sd.dof_iw != nullptr; }
+
+template <typename R> static void upload_rows(R* dst, const double* src, int k, size_t n_env) {  // n_env copies of src[0..k)
+  std::vector<R> h(n_env * k);
+  for (size_t e = 0; e < n_env; e++) for (int q = 0; q < k; q++) h[e * k + q] = (R)src[q];
+  cudaMemcpy(dst, h.data(), h.size() * sizeof(R), cudaMemcpyHostToDevice);
+  cudaStreamSynchronize(cudaStreamLegacy);  // see dev_upload
+}
+
+template <typename R> static int model_override_t(b2s_sim* s, DState<R>& st, const std::string& field, int id) {
+  const bool geom = field == "geom_size" || field == "geom_friction";
+  const size_t N = s->n_env;
+  const int code = DT<R>::code;
+  try {
+    if (!st.dof_iw) {  // first override of the handle: the banks of every slot, the derived constants from the model's values
+      st.mg_size = dev_zeros<R>(s, B2S_MOV * N * 3); st.mg_fric = dev_zeros<R>(s, B2S_MOV * N * 3);
+      st.mg_rbound = dev_zeros<R>(s, B2S_MOV * N); st.mg_aabb = dev_zeros<R>(s, B2S_MOV * N * 6);
+      st.mb_mass = dev_zeros<R>(s, B2S_MOV * N); st.mb_inertia = dev_zeros<R>(s, B2S_MOV * N * 3);
+      R* diw = dev_zeros<R>(s, N * s->nv); R* biw = dev_zeros<R>(s, N * s->nbody * 2); R* mi = dev_zeros<R>(s, N);
+      upload_rows(diw, s->dof_iw_h.data(), s->nv, N);
+      upload_rows(biw, s->body_iw_h.data(), 2 * s->nbody, N);
+      upload_rows(mi, &s->meaninertia_h, 1, N);
+      s->arrays["dof_invweight0"] = ArrayInfo{diw, code, 2, {s->n_env, s->nv, 0, 0}};
+      s->arrays["body_invweight0"] = ArrayInfo{biw, code, 3, {s->n_env, s->nbody, 2, 0}};
+      s->arrays["meaninertia"] = ArrayInfo{mi, code, 1, {s->n_env, 0, 0, 0}};
+      st.dof_iw = diw; st.body_iw = biw; st.mean_inertia = mi;
+    }
+    const std::string key = field + ":" + std::to_string(id);
+    if (s->arrays.count(key)) return B2S_OK;
+    if (geom) {
+      int k = 0;
+      while (k < st.n_mg && st.mg_id[k] != id) k++;
+      if (k == st.n_mg) {  // a new slot: size, friction, bounds of this geom for every environment
+        if (k >= B2S_MOV) return fail(B2S_ERR_UNSUPPORTED, "b2s_model_override: at most 8 geoms per handle");
+        upload_rows(st.mg_size + k * N * 3, &s->geom_size_h[3 * id], 3, N);
+        upload_rows(st.mg_fric + k * N * 3, &s->geom_friction_h[3 * id], 3, N);
+        upload_rows(st.mg_rbound + k * N, &s->geom_rbound_h[id], 1, N);
+        upload_rows(st.mg_aabb + k * N * 6, &s->geom_aabb_h[6 * id], 6, N);
+        st.mg_id[k] = (short)id; st.n_mg = k + 1;
+        s->arrays["geom_rbound:" + std::to_string(id)] = ArrayInfo{st.mg_rbound + k * N, code, 1, {s->n_env, 0, 0, 0}};
+        s->arrays["geom_aabb:" + std::to_string(id)] = ArrayInfo{st.mg_aabb + k * N * 6, code, 2, {s->n_env, 6, 0, 0}};
+      }
+      R* p = field == "geom_size" ? st.mg_size + k * N * 3 : st.mg_fric + k * N * 3;
+      s->arrays[key] = ArrayInfo{p, code, 2, {s->n_env, 3, 0, 0}};
+    } else {
+      int k = 0;
+      while (k < st.n_mb && st.mb_id[k] != id) k++;
+      if (k == st.n_mb) {
+        if (k >= B2S_MOV) return fail(B2S_ERR_UNSUPPORTED, "b2s_model_override: at most 8 bodies per handle");
+        upload_rows(st.mb_mass + k * N, &s->body_mass_h[id], 1, N);
+        upload_rows(st.mb_inertia + k * N * 3, &s->body_inertia_h[3 * id], 3, N);
+        st.mb_id[k] = (short)id; st.n_mb = k + 1;
+      }
+      if (field == "body_mass") s->arrays[key] = ArrayInfo{st.mb_mass + k * N, code, 1, {s->n_env, 0, 0, 0}};
+      else s->arrays[key] = ArrayInfo{st.mb_inertia + k * N * 3, code, 2, {s->n_env, 3, 0, 0}};
+    }
+  } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
+  s->dirty = 1;
+  return B2S_OK;
+}
+
+static int launch_set_const(b2s_sim* s, const uint8_t* mask) {
+  if (!has_model_overrides(s)) return B2S_OK;
+  { int rc = bind_constants(s); if (rc != B2S_OK) return rc; }
+  const size_t rsz = s->precision == B2S_F32 ? 4 : 8;
+  if (s->sc_words == 0) {
+    CUDA_TRY(s->precision == B2S_F32 ? optin_max_smem(set_const_kernel<float>, s->device) : optin_max_smem(set_const_kernel<double>, s->device));
+    s->sc_words = s->lay[LAY_FULL].total + ((s->nv * s->nv + 3) & ~3);
+  }
+  const int wpb = fit_wpb((size_t)s->sc_words * rsz, 16), blocks = (s->n_env + wpb - 1) / wpb;
+  const size_t smem = (size_t)s->sc_words * rsz * wpb;
+  if (s->precision == B2S_F32) set_const_kernel<float><<<blocks, wpb * 32, smem, s->stream>>>(mask, s->slot, s->sc_words);
+  else set_const_kernel<double><<<blocks, wpb * 32, smem, s->stream>>>(mask, s->slot, s->sc_words);
+  s->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return B2S_OK;
+}
+
 extern "C" {
+int b2s_model_override(b2s_sim* s, const char* field, int id) {
+  if (!s || !field) return fail(B2S_ERR_ARG, "b2s_model_override: bad argument");
+  const std::string f = field;
+  if (f == "geom_size" || f == "geom_friction") {
+    if (id < 0 || id >= s->ngeom) return fail(B2S_ERR_ARG, "b2s_model_override: geom id out of range");
+    const int t = s->geom_type_h[id];
+    if (s->cgid[id] < 0 || !(t == G_SPHERE || t == G_CAPSULE || t == G_ELLIPSOID || t == G_CYLINDER || t == G_BOX))
+      return fail(B2S_ERR_UNSUPPORTED, "b2s_model_override: only colliding sphere, capsule, ellipsoid, cylinder and box geoms have per-environment values");
+  } else if (f == "body_mass" || f == "body_inertia") {
+    if (id < 0 || id >= s->nbody) return fail(B2S_ERR_ARG, "b2s_model_override: body id out of range");
+    if (s->body_weldid_h[id] == 0) return fail(B2S_ERR_UNSUPPORTED, "b2s_model_override: the body does not move (world body or welded to it)");
+  } else {
+    return fail(B2S_ERR_ARG, "b2s_model_override: unknown field '" + f + "' (geom_size, geom_friction, body_mass, body_inertia)");
+  }
+  CUDA_TRY(cudaSetDevice(s->device));
+  return s->precision == B2S_F32 ? model_override_t<float>(s, s->sf, f, id) : model_override_t<double>(s, s->sd, f, id);
+}
+
+int b2s_set_const(b2s_sim* s, const uint8_t* env_mask) {
+  if (!s) return fail(B2S_ERR_ARG, "null handle");
+  return launch_set_const(s, env_mask);
+}
+
 int b2s_body_pose_override(b2s_sim* s, int body_id) {
   if (!s || body_id <= 0 || body_id >= s->nbody) return fail(B2S_ERR_ARG, "b2s_body_pose_override: bad argument");
   if (s->body_weldid_h[body_id] != 0) return fail(B2S_ERR_UNSUPPORTED, "b2s_body_pose_override: the body is not welded to the world (move it through qpos)");

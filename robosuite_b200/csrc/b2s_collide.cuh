@@ -23,7 +23,8 @@ DEV void shape_get(const Eng<R>& e, int g, Shape<R>& s) {
   s.type = m.geom_type[g];
   s.pos = e.p(e.lay().gpos) + 3 * k;
   s.mat = e.p(e.lay().gmat) + 9 * k;
-  s.size[0] = m.geom_size[3 * g]; s.size[1] = m.geom_size[3 * g + 1]; s.size[2] = m.geom_size[3 * g + 2];
+  const R* sz = geom_size_of(m, e.state(), g, e.env);
+  s.size[0] = sz[0]; s.size[1] = sz[1]; s.size[2] = sz[2];
   s.vert = nullptr; s.nvert = 0;
   if (s.type == G_MESH) {
     int id = m.geom_dataid[g];
@@ -33,12 +34,13 @@ DEV void shape_get(const Eng<R>& e, int g, Shape<R>& s) {
 }
 
 template <typename R>
-DEV void shape_from(const DModel<R>& m, int g, const R* gpos, const R* gmat, Shape<R>& s) {
+DEV void shape_from(const DModel<R>& m, const DState<R>& st, int env, int g, const R* gpos, const R* gmat, Shape<R>& s) {
   int k = m.geom_cgid[g];
   s.type = m.geom_type[g];
   s.pos = gpos + 3 * k;
   s.mat = gmat + 9 * k;
-  s.size[0] = m.geom_size[3 * g]; s.size[1] = m.geom_size[3 * g + 1]; s.size[2] = m.geom_size[3 * g + 2];
+  const R* sz = geom_size_of(m, st, g, env);
+  s.size[0] = sz[0]; s.size[1] = sz[1]; s.size[2] = sz[2];
   s.vert = nullptr; s.nvert = 0;
   if (s.type == G_MESH) {
     int id = m.geom_dataid[g];
@@ -912,7 +914,7 @@ template <typename R> DEVN bool obb_overlap(const Eng<R> e, int g1, int g2) {
   const DModel<R>& m = e.model();
   int k1 = m.geom_cgid[g1], k2 = m.geom_cgid[g2];
   const R* M1 = e.p(e.lay().gmat) + 9 * k1; const R* M2 = e.p(e.lay().gmat) + 9 * k2;
-  const R* a1 = m.geom_aabb + 6 * g1; const R* a2 = m.geom_aabb + 6 * g2;
+  const R* a1 = geom_aabb_of(m, e.state(), g1, e.env); const R* a2 = geom_aabb_of(m, e.state(), g2, e.env);
   R c1[3], c2[3], t[3];
   R o1[3] = {a1[0], a1[1], a1[2]}, o2[3] = {a2[0], a2[1], a2[2]};
   m3mulv(t, M1, o1); v3add(c1, t, e.p(e.lay().gpos) + 3 * k1);
@@ -964,16 +966,17 @@ template <typename R> DEV bool is_gjk_pair(int t1, int t2) {
 }
 
 // friction / condim mixing (equal priority: max; otherwise the higher-priority geom)
-template <typename R> DEV void mix_contact(const DModel<R>& m, int g1, int g2, R* fric3, int& dim) {
+template <typename R> DEV void mix_contact(const DModel<R>& m, const DState<R>& s, int env, int g1, int g2, R* fric3, int& dim) {
   int p1 = m.geom_priority[g1], p2 = m.geom_priority[g2];
+  const R* f1 = geom_friction_of(m, s, g1, env); const R* f2 = geom_friction_of(m, s, g2, env);
   if (p1 != p2) {
-    int g = p1 > p2 ? g1 : g2;
-    dim = m.geom_condim[g];
-    fric3[0] = m.geom_friction[3 * g]; fric3[1] = m.geom_friction[3 * g + 1]; fric3[2] = m.geom_friction[3 * g + 2];
+    const R* f = p1 > p2 ? f1 : f2;
+    dim = m.geom_condim[p1 > p2 ? g1 : g2];
+    fric3[0] = f[0]; fric3[1] = f[1]; fric3[2] = f[2];
     return;
   }
   dim = max(m.geom_condim[g1], m.geom_condim[g2]);
-  for (int k = 0; k < 3; k++) fric3[k] = r_max(m.geom_friction[3 * g1 + k], m.geom_friction[3 * g2 + k]);
+  for (int k = 0; k < 3; k++) fric3[k] = r_max(f1[k], f2[k]);
 }
 
 template <typename R> DEV int narrow_analytic(const Shape<R>& A, const Shape<R>& B, R* buf) {
@@ -993,6 +996,7 @@ template <typename R> DEV int narrow_analytic(const Shape<R>& A, const Shape<R>&
 // Cull the static pair list (bounding spheres, then oriented boxes); candidate pair indices in pair order.
 template <typename R> DEVN void cull_pairs(Eng<R> e, int* cand, int* cand_g, int maxa, int maxg, int& na_out, int& ng_out) {
   const DModel<R>& m = e.model();
+  const DState<R>& st = e.state();
   const WSLayout& L = e.lay();
   int lane = e.lane, na = 0, ng = 0;
   const R* gpos = e.p(L.gpos); const R* gmat = e.p(L.gmat);
@@ -1006,13 +1010,13 @@ template <typename R> DEVN void cull_pairs(Eng<R> e, int* cand, int* cand_g, int
       if (t1 != G_PLANE && t2 != G_PLANE) {
         R df[3];
         v3sub(df, gpos + 3 * k1, gpos + 3 * k2);
-        R bound = m.geom_rbound[g1] + m.geom_rbound[g2];
+        R bound = geom_rbound_of(m, st, g1, e.env) + geom_rbound_of(m, st, g2, e.env);
         pass = v3dot(df, df) <= bound * bound;
       } else {
         int kp = t1 == G_PLANE ? k1 : k2, ko = t1 == G_PLANE ? k2 : k1, go = t1 == G_PLANE ? g2 : g1;
         R nrm[3] = COLV(gmat + 9 * kp, 2), df[3];
         v3sub(df, gpos + 3 * ko, gpos + 3 * kp);
-        pass = v3dot(df, nrm) <= m.geom_rbound[go];
+        pass = v3dot(df, nrm) <= geom_rbound_of(m, st, go, e.env);
       }
       if (pass) pass = obb_overlap(e, g1, g2);
       isg = is_gjk_pair<R>(t1, t2);
@@ -1037,7 +1041,7 @@ template <typename R> DEV void finish_contacts(const Eng<R>& e, int ncon) {
   for (int c = e.lane; c < ncon; c += 32) {
     R f3[3];
     int dim;
-    mix_contact(m, cint[5 * c], cint[5 * c + 1], f3, dim);
+    mix_contact(m, e.state(), e.env, cint[5 * c], cint[5 * c + 1], f3, dim);
     cfric[3 * c] = f3[0]; cfric[3 * c + 1] = f3[1]; cfric[3 * c + 2] = f3[2];
     cint[5 * c + 2] = dim;
     cint[5 * c + 3] = -1;
@@ -1050,6 +1054,7 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
   long long tp0 = pc ? clock64() : 0;
 #define CTICK(slot) if (pc) { __syncwarp(); long long tp1 = clock64(); pc[slot] += (float)(tp1 - tp0); tp0 = tp1; }
   const DModel<R>& m = e.model();
+  const DState<R>& st = e.state();
   const WSLayout& L = e.lay();
   int lane = e.lane;
   int* cand = reinterpret_cast<int*>(e.p(L.scratch));  // candidate pair indices, analytic first then gjk
@@ -1067,13 +1072,13 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
       if (t1 != G_PLANE && t2 != G_PLANE) {
         R df[3];
         v3sub(df, gpos + 3 * k1, gpos + 3 * k2);
-        R bound = m.geom_rbound[g1] + m.geom_rbound[g2];
+        R bound = geom_rbound_of(m, st, g1, e.env) + geom_rbound_of(m, st, g2, e.env);
         pass = v3dot(df, df) <= bound * bound;
       } else {
         int kp = t1 == G_PLANE ? k1 : k2, ko = t1 == G_PLANE ? k2 : k1, go = t1 == G_PLANE ? g2 : g1;
         R nrm[3] = COLV(gmat + 9 * kp, 2), df[3];
         v3sub(df, gpos + 3 * ko, gpos + 3 * kp);
-        pass = v3dot(df, nrm) <= m.geom_rbound[go];
+        pass = v3dot(df, nrm) <= geom_rbound_of(m, st, go, e.env);
       }
       if (pass) pass = obb_overlap(e, g1, g2);
       isg = is_gjk_pair<R>(t1, t2);
@@ -1208,7 +1213,7 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
   for (int c = lane; c < ncon; c += 32) {
     R f3[3];
     int dim;
-    mix_contact(m, cint[5 * c], cint[5 * c + 1], f3, dim);
+    mix_contact(m, e.state(), e.env, cint[5 * c], cint[5 * c + 1], f3, dim);
     cfric[3 * c] = f3[0]; cfric[3 * c + 1] = f3[1]; cfric[3 * c + 2] = f3[2];
     cint[5 * c + 2] = dim;
     cint[5 * c + 3] = -1;

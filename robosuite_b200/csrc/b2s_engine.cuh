@@ -122,12 +122,50 @@ DEVN int spd_solve_blk(const R* A, int n, const R* dadd, R dscale, R* x, int lan
   return __any_sync(B2S_FULL, bad);
 }
 
+// ---- per-environment model values (b2s_model_override): the environment's override where one is declared, the model's value
+// otherwise.  A handle without overrides pays the test of n_mg / n_mb / a null pointer, uniform across the warp.
+template <typename R> DEV const R* geom_size_of(const DModel<R>& m, const DState<R>& s, int g, int env) {
+  for (int k = 0; k < s.n_mg; k++) if (s.mg_id[k] == g) return s.mg_size + 3 * ((size_t)k * s.n_env + env);
+  return m.geom_size + 3 * g;
+}
+template <typename R> DEV const R* geom_friction_of(const DModel<R>& m, const DState<R>& s, int g, int env) {
+  for (int k = 0; k < s.n_mg; k++) if (s.mg_id[k] == g) return s.mg_fric + 3 * ((size_t)k * s.n_env + env);
+  return m.geom_friction + 3 * g;
+}
+template <typename R> DEV R geom_rbound_of(const DModel<R>& m, const DState<R>& s, int g, int env) {
+  for (int k = 0; k < s.n_mg; k++) if (s.mg_id[k] == g) return s.mg_rbound[(size_t)k * s.n_env + env];
+  return m.geom_rbound[g];
+}
+template <typename R> DEV const R* geom_aabb_of(const DModel<R>& m, const DState<R>& s, int g, int env) {
+  for (int k = 0; k < s.n_mg; k++) if (s.mg_id[k] == g) return s.mg_aabb + 6 * ((size_t)k * s.n_env + env);
+  return m.geom_aabb + 6 * g;
+}
+template <typename R> DEV R body_mass_of(const DModel<R>& m, const DState<R>& s, int b, int env) {
+  for (int k = 0; k < s.n_mb; k++) if (s.mb_id[k] == b) return s.mb_mass[(size_t)k * s.n_env + env];
+  return m.body_mass[b];
+}
+template <typename R> DEV const R* body_inertia_of(const DModel<R>& m, const DState<R>& s, int b, int env) {
+  for (int k = 0; k < s.n_mb; k++) if (s.mb_id[k] == b) return s.mb_inertia + 3 * ((size_t)k * s.n_env + env);
+  return m.body_inertia + 3 * b;
+}
+// constants derived at qpos0 (the set-constants pass writes them per environment once a handle declares an override)
+template <typename R> DEV const R* dof_invweight0_of(const DModel<R>& m, const DState<R>& s, int env) {
+  return s.dof_iw ? s.dof_iw + (size_t)env * m.nv : m.dof_invweight0;
+}
+template <typename R> DEV const R* body_invweight0_of(const DModel<R>& m, const DState<R>& s, int env) {
+  return s.body_iw ? s.body_iw + (size_t)env * 2 * m.nbody : m.body_invweight0;
+}
+template <typename R> DEV R meaninertia_of(const DModel<R>& m, const DState<R>& s, int env) {
+  return s.mean_inertia ? s.mean_inertia[env] : m.meaninertia;
+}
+
 template <typename R>
 struct Eng {
   R* ws;  // this warp's workspace
   int lane;
   int slot, lid;  // descriptor slot of the owning handle, workspace layout of the running kernel (LAY_*)
-  int env = 0;    // environment index (set by the kernels that run kinematics: per-environment poses of world-welded bodies)
+  int env = 0;    // environment index (per-environment poses of world-welded bodies and model overrides): set by every stage that
+                  // starts an environment (kinematics, the tail's rows)
 
   DEV Eng(R* ws_, int lane_, int slot_, int lid_) : ws(ws_), lane(lane_), slot(slot_), lid(lid_) {}
   DEV const DModel<R>& model() const { return cmodel<R>(slot); }
@@ -235,6 +273,9 @@ struct Eng {
     // per body: inertial frame origin + spatial inertia about the world origin
     R* xipos = p(L.xipos); R* cinert = p(L.cinert);
     for (int b = lane; b < m.nbody; b += 32) {
+      // the override lookups come first: the arithmetic below stays in one basic block, where nvcc forms the same FMAs as without them
+      const R* bi = body_inertia_of(m, state(), b, env);
+      const R mass = body_mass_of(m, state(), b, env);
       R ip[3] = {m.body_ipos[3 * b], m.body_ipos[3 * b + 1], m.body_ipos[3 * b + 2]};
       R c[3], qi[4], Ri[9];
       m3mulv(c, xmat + 9 * b, ip);
@@ -243,7 +284,7 @@ struct Eng {
       R iq[4] = {m.body_iquat[4 * b], m.body_iquat[4 * b + 1], m.body_iquat[4 * b + 2], m.body_iquat[4 * b + 3]};
       qmul(qi, xquat + 4 * b, iq);
       q2mat(Ri, qi);
-      R I0 = m.body_inertia[3 * b], I1 = m.body_inertia[3 * b + 1], I2 = m.body_inertia[3 * b + 2], mass = m.body_mass[b];
+      R I0 = bi[0], I1 = bi[1], I2 = bi[2];
       R* ci = cinert + 10 * b;
       R cc = v3dot(c, c);
 #define IW(r, s) (Ri[3 * r] * I0 * Ri[3 * s] + Ri[3 * r + 1] * I1 * Ri[3 * s + 1] + Ri[3 * r + 2] * I2 * Ri[3 * s + 2])
@@ -365,9 +406,10 @@ struct Eng {
       for (int e = 0; e < 6; e++) frne[6 * b + e] = Ia[e] + x[e];
       // fluid (inertia-box model); result as spatial force about the world origin
       R ff[6] = {0, 0, 0, 0, 0, 0};
-      R mass = m.body_mass[b];
+      R mass = body_mass_of(m, state(), b, env);
       if (b > 0 && mass >= Lim<R>::minval() && (m.density > 0 || m.viscosity > 0)) {
-        R I0 = m.body_inertia[3 * b], I1 = m.body_inertia[3 * b + 1], I2 = m.body_inertia[3 * b + 2];
+        const R* bi = body_inertia_of(m, state(), b, env);
+        R I0 = bi[0], I1 = bi[1], I2 = bi[2];
         R box[3];
         box[0] = r_sqrt(r_max(Lim<R>::minval(), I1 + I2 - I0) / mass * R(6));
         box[1] = r_sqrt(r_max(Lim<R>::minval(), I0 + I2 - I1) / mass * R(6));

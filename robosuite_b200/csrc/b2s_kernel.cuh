@@ -213,6 +213,115 @@ __global__ void reset_envs_kernel(const uint8_t* mask, const R* qpos_new, int sl
   if (s.obs_fresh) s.obs_fresh[env] = 1;
 }
 
+// ---- set-constants pass (b2s_set_const): the compiler's _set_const (mjcf/compiler.py) for the masked environments, one warp each,
+// from the environment's own masses, moments and sizes.  Kinematics and CRB at qpos0 (world-pose overrides honoured) give M, then
+//   meaninertia       = mean diag(M)
+//   dof_invweight0    = diag(M^-1), averaged over the translational and the rotational block of each free joint
+//   body_invweight0   = (mean translational, mean rotational) diagonal of J M^-1 J^T, J = Jacobian of the body's centre of mass
+// and every overridden geom gets its bounding radius and local box from its size (the compiler's per-type rules).  Override values
+// that are non-finite or non-positive, or moments that violate the triangle inequality, set warn bit 128.
+// Workspace per warp: the fused layout followed by nv * nv words for M^-1 (`stride` words in all).
+template <typename R>
+__global__ void __launch_bounds__(512, 1) set_const_kernel(const uint8_t* mask, int slot, int stride) {
+  const DModel<R>& m = cmodel<R>(slot);
+  const DState<R>& s = cstate<R>(slot);
+  const WSLayout& L = c_lay[slot][LAY_FULL];
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  const int env = blockIdx.x * wpb + warp;
+  if (env >= s.n_env || (mask && !mask[env])) return;
+  Eng<R> e(reinterpret_cast<R*>(smem_raw) + (size_t)warp * stride, lane, slot, LAY_FULL);
+  e.env = env;
+  const int nv = m.nv, nb = m.nbody;
+  const size_t E = env;
+  auto pos = [](R v) { return isfinite(v) && v > R(0); };
+  int bad = 0;
+  for (int k = lane; k < s.n_mg; k += 32) {
+    const size_t o = (size_t)k * s.n_env + E;
+    const int t = m.geom_type[s.mg_id[k]];
+    const R* sz = s.mg_size + 3 * o;
+    const R* fr = s.mg_fric + 3 * o;
+    const int nsz = t == G_SPHERE ? 1 : (t == G_CAPSULE || t == G_CYLINDER ? 2 : 3);
+    for (int q = 0; q < 3; q++) if (!pos(fr[q]) || (q < nsz && !pos(sz[q]))) bad = 1;
+    R r = sz[0], h = sz[1], rb, hx = r, hy = r, hz = r;
+    if (t == G_SPHERE) rb = r;
+    else if (t == G_CAPSULE) { rb = r + h; hz = r + h; }
+    else if (t == G_CYLINDER) { rb = r_sqrt(r * r + h * h); hz = h; }
+    else {  // ellipsoid, box
+      hx = sz[0]; hy = sz[1]; hz = sz[2];
+      rb = t == G_ELLIPSOID ? r_max(r_max(hx, hy), hz) : r_sqrt(hx * hx + hy * hy + hz * hz);
+    }
+    s.mg_rbound[o] = rb;
+    R* a = s.mg_aabb + 6 * o;
+    a[0] = 0; a[1] = 0; a[2] = 0; a[3] = hx; a[4] = hy; a[5] = hz;
+  }
+  for (int k = lane; k < s.n_mb; k += 32) {
+    const size_t o = (size_t)k * s.n_env + E;
+    const R* I = s.mb_inertia + 3 * o;
+    if (!pos(s.mb_mass[o]) || !pos(I[0]) || !pos(I[1]) || !pos(I[2]) || I[0] + I[1] < I[2] || I[0] + I[2] < I[1] || I[1] + I[2] < I[0]) bad = 1;
+  }
+  bad = warp_or_i(bad);
+  if (bad && lane == 0) s.warn[env] |= 128;
+  // M at qpos0
+  for (int i = lane; i < m.nq; i += 32) e.p(L.qpos)[i] = m.qpos0[i];
+  for (int i = lane; i < nv; i += 32) e.p(L.qvel)[i] = 0;
+  __syncwarp();
+  e.kinematics();
+  e.crb();
+  const R* M = e.p(L.M);
+  R tr = 0;
+  for (int i = 0; i < nv; i++) tr += M[i * nv + i];
+  if (lane == 0) s.mean_inertia[env] = nv > 0 ? tr / R(nv) : R(1);
+  // M^-1, column by column from one Cholesky factor (in H)
+  R* H = e.p(L.H); R* x = e.p(L.grad); R* Mi = e.ws + L.total;
+  for (int k = lane; k < nv * nv; k += 32) H[k] = M[k];
+  __syncwarp();
+  e.chol(H, nv);
+  for (int c = 0; c < nv; c++) {
+    for (int i = lane; i < nv; i += 32) x[i] = i == c ? R(1) : R(0);
+    __syncwarp();
+    e.chol_solve(H, x, nv);
+    for (int i = lane; i < nv; i += 32) Mi[i * nv + c] = x[i];
+    __syncwarp();
+  }
+  for (int i = lane; i < nv; i += 32) {
+    int j = m.dof_jntid[i], b = i;
+    R v = Mi[i * nv + i];
+    if (m.jnt_type[j] == JNT_FREE) {
+      b = m.jnt_dofadr[j] + (i - m.jnt_dofadr[j] < 3 ? 0 : 3);
+      v = (Mi[b * nv + b] + Mi[(b + 1) * nv + b + 1] + Mi[(b + 2) * nv + b + 2]) / R(3);
+    }
+    s.dof_iw[E * nv + i] = v;
+  }
+  const R* cdof = e.p(L.cdof); const R* xipos = e.p(L.xipos);
+  for (int b = lane; b < nb; b += 32) {
+    R at = 0, ar = 0;
+    if (b > 0 && m.body_weldid[b] != 0) {
+      const R* p = xipos + 3 * b;
+      const unsigned long long chain = m.body_dofmask[b];
+      for (int i = 0; i < nv; i++) {
+        if (!((chain >> i) & 1ull)) continue;
+        const R* ci = cdof + 6 * i;
+        R pi[3];
+        v3cross(pi, ci, p);
+        pi[0] += ci[3]; pi[1] += ci[4]; pi[2] += ci[5];
+        for (int j = 0; j < nv; j++) {
+          if (!((chain >> j) & 1ull)) continue;
+          const R* cj = cdof + 6 * j;
+          R pj[3];
+          v3cross(pj, cj, p);
+          pj[0] += cj[3]; pj[1] += cj[4]; pj[2] += cj[5];
+          const R w = Mi[i * nv + j];
+          at += w * v3dot(pi, pj);
+          ar += w * v3dot(ci, cj);
+        }
+      }
+    }
+    s.body_iw[(E * nb + b) * 2] = at / R(3);
+    s.body_iw[(E * nb + b) * 2 + 1] = ar / R(3);
+  }
+}
+
 template <typename R>
 __global__ void reset_kernel(const uint8_t* mask, int slot) {
   const DModel<R>& m = cmodel<R>(slot);

@@ -123,14 +123,15 @@ struct P1Cfg { int nG, nC, sub; };
 
 // ---- one narrow-phase pair of an environment, for the phase-1 roles and the unit queue alike: geoms in type order (what the fused
 // collide produces), shapes from the environment's workspace row, contact count + records -> the output record `out`
-template <typename R> DEV void narrow_pair_analytic(int slot, const R* row, int pidx, R* out) {
+template <typename R> DEV void narrow_pair_analytic(int slot, int env, const R* row, int pidx, R* out) {
   const DModel<R>& m = cmodel<R>(slot);
+  const DState<R>& s = cstate<R>(slot);
   const WSLayout& RL = c_lay[slot][LAY_ROW];
   int g1 = m.pair_geom[2 * pidx], g2 = m.pair_geom[2 * pidx + 1];
   if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
   Shape<R> A, B;
-  shape_from(m, g1, row + RL.gpos, row + RL.gmat, A);
-  shape_from(m, g2, row + RL.gpos, row + RL.gmat, B);
+  shape_from(m, s, env, g1, row + RL.gpos, row + RL.gmat, A);
+  shape_from(m, s, env, g2, row + RL.gpos, row + RL.gmat, B);
   R buf[8 * CREC];
   int n = narrow_analytic(A, B, buf);
   out[0] = R(n);
@@ -147,8 +148,8 @@ DEV void narrow_pair_convex(int slot, int env, const R* row, int pidx, R* out, R
   int g1 = m.pair_geom[2 * pidx], g2 = m.pair_geom[2 * pidx + 1];
   if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
   Shape<R> A, B;
-  shape_from(m, g1, row + RL.gpos, row + RL.gmat, A);
-  shape_from(m, g2, row + RL.gpos, row + RL.gmat, B);
+  shape_from(m, s, env, g1, row + RL.gpos, row + RL.gmat, A);
+  shape_from(m, s, env, g2, row + RL.gpos, row + RL.gmat, B);
   R buf[CREC];
 #ifdef B2S_INSTR
   long long it0 = clock64();
@@ -189,7 +190,7 @@ template <typename R> DEV void narrow_analytic_block(const Grp& g, int rb) {
   tid += g.env0 * s.cl_maxa;  // this group's slice of the candidate list / output slots
   int code = s.cl_listA[tid];
   int env = code >> 12;
-  narrow_pair_analytic(g.slot, s.wsg + (size_t)env * RL.total, code & 4095, s.cl_outA + (size_t)tid * CL_RECA);
+  narrow_pair_analytic(g.slot, env, s.wsg + (size_t)env * RL.total, code & 4095, s.cl_outA + (size_t)tid * CL_RECA);
 }
 
 // convex pairs: ONE WARP per candidate pair (mesh support scans split over the lanes).  The block owns one EPA polytope and the
@@ -372,6 +373,7 @@ template <typename R> DEV int tail_rows(Eng<R>& e, int env, unsigned long long* 
   const int lane = e.lane;
   const bool tiered = L.mc < m.maxcon || L.me < m.maxefc;
   const size_t E = env;
+  e.env = env;
   const R* row = s.wsg + E * RL.total;
   const int warn = reinterpret_cast<const int*>(row + RL.hdr)[2];  // phase 0: divergence reset, candidate-list overflow
   ws_load(e, row, c_pio[e.slot][e.lid == LAY_TL ? PIO_TL : PIO_TS], bar, parity);

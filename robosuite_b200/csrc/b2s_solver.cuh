@@ -194,17 +194,18 @@ template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn, fl
       solref[0] = m.dof_solref[2 * id]; solref[1] = m.dof_solref[2 * id + 1];
       B2S_LOOP
       for (int q = 0; q < 5; q++) solimp[q] = m.dof_solimp[5 * id + q];
-      diag = m.dof_invweight0[id];
+      diag = dof_invweight0_of(m, e.state(), e.env)[id];
     } else if (type == C_LIMIT) {
       solref[0] = m.jnt_solref[2 * id]; solref[1] = m.jnt_solref[2 * id + 1];
       B2S_LOOP
       for (int q = 0; q < 5; q++) solimp[q] = m.jnt_solimp[5 * id + q];
-      diag = m.dof_invweight0[m.jnt_dofadr[id]];
+      diag = dof_invweight0_of(m, e.state(), e.env)[m.jnt_dofadr[id]];
     } else {
       int g1 = cint[5 * id], g2 = cint[5 * id + 1], k = r - cint[5 * id + 3];
       first = k == 0;
       int b1 = m.geom_bodyid[g1], b2 = m.geom_bodyid[g2];
-      diag = k < 3 ? m.body_invweight0[2 * b1] + m.body_invweight0[2 * b2] : m.body_invweight0[2 * b1 + 1] + m.body_invweight0[2 * b2 + 1];
+      const R* biw = body_invweight0_of(m, e.state(), e.env);
+      diag = k < 3 ? biw[2 * b1] + biw[2 * b2] : biw[2 * b1 + 1] + biw[2 * b2 + 1];
       // solref / solimp mixing (solmix-weighted)
       R s1 = m.geom_solmix[g1], s2 = m.geom_solmix[g2], mix;
       int p1 = m.geom_priority[g1], p2 = m.geom_priority[g2];
@@ -432,7 +433,7 @@ template <typename R> DEVN int solve(Eng<R> e, int nefc, int ncon, int& warn) {
   const int* cint = e.pi(L.c_int);
   const int* eint = e.pi(L.e_int);
   R* act = e.p(L.scratch); R* Hcb = e.p(L.scratch) + L.me;
-  R scale = R(1) / (m.meaninertia * R(nv > 1 ? nv : 1));
+  R scale = R(1) / (meaninertia_of(m, e.state(), e.env) * R(nv > 1 ? nv : 1));
   int first_contact_row = nefc;
   B2S_LOOP
   for (int c = 0; c < ncon; c++) { int a = cint[5 * c + 3]; if (a >= 0) { first_contact_row = a; break; } }

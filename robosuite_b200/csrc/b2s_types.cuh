@@ -6,6 +6,7 @@
 #include <stdint.h>
 
 #define B2S_FULL 0xffffffffu
+#define B2S_MOV 8  // per-handle cap of b2s_model_override: geoms, and separately bodies
 
 enum { JNT_FREE = 0, JNT_BALL = 1, JNT_SLIDE = 2, JNT_HINGE = 3 };
 enum { G_PLANE = 0, G_HFIELD, G_SPHERE, G_CAPSULE, G_ELLIPSOID, G_CYLINDER, G_BOX, G_MESH };
@@ -98,6 +99,14 @@ struct DState {
   int n_ov, ov_body[4];
   R* ov_pos[4];    // [n_env, 3]
   R* ov_quat[4];   // [n_env, 4]
+  // per-environment model values (b2s_model_override): up to B2S_MOV colliding primitive geoms (size, friction) and B2S_MOV moving
+  // bodies (mass, principal moments).  Slot k of environment e sits at [k * n_env + e].  n_mg == n_mb == 0 and null derived
+  // arrays: the handle has no overrides and every lookup (b2s_engine.cuh, *_of) costs one warp-uniform test.
+  int n_mg, n_mb;
+  short mg_id[B2S_MOV], mb_id[B2S_MOV];
+  R *mg_size, *mg_fric, *mg_rbound, *mg_aabb;  // [B2S_MOV][n_env] x 3 / 3 / 1 / 6 (rbound, aabb: written by the set-constants pass)
+  R *mb_mass, *mb_inertia;                     // [B2S_MOV][n_env] x 1 / 3
+  R *dof_iw, *body_iw, *mean_inertia;          // [n_env] x nv / nbody * 2 / 1: dof_invweight0, body_invweight0, meaninertia
   R* task_vec;     // [n_env, task_dim] task table values after the last substep
   R* task_out;     // [n_env, 8]: body height, |grip site - body|, grasp flag, horizontal |body - body2|, obj-obj2 contact flag
   // -DB2S_INSTR builds only (measurement aid, see b2s_instr in b2s_pipeline.cuh): device timeline of the graph replay and

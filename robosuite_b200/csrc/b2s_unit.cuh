@@ -70,7 +70,7 @@ template <typename R> DEVN void unit_narrow(R* area, int area_words, int lane, i
   const int* tab = s.cl_env + E * CL_ENVW(s);
   for (int base = 0; base < na; base += 32) {
     int i = base + lane;
-    if (i < na) narrow_pair_analytic(slot, row, tab[2 + 2 * i], s.cl_outA + (E * s.cl_maxa + i) * CL_RECA);
+    if (i < na) narrow_pair_analytic(slot, env, row, tab[2 + 2 * i], s.cl_outA + (E * s.cl_maxa + i) * CL_RECA);
   }
   __syncwarp();
   const int stage_cap = area_words - EPA_PIPE_WORDS;
@@ -93,8 +93,9 @@ template <typename R> DEVN int unit_tail_acc(R* area, int lane, int slot) {
   Eng<R> e(area, lane, slot, LAY_TS);
   return tail_accel(e);
 }
-template <typename R> DEVN int unit_tail_solve(R* area, int lane, int slot, int nefc, int ncon) {
+template <typename R> DEVN int unit_tail_solve(R* area, int lane, int slot, int env, int nefc, int ncon) {
   Eng<R> e(area, lane, slot, LAY_TS);
+  e.env = env;
   return tail_newton(e, nefc, ncon);
 }
 template <typename R>
@@ -261,7 +262,7 @@ __global__ void __launch_bounds__(B2S_LBU_THREADS, B2S_LBU_BLOCKS) unit_kernel(i
     if (live) warn |= unit_tail_acc<R>(area, lane, slot);
     __syncthreads();
     UTICK(6)
-    if (live) warn |= unit_tail_solve<R>(area, lane, slot, nefc, ncon);
+    if (live) warn |= unit_tail_solve<R>(area, lane, slot, env, nefc, ncon);
     __syncthreads();
     UTICK(7)
     if (live) {

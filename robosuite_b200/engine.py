@@ -68,6 +68,8 @@ def lib():
         L.b2s_env_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
         L.b2s_reset_envs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.b2s_body_pose_override.argtypes = [C.c_void_p, C.c_int]
+        L.b2s_model_override.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
+        L.b2s_set_const.argtypes = [C.c_void_p, C.c_void_p]
         L.b2s_obs_config.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.b2s_task_config.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.b2s_task_config2.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
@@ -225,6 +227,19 @@ class BatchedSim:
         (b2s_body_pose_override; the reference writes model.body_pos / body_quat per reset, door.py:417-427)"""
         self._check(self._L.b2s_body_pose_override(self._h, int(body_id)))
         return self.array("body_xpos_ov:%d" % body_id), self.array("body_xquat_ov:%d" % body_id)
+
+    def model_override(self, field, obj_id):
+        """[n_env, ...] tensor of per-environment values of one model field for one object (b2s_model_override): "geom_size" /
+        "geom_friction" [n_env, 3] of a colliding primitive geom, "body_mass" [n_env] / "body_inertia" [n_env, 3] (principal moments in
+        the model's inertial frame) of a moving body.  Starts at the model's values.  The constants derived from these values
+        (dof_invweight0, body_invweight0, meaninertia, the geom's bounding radius and box) follow at the next set_const() or reset."""
+        self._check(self._L.b2s_model_override(self._h, field.encode(), int(obj_id)))
+        return self.array("%s:%d" % (field, obj_id))
+
+    def set_const(self, mask=None):
+        """recompute the derived constants of the masked environments (uint8 [n_env] device mask, None = all) from their
+        per-environment model values, on the device (b2s_set_const); warn bit 128 marks invalid values"""
+        self._check(self._L.b2s_set_const(self._h, None if mask is None else C.c_void_p(mask.data_ptr())))
 
     def ctrl_reset(self, mask=None):
         self._check(self._L.b2s_ctrl_reset(self._h, None if mask is None else C.c_void_p(mask.data_ptr())))

@@ -96,7 +96,9 @@ class ObsBuilder:
 SIM_WARN_BITS = {1: "singular mass matrix", 2: "non-finite state in the integrator", 4: "contact capacity overflow (maxcon)",
                  8: "constraint-row capacity overflow (maxefc)", 16: "singular Newton Hessian",
                  32: "diverged state (non-finite / huge qpos, qvel or qacc): data reset to the model defaults, as mj_checkPos/Vel/Acc do",
-                 64: "unit-queue watchdog fired: the control step is incomplete (mode 2 only; a library bug, please report)"}
+                 64: "unit-queue watchdog fired: the control step is incomplete (mode 2 only; a library bug, please report)",
+                 128: "invalid model override (non-finite or non-positive size, friction, mass or moment, or moments violating the "
+                      "triangle inequality)"}
 
 
 class BatchedMujocoEnv:
@@ -126,6 +128,7 @@ class BatchedMujocoEnv:
         self.ignore_done = ignore_done
         self.reward_scale = reward_scale
         self.reward_shaping = reward_shaping
+        self.hard_reset = hard_reset
         self.use_object_obs = use_object_obs
         self.initialization_noise = {"magnitude": 0.02, "type": "gaussian"} if initialization_noise == "default" \
             else (initialization_noise or {"magnitude": 0.0, "type": "gaussian"})

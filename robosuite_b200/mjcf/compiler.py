@@ -160,6 +160,48 @@ class Model:
 
 
 # ----------------------------------------------------------------------------------------------- compile
+def primitive_geom_props(t, sz):
+    """(volume, inertia diagonal per unit mass in the geom frame, bounding radius, local box [centre 3, half sizes 3]) of a primitive
+    geom of type t and size sz.  The set-constants pass (b2s_set_const) applies the same bound rules to per-environment sizes."""
+    vol, I, rbound, aabb = 0.0, np.zeros(3), 0.0, [0, 0, 0, 0, 0, 0]
+    if t == GEOM_SPHERE:
+        r = sz[0]
+        vol = 4.0 / 3.0 * math.pi * r ** 3
+        I[:] = 0.4 * r * r
+        rbound = r
+        aabb = [0, 0, 0, r, r, r]
+    elif t == GEOM_BOX:
+        vol = 8 * sz[0] * sz[1] * sz[2]
+        I = np.array([sz[1] ** 2 + sz[2] ** 2, sz[0] ** 2 + sz[2] ** 2, sz[0] ** 2 + sz[1] ** 2]) / 3.0
+        rbound = np.linalg.norm(sz)
+        aabb = [0, 0, 0, sz[0], sz[1], sz[2]]
+    elif t == GEOM_CYLINDER:
+        r, h = sz[0], sz[1]
+        vol = math.pi * r * r * 2 * h
+        I = np.array([(3 * r * r + 4 * h * h) / 12.0, (3 * r * r + 4 * h * h) / 12.0, r * r / 2.0])
+        rbound = math.sqrt(r * r + h * h)
+        aabb = [0, 0, 0, r, r, h]
+    elif t == GEOM_CAPSULE:
+        r, h = sz[0], sz[1]
+        vc = math.pi * r * r * 2 * h
+        vs = 4.0 / 3.0 * math.pi * r ** 3
+        vol = vc + vs
+        izz = (vc * r * r / 2 + vs * 0.4 * r * r) / vol
+        ixx = (vc * (3 * r * r + 4 * h * h) / 12 + vs * (0.4 * r * r + h * h + 0.75 * r * h)) / vol
+        I = np.array([ixx, ixx, izz])
+        rbound = r + h
+        aabb = [0, 0, 0, r, r, r + h]
+    elif t == GEOM_ELLIPSOID:
+        vol = 4.0 / 3.0 * math.pi * sz[0] * sz[1] * sz[2]
+        I = np.array([sz[1] ** 2 + sz[2] ** 2, sz[0] ** 2 + sz[2] ** 2, sz[0] ** 2 + sz[1] ** 2]) / 5.0
+        rbound = sz.max()
+        aabb = [0, 0, 0, sz[0], sz[1], sz[2]]
+    elif t == GEOM_PLANE:
+        rbound = 0.0
+        aabb = [0, 0, -1e10, 1e10, 1e10, 1e10]
+    return vol, I, rbound, aabb
+
+
 def compile_mjcf(xml_string: str, mesh_root: str = None) -> Model:
     from ..errors import XMLError
 
@@ -446,45 +488,12 @@ def compile_mjcf(xml_string: str, mesh_root: str = None) -> Model:
                 sz[2] = half
         g["size"][i], g["pos"][i], g["quat"][i] = sz, pos, quat
         density = float(el.get("density", 1000))
-        vol, I = 0.0, np.zeros(3)
-        if t == GEOM_SPHERE:
-            r = sz[0]
-            vol = 4.0 / 3.0 * math.pi * r ** 3
-            I[:] = 0.4 * r * r
-            g["rbound"][i] = r
-            g["aabb"][i] = [0, 0, 0, r, r, r]
-        elif t == GEOM_BOX:
-            vol = 8 * sz[0] * sz[1] * sz[2]
-            I = np.array([sz[1] ** 2 + sz[2] ** 2, sz[0] ** 2 + sz[2] ** 2, sz[0] ** 2 + sz[1] ** 2]) / 3.0
-            g["rbound"][i] = np.linalg.norm(sz)
-            g["aabb"][i] = [0, 0, 0, sz[0], sz[1], sz[2]]
-        elif t == GEOM_CYLINDER:
-            r, h = sz[0], sz[1]
-            vol = math.pi * r * r * 2 * h
-            I = np.array([(3 * r * r + 4 * h * h) / 12.0, (3 * r * r + 4 * h * h) / 12.0, r * r / 2.0])
-            g["rbound"][i] = math.sqrt(r * r + h * h)
-            g["aabb"][i] = [0, 0, 0, r, r, h]
-        elif t == GEOM_CAPSULE:
-            r, h = sz[0], sz[1]
-            vc = math.pi * r * r * 2 * h
-            vs = 4.0 / 3.0 * math.pi * r ** 3
-            vol = vc + vs
-            izz = (vc * r * r / 2 + vs * 0.4 * r * r) / vol
-            ixx = (vc * (3 * r * r + 4 * h * h) / 12 + vs * (0.4 * r * r + h * h + 0.75 * r * h)) / vol
-            I = np.array([ixx, ixx, izz])
-            g["rbound"][i] = r + h
-            g["aabb"][i] = [0, 0, 0, r, r, r + h]
-        elif t == GEOM_ELLIPSOID:
-            vol = 4.0 / 3.0 * math.pi * sz[0] * sz[1] * sz[2]
-            I = np.array([sz[1] ** 2 + sz[2] ** 2, sz[0] ** 2 + sz[2] ** 2, sz[0] ** 2 + sz[1] ** 2]) / 5.0
-            g["rbound"][i] = sz.max()
-            g["aabb"][i] = [0, 0, 0, sz[0], sz[1], sz[2]]
-        elif t == GEOM_PLANE:
-            g["rbound"][i] = 0.0
-            g["aabb"][i] = [0, 0, -1e10, 1e10, 1e10, 1e10]
-        elif t == GEOM_MESH:
+        if t == GEOM_MESH:
+            vol, I = 0.0, np.zeros(3)
             mid = mesh_names.index(el.get("mesh"))
             g["dataid"][i] = mid
+        else:
+            vol, I, g["rbound"][i], g["aabb"][i] = primitive_geom_props(t, sz)
         Il = np.diag(I)
         if t == GEOM_MESH:
             md = get_mesh(g["dataid"][i])
