@@ -126,7 +126,13 @@ int b2s_body_pose_override(b2s_sim* sim, int body_id);
  *   "geom_friction" [n_env, 3]  same geoms
  *   "body_mass"     [n_env]     moving bodies
  *   "body_inertia"  [n_env, 3]  moving bodies: principal moments in the model's inertial frame (body_ipos / body_iquat stay shared)
- * A declared geom also gets "geom_rbound:<id>" [n_env] and "geom_aabb:<id>" [n_env, 6]; the first declaration of a handle creates
+ *   "dof_damping", "dof_armature", "dof_frictionloss"  [n_env, nv]  id must be -1 (the whole vector); the array is named "<field>".
+ *       Damping enters the passive force and the implicit Euler step, armature the mass matrix (and so the derived constants).
+ *       Once "dof_frictionloss" is declared, an environment's friction-loss rows are its dofs whose own value is > 0, in dof order;
+ *       it needs opt_maxefc >= nv + 8 (B2S_ERR_UNSUPPORTED otherwise).
+ * A declared geom (geom_size or geom_friction) also gets "geom_rbound:<id>" [n_env] and "geom_aabb:<id>" [n_env, 6], and its contact
+ * parameters "geom_solref:<id>" [n_env, 2] and "geom_solimp:<id>" [n_env, 5], initialised to the model's and read by the contact
+ * solref / solimp mixing of every step (they are not fields of their own: they come with the geom's slot).  The first declaration of a handle creates
  * "dof_invweight0" [n_env, nv], "body_invweight0" [n_env, nbody, 2] and "meaninertia" [n_env].  These DERIVED constants start at the
  * model's values and are STALE after a change until b2s_set_const or b2s_reset / b2s_reset_envs (which run the same pass for their
  * masked environments whenever the handle has overrides) recomputes them.  Returns B2S_ERR_ARG for an unknown field or an id out of
@@ -136,9 +142,26 @@ int b2s_model_override(b2s_sim* sim, const char* field, int id);
 /* The set-constants pass for the masked environments (env_mask: n_env device bytes, NULL = all), one warp each, on the handle's
  * stream: kinematics and composite inertia at qpos0 (world-pose overrides honoured) -> dof_invweight0, body_invweight0, meaninertia
  * (the compiler's definitions), and the bounding radius / box of every overridden geom from its size.  Environments whose override
- * values are non-finite or non-positive, or whose moments violate the triangle inequality, get warn bit 128.  No-op on a handle
- * without overrides. */
+ * values are non-finite or non-positive (damping, armature, friction loss: non-finite or negative), whose solref / solimp has a
+ * non-finite component, or whose moments violate the triangle inequality, get warn bit 128.  No-op on a handle without overrides. */
 int b2s_set_const(b2s_sim* sim, const uint8_t* env_mask);
+
+/* Device perturbation of declared override arrays (dynamics randomisation, the batched counterpart of the reference's DynamicsModder,
+ * utils/mjmod.py).  b2s_perturb_config copies a list of (field, id) entries once (n = 0 clears it); every field must already be
+ * declared with b2s_model_override.  For the dof fields id -1 perturbs every dof and a dof index that dof alone.
+ * b2s_perturb_model then writes every entry of the masked environments (env_mask: n_env device bytes, NULL = all) in ONE launch on the
+ * handle's stream, without host data, drawing around the MODEL's value (repeated calls do not random-walk):
+ *   B2S_PERTURB_SCALE: v = v_model * (1 + d)     B2S_PERTURB_SHIFT: v = max(0, v_model + d)     d ~ U(-amplitude, amplitude)
+ * one_draw = 1 uses one draw for all components of the entry (body_inertia: keeps the triangle inequality).  d comes from
+ * Philox4x32-10 with key = seed and counter = (env, counter, entry index, component; 0 with one_draw), u = 53 bits of the first two
+ * output words ((w0 >> 5) * 2^26 + (w1 >> 6)) / 2^53, d = amplitude * (2u - 1) in fp64, rounded to the handle's precision last:
+ * an environment's values depend only on (seed, counter, env, spec).  The derived constants are NOT updated: they follow at the next
+ * b2s_set_const or reset.  B2S_ERR_ARG: undeclared field, negative or non-finite amplitude, amplitude >= 1 in scale mode, counter
+ * >= 2^32.  Without a configuration b2s_perturb_model does nothing. */
+enum { B2S_PERTURB_SCALE = 0, B2S_PERTURB_SHIFT = 1 };
+typedef struct { const char* field; int id; int mode; double amplitude; int one_draw; } b2s_perturb;
+int b2s_perturb_config(b2s_sim* sim, const b2s_perturb* spec_host, int n);
+int b2s_perturb_model(b2s_sim* sim, const uint8_t* env_mask, uint64_t seed, uint64_t counter);
 
 /* Observation program = MujocoEnv._get_observations flattened (environments/base.py:429-465): one (op, a, b) entry
  * per output scalar (ops: enum OB_* in csrc/b2s_types.cuh; OB_REL_*_LAG entries read the previous sample, as the reference's

@@ -3,6 +3,7 @@
 #include "../../include/b2s.h"
 #include "b2s_unit.cuh"
 
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -96,8 +97,13 @@ struct b2s_sim {
   // model values that b2s_model_override copies per environment, and the host-computed constants derived from them
   std::vector<int> geom_type_h;
   std::vector<double> geom_size_h, geom_friction_h, geom_rbound_h, geom_aabb_h, body_mass_h, body_inertia_h, dof_iw_h, body_iw_h;
+  std::vector<double> geom_solref_h, geom_solimp_h, dof_damping_h, dof_armature_h, dof_frictionloss_h;
   double meaninertia_h = 1;
   int sc_words = 0;  // set-constants pass: words of shared memory per warp (0 until its first launch)
+  // b2s_perturb_config: entry and item tables on the device (perturb_kernel), items per environment (0 = not configured)
+  PerturbEntry* pert_ent = nullptr;
+  PerturbItem* pert_item = nullptr;
+  int pert_nitems = 0;
 };
 
 static int launch_set_const(b2s_sim* s, const uint8_t* mask);  // the set-constants pass (no-op without model overrides)
@@ -274,6 +280,8 @@ template <typename R> static void build_model(b2s_sim* s, const Blob& b, DModel<
     host("geom_size", s->geom_size_h); host("geom_friction", s->geom_friction_h); host("geom_rbound", s->geom_rbound_h);
     host("geom_aabb", s->geom_aabb_h); host("body_mass", s->body_mass_h); host("body_inertia", s->body_inertia_h);
     host("dof_invweight0", s->dof_iw_h); host("body_invweight0", s->body_iw_h);
+    host("geom_solref", s->geom_solref_h); host("geom_solimp", s->geom_solimp_h); host("dof_damping", s->dof_damping_h);
+    host("dof_armature", s->dof_armature_h); host("dof_frictionloss", s->dof_frictionloss_h);
     s->meaninertia_h = b.scalar_f("stat_meaninertia");
     const int* gt = b.i32("geom_type"); s->geom_type_h.assign(gt, gt + ng);
   }
@@ -1333,14 +1341,25 @@ template <typename R> static void upload_rows(R* dst, const double* src, int k, 
   cudaStreamSynchronize(cudaStreamLegacy);  // see dev_upload
 }
 
+// geom fields a caller declares; declaring either one gives the geom a slot, and the slot also carries the geom's contact solref /
+// solimp ("geom_solref:<id>", "geom_solimp:<id>"), as it carries its bounding radius and box
+static bool is_geom_decl_field(const std::string& f) { return f == "geom_size" || f == "geom_friction"; }
+// every per-environment geom array a perturbation may write
+static bool is_geom_field(const std::string& f) { return is_geom_decl_field(f) || f == "geom_solref" || f == "geom_solimp"; }
+static bool is_body_field(const std::string& f) { return f == "body_mass" || f == "body_inertia"; }
+static bool is_dof_field(const std::string& f) { return f == "dof_damping" || f == "dof_armature" || f == "dof_frictionloss"; }
+// name of the per-environment array of (field, id): "<field>" for the whole-vector dof fields, "<field>:<id>" otherwise
+static std::string override_key(const std::string& f, int id) { return is_dof_field(f) ? f : f + ":" + std::to_string(id); }
+
 template <typename R> static int model_override_t(b2s_sim* s, DState<R>& st, const std::string& field, int id) {
-  const bool geom = field == "geom_size" || field == "geom_friction";
+  const bool geom = is_geom_decl_field(field);
   const size_t N = s->n_env;
   const int code = DT<R>::code;
   try {
     if (!st.dof_iw) {  // first override of the handle: the banks of every slot, the derived constants from the model's values
       st.mg_size = dev_zeros<R>(s, B2S_MOV * N * 3); st.mg_fric = dev_zeros<R>(s, B2S_MOV * N * 3);
       st.mg_rbound = dev_zeros<R>(s, B2S_MOV * N); st.mg_aabb = dev_zeros<R>(s, B2S_MOV * N * 6);
+      st.mg_solref = dev_zeros<R>(s, B2S_MOV * N * 2); st.mg_solimp = dev_zeros<R>(s, B2S_MOV * N * 5);
       st.mb_mass = dev_zeros<R>(s, B2S_MOV * N); st.mb_inertia = dev_zeros<R>(s, B2S_MOV * N * 3);
       R* diw = dev_zeros<R>(s, N * s->nv); R* biw = dev_zeros<R>(s, N * s->nbody * 2); R* mi = dev_zeros<R>(s, N);
       upload_rows(diw, s->dof_iw_h.data(), s->nv, N);
@@ -1351,20 +1370,30 @@ template <typename R> static int model_override_t(b2s_sim* s, DState<R>& st, con
       s->arrays["meaninertia"] = ArrayInfo{mi, code, 1, {s->n_env, 0, 0, 0}};
       st.dof_iw = diw; st.body_iw = biw; st.mean_inertia = mi;
     }
-    const std::string key = field + ":" + std::to_string(id);
+    const std::string key = override_key(field, id);
     if (s->arrays.count(key)) return B2S_OK;
-    if (geom) {
+    if (is_dof_field(field)) {
+      const std::vector<double>& h = field == "dof_damping" ? s->dof_damping_h : field == "dof_armature" ? s->dof_armature_h : s->dof_frictionloss_h;
+      R* p = dev_zeros<R>(s, N * s->nv);
+      upload_rows(p, h.data(), s->nv, N);
+      (field == "dof_damping" ? st.dof_damp : field == "dof_armature" ? st.dof_arm : st.dof_floss) = p;
+      s->arrays[key] = ArrayInfo{p, code, 2, {s->n_env, s->nv, 0, 0}};
+    } else if (geom) {
       int k = 0;
       while (k < st.n_mg && st.mg_id[k] != id) k++;
-      if (k == st.n_mg) {  // a new slot: size, friction, bounds of this geom for every environment
+      if (k == st.n_mg) {  // a new slot: size, friction, bounds, solref, solimp of this geom for every environment
         if (k >= B2S_MOV) return fail(B2S_ERR_UNSUPPORTED, "b2s_model_override: at most 8 geoms per handle");
         upload_rows(st.mg_size + k * N * 3, &s->geom_size_h[3 * id], 3, N);
         upload_rows(st.mg_fric + k * N * 3, &s->geom_friction_h[3 * id], 3, N);
         upload_rows(st.mg_rbound + k * N, &s->geom_rbound_h[id], 1, N);
         upload_rows(st.mg_aabb + k * N * 6, &s->geom_aabb_h[6 * id], 6, N);
+        upload_rows(st.mg_solref + k * N * 2, &s->geom_solref_h[2 * id], 2, N);
+        upload_rows(st.mg_solimp + k * N * 5, &s->geom_solimp_h[5 * id], 5, N);
         st.mg_id[k] = (short)id; st.n_mg = k + 1;
         s->arrays["geom_rbound:" + std::to_string(id)] = ArrayInfo{st.mg_rbound + k * N, code, 1, {s->n_env, 0, 0, 0}};
         s->arrays["geom_aabb:" + std::to_string(id)] = ArrayInfo{st.mg_aabb + k * N * 6, code, 2, {s->n_env, 6, 0, 0}};
+        s->arrays["geom_solref:" + std::to_string(id)] = ArrayInfo{st.mg_solref + k * N * 2, code, 2, {s->n_env, 2, 0, 0}};
+        s->arrays["geom_solimp:" + std::to_string(id)] = ArrayInfo{st.mg_solimp + k * N * 5, code, 2, {s->n_env, 5, 0, 0}};
       }
       R* p = field == "geom_size" ? st.mg_size + k * N * 3 : st.mg_fric + k * N * 3;
       s->arrays[key] = ArrayInfo{p, code, 2, {s->n_env, 3, 0, 0}};
@@ -1406,16 +1435,22 @@ extern "C" {
 int b2s_model_override(b2s_sim* s, const char* field, int id) {
   if (!s || !field) return fail(B2S_ERR_ARG, "b2s_model_override: bad argument");
   const std::string f = field;
-  if (f == "geom_size" || f == "geom_friction") {
+  if (is_geom_decl_field(f)) {
     if (id < 0 || id >= s->ngeom) return fail(B2S_ERR_ARG, "b2s_model_override: geom id out of range");
     const int t = s->geom_type_h[id];
     if (s->cgid[id] < 0 || !(t == G_SPHERE || t == G_CAPSULE || t == G_ELLIPSOID || t == G_CYLINDER || t == G_BOX))
       return fail(B2S_ERR_UNSUPPORTED, "b2s_model_override: only colliding sphere, capsule, ellipsoid, cylinder and box geoms have per-environment values");
-  } else if (f == "body_mass" || f == "body_inertia") {
+  } else if (is_body_field(f)) {
     if (id < 0 || id >= s->nbody) return fail(B2S_ERR_ARG, "b2s_model_override: body id out of range");
     if (s->body_weldid_h[id] == 0) return fail(B2S_ERR_UNSUPPORTED, "b2s_model_override: the body does not move (world body or welded to it)");
+  } else if (is_dof_field(f)) {
+    if (id != -1) return fail(B2S_ERR_ARG, "b2s_model_override: the dof fields are whole vectors (id -1)");
+    // any dof may get a friction-loss row: the large tier must hold nv of them besides the limit and contact rows
+    if (f == "dof_frictionloss" && s->maxefc < s->nv + 8)
+      return fail(B2S_ERR_UNSUPPORTED, "b2s_model_override: opt_maxefc cannot hold a friction-loss row for every dof (needs nv + 8)");
   } else {
-    return fail(B2S_ERR_ARG, "b2s_model_override: unknown field '" + f + "' (geom_size, geom_friction, body_mass, body_inertia)");
+    return fail(B2S_ERR_ARG, "b2s_model_override: unknown field '" + f + "' (geom_size, geom_friction, body_mass, body_inertia, "
+                             "dof_damping, dof_armature, dof_frictionloss; a declared geom's solref / solimp come with its slot)");
   }
   CUDA_TRY(cudaSetDevice(s->device));
   return s->precision == B2S_F32 ? model_override_t<float>(s, s->sf, f, id) : model_override_t<double>(s, s->sd, f, id);
@@ -1424,6 +1459,72 @@ int b2s_model_override(b2s_sim* s, const char* field, int id) {
 int b2s_set_const(b2s_sim* s, const uint8_t* env_mask) {
   if (!s) return fail(B2S_ERR_ARG, "null handle");
   return launch_set_const(s, env_mask);
+}
+
+int b2s_perturb_config(b2s_sim* s, const b2s_perturb* spec, int n) {
+  if (!s || n < 0 || (n > 0 && !spec)) return fail(B2S_ERR_ARG, "b2s_perturb_config: bad argument");
+  std::vector<PerturbEntry> ent;
+  std::vector<PerturbItem> item;
+  for (int i = 0; i < n; i++) {
+    const b2s_perturb& p = spec[i];
+    const std::string f = p.field ? p.field : "";
+    const std::string at = "b2s_perturb_config: entry " + std::to_string(i) + " ('" + f + "'): ";
+    if (!(p.mode == B2S_PERTURB_SCALE || p.mode == B2S_PERTURB_SHIFT)) return fail(B2S_ERR_ARG, at + "mode must be scale or shift");
+    if (!(p.amplitude >= 0) || !std::isfinite(p.amplitude)) return fail(B2S_ERR_ARG, at + "the amplitude must be finite and >= 0");
+    if (p.mode == B2S_PERTURB_SCALE && p.amplitude >= 1) return fail(B2S_ERR_ARG, at + "a scale amplitude must be below 1");
+    const bool dof = is_dof_field(f);
+    if (!dof && !is_geom_field(f) && !is_body_field(f)) return fail(B2S_ERR_ARG, at + "unknown field");
+    if (dof && (p.id < -1 || p.id >= s->nv)) return fail(B2S_ERR_ARG, at + "dof id out of range");
+    auto it = s->arrays.find(override_key(f, p.id));
+    if (it == s->arrays.end()) return fail(B2S_ERR_ARG, at + "the field is not declared (b2s_model_override)");
+    const size_t rsz = s->precision == B2S_F32 ? 4 : 8;
+    PerturbEntry e{};
+    e.mode = p.mode; e.one_draw = p.one_draw != 0; e.amp = p.amplitude;
+    const double* model;
+    int ncomp;
+    if (dof) {  // id -1: every dof; a dof index: that component of the vector alone
+      const std::vector<double>& h = f == "dof_damping" ? s->dof_damping_h : f == "dof_armature" ? s->dof_armature_h : s->dof_frictionloss_h;
+      const int first = p.id < 0 ? 0 : p.id;
+      e.stride = s->nv;
+      e.dst = (char*)it->second.ptr + first * rsz;
+      model = h.data() + first;
+      ncomp = p.id < 0 ? s->nv : 1;
+    } else {
+      const int w = it->second.ndim == 1 ? 1 : (int)it->second.shape[1];
+      const std::vector<double>& h = f == "geom_size" ? s->geom_size_h : f == "geom_friction" ? s->geom_friction_h : f == "geom_solref" ? s->geom_solref_h
+                                   : f == "geom_solimp" ? s->geom_solimp_h : f == "body_mass" ? s->body_mass_h : s->body_inertia_h;
+      e.stride = w;
+      e.dst = it->second.ptr;
+      model = h.data() + (size_t)w * p.id;
+      ncomp = w;
+    }
+    for (int c = 0; c < ncomp; c++) item.push_back(PerturbItem{(int)ent.size(), c, model[c]});
+    ent.push_back(e);
+  }
+  CUDA_TRY(cudaSetDevice(s->device));
+  try {  // replaced tables stay allocated until the handle is destroyed (configuration is a set-up step)
+    s->pert_ent = ent.empty() ? nullptr : dev_upload(s, ent);
+    s->pert_item = item.empty() ? nullptr : dev_upload(s, item);
+  } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
+  s->pert_nitems = (int)item.size();
+  return B2S_OK;
+}
+
+int b2s_perturb_model(b2s_sim* s, const uint8_t* env_mask, uint64_t seed, uint64_t counter) {
+  if (!s) return fail(B2S_ERR_ARG, "null handle");
+  if (counter >> 32) return fail(B2S_ERR_ARG, "b2s_perturb_model: the counter must be below 2^32");
+  if (s->pert_nitems == 0) return B2S_OK;
+  CUDA_TRY(cudaSetDevice(s->device));
+  const long long total = (long long)s->n_env * s->pert_nitems;
+  const int threads = 256;
+  const unsigned blocks = (unsigned)((total + threads - 1) / threads);
+  if (s->precision == B2S_F32)
+    perturb_kernel<float><<<blocks, threads, 0, s->stream>>>(s->pert_ent, s->pert_item, s->pert_nitems, s->n_env, env_mask, seed, (unsigned)counter);
+  else
+    perturb_kernel<double><<<blocks, threads, 0, s->stream>>>(s->pert_ent, s->pert_item, s->pert_nitems, s->n_env, env_mask, seed, (unsigned)counter);
+  s->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return B2S_OK;
 }
 
 int b2s_body_pose_override(b2s_sim* s, int body_id) {

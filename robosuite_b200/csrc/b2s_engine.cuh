@@ -148,6 +148,24 @@ template <typename R> DEV const R* body_inertia_of(const DModel<R>& m, const DSt
   for (int k = 0; k < s.n_mb; k++) if (s.mb_id[k] == b) return s.mb_inertia + 3 * ((size_t)k * s.n_env + env);
   return m.body_inertia + 3 * b;
 }
+template <typename R> DEV const R* geom_solref_of(const DModel<R>& m, const DState<R>& s, int g, int env) {
+  for (int k = 0; k < s.n_mg; k++) if (s.mg_id[k] == g) return s.mg_solref + 2 * ((size_t)k * s.n_env + env);
+  return m.geom_solref + 2 * g;
+}
+template <typename R> DEV const R* geom_solimp_of(const DModel<R>& m, const DState<R>& s, int g, int env) {
+  for (int k = 0; k < s.n_mg; k++) if (s.mg_id[k] == g) return s.mg_solimp + 5 * ((size_t)k * s.n_env + env);
+  return m.geom_solimp + 5 * g;
+}
+// whole dof vectors: a stage picks the row once, at its top, and its loops index it (no lookup inside the arithmetic)
+template <typename R> DEV const R* dof_damping_of(const DModel<R>& m, const DState<R>& s, int env) {
+  return s.dof_damp ? s.dof_damp + (size_t)env * m.nv : m.dof_damping;
+}
+template <typename R> DEV const R* dof_armature_of(const DModel<R>& m, const DState<R>& s, int env) {
+  return s.dof_arm ? s.dof_arm + (size_t)env * m.nv : m.dof_armature;
+}
+template <typename R> DEV const R* dof_frictionloss_of(const DModel<R>& m, const DState<R>& s, int env) {
+  return s.dof_floss ? s.dof_floss + (size_t)env * m.nv : m.dof_frictionloss;
+}
 // constants derived at qpos0 (the set-constants pass writes them per environment once a handle declares an override)
 template <typename R> DEV const R* dof_invweight0_of(const DModel<R>& m, const DState<R>& s, int env) {
   return s.dof_iw ? s.dof_iw + (size_t)env * m.nv : m.dof_invweight0;
@@ -454,6 +472,7 @@ struct Eng {
     __syncwarp();
     // per dof: project the subtree sums on the motion axis
     R* bias = p(L.bias); R* passive = p(L.passive);
+    const R* damping = dof_damping_of(m, state(), env);
     for (int i = lane; i < m.nv; i += 32) {
       int b0 = m.dof_bodyid[i], b1 = m.body_subtree_end[b0];
       R f[6] = {0, 0, 0, 0, 0, 0}, g[6] = {0, 0, 0, 0, 0, 0};
@@ -462,7 +481,7 @@ struct Eng {
         for (int e = 0; e < 6; e++) { f[e] += frne[6 * b + e]; g[e] += ffl[6 * b + e]; }
       }
       bias[i] = dot6(cdof + 6 * i, f);
-      passive[i] = -m.dof_damping[i] * qvel[i] + dot6(cdof + 6 * i, g);
+      passive[i] = -damping[i] * qvel[i] + dot6(cdof + 6 * i, g);
     }
     __syncwarp();
   }
@@ -471,6 +490,7 @@ struct Eng {
   DEVN void crb() {
     const DModel<R>& m = model(); const WSLayout& L = lay();
     R* cinert = p(L.cinert);
+    const R* armature = dof_armature_of(m, state(), env);
     // composite inertia = sum over the (contiguous, DFS-ordered) subtree, written to scratch
     int nb = m.nbody;
     R* crbuf = p(L.scratch);  // 10 * nbody reals of scratch
@@ -498,7 +518,7 @@ struct Eng {
     for (int e = lane; e < m.nment; e += 32) {
       int i = m.ment_i[e], j = m.ment_j[e];
       R v = dot6(cdof + 6 * j, fi + 6 * i);
-      if (i == j) v += m.dof_armature[i];
+      if (i == j) v += armature[i];
       M[i * nv + j] = v;
       M[j * nv + i] = v;
     }
@@ -620,7 +640,7 @@ struct Eng {
     R* a = p(L.grad);  // reuse solver vector as the integration acceleration
     for (int i = lane; i < nv; i += 32) a[i] = p(L.qsmooth)[i] + p(L.qcon)[i];
     __syncwarp();
-    int bad = spd_solve(p(L.M), nv, m.dof_damping, h, a, p(L.H), true);
+    int bad = spd_solve(p(L.M), nv, dof_damping_of(m, state(), env), h, a, p(L.H), true);
     R* qvel = p(L.qvel); R* qpos = p(L.qpos);
     for (int i = lane; i < nv; i += 32) qvel[i] += h * a[i];
     __syncwarp();

@@ -218,8 +218,9 @@ __global__ void reset_envs_kernel(const uint8_t* mask, const R* qpos_new, int sl
 //   meaninertia       = mean diag(M)
 //   dof_invweight0    = diag(M^-1), averaged over the translational and the rotational block of each free joint
 //   body_invweight0   = (mean translational, mean rotational) diagonal of J M^-1 J^T, J = Jacobian of the body's centre of mass
-// and every overridden geom gets its bounding radius and local box from its size (the compiler's per-type rules).  Override values
-// that are non-finite or non-positive, or moments that violate the triangle inequality, set warn bit 128.
+// and every overridden geom gets its bounding radius and local box from its size (the compiler's per-type rules).  The CRB adds the
+// environment's own armature.  Override values that are non-finite or non-positive (damping, armature and friction loss: negative),
+// a non-finite solref / solimp component, or moments that violate the triangle inequality set warn bit 128.
 // Workspace per warp: the fused layout followed by nv * nv words for M^-1 (`stride` words in all).
 template <typename R>
 __global__ void __launch_bounds__(512, 1) set_const_kernel(const uint8_t* mask, int slot, int stride) {
@@ -243,6 +244,8 @@ __global__ void __launch_bounds__(512, 1) set_const_kernel(const uint8_t* mask, 
     const R* fr = s.mg_fric + 3 * o;
     const int nsz = t == G_SPHERE ? 1 : (t == G_CAPSULE || t == G_CYLINDER ? 2 : 3);
     for (int q = 0; q < 3; q++) if (!pos(fr[q]) || (q < nsz && !pos(sz[q]))) bad = 1;
+    for (int q = 0; q < 2; q++) if (!isfinite(s.mg_solref[2 * o + q])) bad = 1;
+    for (int q = 0; q < 5; q++) if (!isfinite(s.mg_solimp[5 * o + q])) bad = 1;
     R r = sz[0], h = sz[1], rb, hx = r, hy = r, hz = r;
     if (t == G_SPHERE) rb = r;
     else if (t == G_CAPSULE) { rb = r + h; hz = r + h; }
@@ -260,6 +263,10 @@ __global__ void __launch_bounds__(512, 1) set_const_kernel(const uint8_t* mask, 
     const R* I = s.mb_inertia + 3 * o;
     if (!pos(s.mb_mass[o]) || !pos(I[0]) || !pos(I[1]) || !pos(I[2]) || I[0] + I[1] < I[2] || I[0] + I[2] < I[1] || I[1] + I[2] < I[0]) bad = 1;
   }
+  auto nonneg = [](R v) { return isfinite(v) && v >= R(0); };
+  const R* dofv[3] = {s.dof_damp, s.dof_arm, s.dof_floss};
+  for (int k = 0; k < 3; k++)
+    if (dofv[k]) for (int i = lane; i < nv; i += 32) if (!nonneg(dofv[k][E * nv + i])) bad = 1;
   bad = warp_or_i(bad);
   if (bad && lane == 0) s.warn[env] |= 128;
   // M at qpos0
@@ -320,6 +327,43 @@ __global__ void __launch_bounds__(512, 1) set_const_kernel(const uint8_t* mask, 
     s.body_iw[(E * nb + b) * 2] = at / R(3);
     s.body_iw[(E * nb + b) * 2 + 1] = ar / R(3);
   }
+}
+
+// ---- device perturbation of the override arrays (b2s_perturb_model), the batched counterpart of the reference's DynamicsModder
+// (utils/mjmod.py): every configured (field, id) of the masked environments is redrawn around the MODEL's value.
+//   scale: v = v_model * (1 + d)       shift: v = max(0, v_model + d)       d = a * (2u - 1), u in [0, 1)
+// u comes from Philox4x32-10 (Salmon et al., SC'11) keyed by the seed, counter (env, call counter, entry, component), so an
+// environment's draws do not depend on n_env or on the mask.  u = 53 bits of the first two output words.  The arithmetic is in fp64
+// with explicit roundings (no contraction), so a host restatement reproduces every bit; the result is rounded to the handle's precision.
+struct PerturbEntry { void* dst; int stride, mode, one_draw; double amp; };  // value of (env, component c) at dst[env * stride + c]
+struct PerturbItem { int entry, comp; double model; };                     // one per (entry, component), in entry order
+
+DEV uint4 philox4x32_10(uint4 c, unsigned k0, unsigned k1) {
+#pragma unroll
+  for (int r = 0; r < 10; r++) {
+    if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    const unsigned lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+    const unsigned lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+  }
+  return c;
+}
+
+template <typename R>
+__global__ void perturb_kernel(const PerturbEntry* ent, const PerturbItem* item, int nitems, int n_env, const uint8_t* mask,
+                               unsigned long long seed, unsigned counter) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (long long)n_env * nitems) return;
+  const int env = (int)(t / nitems), it = (int)(t % nitems);
+  if (mask && !mask[env]) return;
+  const PerturbItem p = item[it];
+  const PerturbEntry& en = ent[p.entry];
+  const uint4 x = philox4x32_10(make_uint4((unsigned)env, counter, (unsigned)p.entry, en.one_draw ? 0u : (unsigned)p.comp),
+                                (unsigned)seed, (unsigned)(seed >> 32));
+  const double u = (double)(((unsigned long long)(x.x >> 5) << 26) | (x.y >> 6)) * 0x1p-53;
+  const double d = __dmul_rn(en.amp, __dsub_rn(__dmul_rn(2.0, u), 1.0));
+  const double v = en.mode == 0 ? __dmul_rn(p.model, __dadd_rn(1.0, d)) : fmax(0.0, __dadd_rn(p.model, d));
+  reinterpret_cast<R*>(en.dst)[(size_t)env * en.stride + p.comp] = (R)v;
 }
 
 template <typename R>

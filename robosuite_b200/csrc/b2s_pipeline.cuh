@@ -438,6 +438,7 @@ template <typename R> DEV void store_state(const Eng<R>& e, int env, R time, int
 template <typename R>
 DEV void tail_finish(Eng<R>& e, int env, int sub, int nsub, int phases, int ncon, int warn, unsigned long long* bar, unsigned& parity) {
   const DState<R>& s = e.state();
+  e.env = env;  // Euler reads the environment's damping
   R time = s.time[env];
   if (!(phases & PH_NOINTEGRATE)) {
     { int eb = e.euler(&time); if (eb & 32) warn |= 32; else if (eb) warn |= 2; }

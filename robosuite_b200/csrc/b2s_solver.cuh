@@ -57,17 +57,39 @@ template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn, fl
   int* eint = e.pi(L.e_int);
   const R* qpos = e.p(L.qpos); const R* qvel = e.p(L.qvel);
   int nefc = 0;
-  // --- friction-loss rows (static list)
-  B2S_LOOP
-  for (int r = lane; r < m.nfl; r += 32) {
-    int dof = m.fl_dof[r];
+  const DState<R>& st = e.state();
+  if (!st.dof_floss) {
+    // --- friction-loss rows (static list)
     B2S_LOOP
-    for (int i = 0; i < nv; i++) J[r * nv + i] = i == dof ? R(1) : R(0);
-    eint[r] = C_FRICTION | (dof << 8);
-    epos[r] = 0;
-    efl[r] = m.dof_frictionloss[dof];
+    for (int r = lane; r < m.nfl; r += 32) {
+      int dof = m.fl_dof[r];
+      B2S_LOOP
+      for (int i = 0; i < nv; i++) J[r * nv + i] = i == dof ? R(1) : R(0);
+      eint[r] = C_FRICTION | (dof << 8);
+      epos[r] = 0;
+      efl[r] = m.dof_frictionloss[dof];
+    }
+    nefc = m.nfl;
+  } else {
+    // --- friction-loss rows of this environment (b2s_model_override "dof_frictionloss"): its dofs with a value > 0, in dof order
+    const R* floss = st.dof_floss + (size_t)e.env * nv;
+    B2S_LOOP
+    for (int base = 0; base < nv; base += 32) {
+      int dof = base + lane;
+      R fl = dof < nv ? floss[dof] : R(0);
+      int act = fl > 0;
+      unsigned mask = __ballot_sync(B2S_FULL, act);
+      int r = nefc + __popc(mask & ((1u << lane) - 1));
+      if (act && r < L.me) {
+        B2S_LOOP
+        for (int i = 0; i < nv; i++) J[r * nv + i] = i == dof ? R(1) : R(0);
+        eint[r] = C_FRICTION | (dof << 8);
+        epos[r] = 0;
+        efl[r] = fl;
+      }
+      nefc += __popc(mask);
+    }
   }
-  nefc = m.nfl;
   // --- joint limits
   B2S_LOOP
   for (int base = 0; base < m.nlim; base += 32) {
@@ -205,6 +227,8 @@ template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn, fl
       first = k == 0;
       int b1 = m.geom_bodyid[g1], b2 = m.geom_bodyid[g2];
       const R* biw = body_invweight0_of(m, e.state(), e.env);
+      const R* sr1 = geom_solref_of(m, e.state(), g1, e.env); const R* sr2 = geom_solref_of(m, e.state(), g2, e.env);
+      const R* si1 = geom_solimp_of(m, e.state(), g1, e.env); const R* si2 = geom_solimp_of(m, e.state(), g2, e.env);
       diag = k < 3 ? biw[2 * b1] + biw[2 * b2] : biw[2 * b1 + 1] + biw[2 * b2 + 1];
       // solref / solimp mixing (solmix-weighted)
       R s1 = m.geom_solmix[g1], s2 = m.geom_solmix[g2], mix;
@@ -213,11 +237,11 @@ template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn, fl
       else if (s1 >= Lim<R>::minval() && s2 >= Lim<R>::minval()) mix = s1 / (s1 + s2);
       else if (s1 < Lim<R>::minval() && s2 < Lim<R>::minval()) mix = R(0.5);
       else mix = s1 < Lim<R>::minval() ? R(0) : R(1);
-      R r10 = m.geom_solref[2 * g1], r11 = m.geom_solref[2 * g1 + 1], r20 = m.geom_solref[2 * g2], r21 = m.geom_solref[2 * g2 + 1];
+      R r10 = sr1[0], r11 = sr1[1], r20 = sr2[0], r21 = sr2[1];
       if (p1 != p2 || (r10 > 0 && r20 > 0)) { solref[0] = mix * r10 + (1 - mix) * r20; solref[1] = mix * r11 + (1 - mix) * r21; }
       else { solref[0] = r_min(r10, r20); solref[1] = r_min(r11, r21); }
       B2S_LOOP
-      for (int q = 0; q < 5; q++) solimp[q] = mix * m.geom_solimp[5 * g1 + q] + (1 - mix) * m.geom_solimp[5 * g2 + q];
+      for (int q = 0; q < 5; q++) solimp[q] = mix * si1[q] + (1 - mix) * si2[q];
     }
     R pos = epos[r];
     // friction rows of a cone reuse the normal row's impedance: evaluate it from the normal's pos

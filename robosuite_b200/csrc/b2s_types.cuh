@@ -106,7 +106,11 @@ struct DState {
   short mg_id[B2S_MOV], mb_id[B2S_MOV];
   R *mg_size, *mg_fric, *mg_rbound, *mg_aabb;  // [B2S_MOV][n_env] x 3 / 3 / 1 / 6 (rbound, aabb: written by the set-constants pass)
   R *mb_mass, *mb_inertia;                     // [B2S_MOV][n_env] x 1 / 3
+  R *mg_solref, *mg_solimp;                    // [B2S_MOV][n_env] x 2 / 5 (same geom slots as size and friction)
   R *dof_iw, *body_iw, *mean_inertia;          // [n_env] x nv / nbody * 2 / 1: dof_invweight0, body_invweight0, meaninertia
+  // whole-vector dof overrides, [n_env, nv] each; null = the model's vector.  A non-null dof_floss makes the friction-loss rows
+  // per environment (the dofs whose own value is > 0) instead of the model's static list
+  R *dof_damp, *dof_arm, *dof_floss;
   R* task_vec;     // [n_env, task_dim] task table values after the last substep
   R* task_out;     // [n_env, 8]: body height, |grip site - body|, grasp flag, horizontal |body - body2|, obj-obj2 contact flag
   // -DB2S_INSTR builds only (measurement aid, see b2s_instr in b2s_pipeline.cuh): device timeline of the graph replay and

@@ -36,6 +36,31 @@ class CtrlCfg(C.Structure):
     ]
 
 
+# per-environment model fields that are whole dof vectors (model_override(field) with no object id)
+DOF_FIELDS = ("dof_damping", "dof_armature", "dof_frictionloss")
+# per-environment contact parameters of a declared geom (arrays "<field>:<id>" that come with the geom's slot)
+GEOM_CONTACT_FIELDS = ("geom_solref", "geom_solimp")
+PERTURB_SCALE, PERTURB_SHIFT = 0, 1
+
+
+class PerturbSpec(C.Structure):
+    """b2s_perturb: one (field, id) entry of b2s_perturb_config"""
+    _fields_ = [("field", C.c_char_p), ("id", C.c_int), ("mode", C.c_int), ("amplitude", C.c_double), ("one_draw", C.c_int)]
+
+
+def normalize_perturb_spec(spec):
+    """perturb_config entries as (field, id, mode, amplitude, one_draw) tuples: dicts or tuples in, id None -> -1, mode names -> codes"""
+    out = []
+    for e in spec:
+        if isinstance(e, dict):
+            e = (e["field"], e.get("id"), e.get("mode", PERTURB_SCALE), e["amplitude"], e.get("one_draw", False))
+        f, i, mode, amp = e[:4]
+        one = e[4] if len(e) > 4 else False
+        mode = {"scale": PERTURB_SCALE, "shift": PERTURB_SHIFT}.get(mode, mode)
+        out.append((str(f), -1 if i is None else int(i), int(mode), float(amp), int(bool(one))))
+    return out
+
+
 def lib():
     global _LIB
     if _LIB is None:
@@ -70,6 +95,8 @@ def lib():
         L.b2s_body_pose_override.argtypes = [C.c_void_p, C.c_int]
         L.b2s_model_override.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
         L.b2s_set_const.argtypes = [C.c_void_p, C.c_void_p]
+        L.b2s_perturb_config.argtypes = [C.c_void_p, C.POINTER(PerturbSpec), C.c_int]
+        L.b2s_perturb_model.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64]
         L.b2s_obs_config.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.b2s_task_config.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.b2s_task_config2.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
@@ -228,13 +255,36 @@ class BatchedSim:
         self._check(self._L.b2s_body_pose_override(self._h, int(body_id)))
         return self.array("body_xpos_ov:%d" % body_id), self.array("body_xquat_ov:%d" % body_id)
 
-    def model_override(self, field, obj_id):
+    def model_override(self, field, obj_id=None):
         """[n_env, ...] tensor of per-environment values of one model field for one object (b2s_model_override): "geom_size" /
-        "geom_friction" [n_env, 3] of a colliding primitive geom, "body_mass" [n_env] / "body_inertia" [n_env, 3] (principal moments in
-        the model's inertial frame) of a moving body.  Starts at the model's values.  The constants derived from these values
-        (dof_invweight0, body_invweight0, meaninertia, the geom's bounding radius and box) follow at the next set_const() or reset."""
-        self._check(self._L.b2s_model_override(self._h, field.encode(), int(obj_id)))
-        return self.array("%s:%d" % (field, obj_id))
+        "geom_friction" [n_env, 3], "geom_solref" [n_env, 2] and "geom_solimp" [n_env, 5] of a colliding primitive geom, "body_mass"
+        [n_env] / "body_inertia" [n_env, 3] (principal moments in the model's inertial frame) of a moving body, and the whole dof
+        vectors "dof_damping" / "dof_armature" / "dof_frictionloss" [n_env, nv] (obj_id None).  Starts at the model's values.  The
+        constants derived from these values (dof_invweight0, body_invweight0, meaninertia, the geom's bounding radius and box) follow
+        at the next set_const() or reset.  A geom's solref / solimp come with its slot in the library: asking for them declares the
+        geom through its friction (an array that starts at, and keeps, the model's values until written)."""
+        oid = -1 if obj_id is None else int(obj_id)
+        declared = "geom_friction" if field in GEOM_CONTACT_FIELDS else field
+        self._check(self._L.b2s_model_override(self._h, declared.encode(), oid))
+        return self.array(field if field in DOF_FIELDS else "%s:%d" % (field, oid))
+
+    def perturb_config(self, spec):
+        """configure perturb_model (b2s_perturb_config): a list of entries (field, id, mode, amplitude, one_draw) or dicts with those
+        keys (id None = -1, mode "scale" / "shift" or PERTURB_SCALE / PERTURB_SHIFT, one_draw default False); every field must be
+        declared with model_override first.  An empty list clears the configuration."""
+        entries = normalize_perturb_spec(spec)
+        arr = (PerturbSpec * max(len(entries), 1))()
+        names = [f.encode() for f, *_ in entries]  # kept alive for the call
+        for k, (f, i, mode, amp, one) in enumerate(entries):
+            arr[k] = PerturbSpec(names[k], i, mode, amp, one)
+        self._check(self._L.b2s_perturb_config(self._h, arr, len(entries)))
+
+    def perturb_model(self, mask=None, seed=0, counter=0):
+        """redraw every configured override of the masked environments (uint8 [n_env] device mask, None = all) around the model's
+        values in one launch (b2s_perturb_model): Philox4x32-10 keyed by `seed`, counter (env, counter, entry, component).  The
+        derived constants follow at the next set_const() or reset."""
+        self._check(self._L.b2s_perturb_model(self._h, None if mask is None else C.c_void_p(mask.data_ptr()), int(seed) & (2 ** 64 - 1),
+                                              int(counter)))
 
     def set_const(self, mask=None):
         """recompute the derived constants of the masked environments (uint8 [n_env] device mask, None = all) from their

@@ -97,8 +97,9 @@ SIM_WARN_BITS = {1: "singular mass matrix", 2: "non-finite state in the integrat
                  8: "constraint-row capacity overflow (maxefc)", 16: "singular Newton Hessian",
                  32: "diverged state (non-finite / huge qpos, qvel or qacc): data reset to the model defaults, as mj_checkPos/Vel/Acc do",
                  64: "unit-queue watchdog fired: the control step is incomplete (mode 2 only; a library bug, please report)",
-                 128: "invalid model override (non-finite or non-positive size, friction, mass or moment, or moments violating the "
-                      "triangle inequality)"}
+                 128: "invalid model override (non-finite or non-positive size, friction, mass or moment, moments violating the "
+                      "triangle inequality, non-finite or negative damping, armature or friction loss, or a non-finite solref / "
+                      "solimp component)"}
 
 
 class BatchedMujocoEnv:
