@@ -193,8 +193,10 @@ int b2s_task_table(b2s_sim* sim, int n, const int* op, const int* a, const int* 
 int b2s_set_export(b2s_sim* sim, int flag);
 
 /* Scheduling of b2s_env_step / b2s_step: 0 = fused (one kernel per call, state resident in shared memory for all
- * substeps), 1 = pipeline (five phase kernels per substep exchanging a workspace row through L2).  Results are
- * identical; see DESIGN.md section 5 for when each wins. */
+ * substeps), 1 = pipeline (per substep and environment group: phase 0, phase 1 (narrow phase + controller), the tail kernel and,
+ * when the model has a small tail tier, its large-tier re-run, exchanging a workspace row through L2; one CUDA graph per group,
+ * replayed on the group's own stream), 2 = unit queue (one persistent kernel per control step).  Results are identical; see
+ * DESIGN.md sections 4 and 5 for when each wins. */
 int b2s_set_mode(b2s_sim* sim, int mode);
 
 /* debugging aid: b2s_env_step accumulates per-phase clock cycles per environment into the array "prof" [n_env,12]
@@ -204,11 +206,6 @@ int b2s_set_profile(b2s_sim* sim, int flag);
 
 /* number of kernels this handle has launched since creation (bench.py "gpu_launches") */
 int64_t b2s_launch_count(const b2s_sim* sim);
-/* Measurement aid (pipeline mode): enable = 1 switches b2s_env_step / b2s_step to eager launches bracketed by timing events,
- * enable = 0 back to CUDA-graph replay, enable < 0 only reads.  mean_us / count (may be NULL) receive, for the LAST call made
- * while enabled, the mean event-to-event interval per launch kind: [1] counter memset, [2] phase 0, [3] analytic narrow phase,
- * [4] convex narrow phase, [5] merged tail phase (or phase 2), [6] phase 3, [7] phase 4. */
-int b2s_timeline(b2s_sim* sim, int enable, double mean_us[8], int count[8]);
 
 /* Host-only diagnostic (no device needed): words per warp of the shared-memory layouts and of the global workspace row that a model
  * of these dimensions gets - out_words[5] = fused kernel, phase 0, tail small tier, tail large tier, row.  out_layouts / out_pio may

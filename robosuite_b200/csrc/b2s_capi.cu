@@ -10,6 +10,7 @@
 #include <map>
 #include <algorithm>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 static thread_local std::string g_err;
@@ -71,25 +72,19 @@ struct b2s_sim {
   std::vector<double> qpos0;
   std::vector<int> site_bodyid, cgid;
   std::map<std::string, std::vector<std::string>> names;  // object type -> names by id (MjModel name tables)
-  int has_obs = 0, export_env_step = 1, dirty = 1, profile = 0, mode = 0, worklist = 1, ngroups = 8;
-  int timeline = 0, debug_skip = 0;  // B2S_DEBUG_SKIP: bit 0 / 1 = leave out the analytic / convex narrow-phase launch (timing experiments)
-  struct TlEv { int group, type; cudaEvent_t ev; };
-  std::vector<TlEv> tl_events;
-  double tl_mean_us[8] = {0}; int tl_count[8] = {0};
+  int has_obs = 0, export_env_step = 1, dirty = 1, profile = 0, mode = 0, ngroups = 8;
   int ctrl_split = 1;  // pipeline: OSC controller as its own thread-per-environment kernel (B2S_CTRL_SPLIT=0: inside the tail kernel)
+  // pipeline: one CUDA graph per environment group, replayed on the group's stream and joined to `stream` through gevents
   std::vector<cudaStream_t> gstreams;
   std::vector<cudaEvent_t> gevents;
-  cudaEvent_t fork_event = nullptr, in_event = nullptr, out_event = nullptr;
-  cudaStream_t pstream = nullptr;
+  cudaEvent_t in_event = nullptr;
   void* action_buf = nullptr;
-  int use_graph = 1;
-  int graph_per_group = 1;  // one CUDA graph per environment group on its own stream (B2S_GRAPH_PER_GROUP=0: one graph for all)
   std::map<long long, cudaGraphExec_t> graphs;
   PhaseIO pio[B2S_NPIO];
   std::map<std::string, Region> reg;
   // unit-queue mode (mode 2, b2s_unit.cuh)
   int* uq_ring = nullptr; int* uq_ovf = nullptr; int* uq_ctr = nullptr; int uq_cap = 0;
-  int uq_wpb = 0, uq_bps = 0, uq_stride = 0, uq_stride_large = 0, uq_wpb_large = 0, uq_nlarge = 0, uq_grid = 0;
+  int uq_wpb = 0, uq_stride = 0, uq_stride_large = 0, uq_wpb_large = 0, uq_nlarge = 0, uq_grid = 0;
   size_t uq_smem = 0;
   unsigned long long* uq_prof = nullptr;
   std::vector<double> xpos0_h, xquat0_h;  // world poses of the bodies welded to the world (model constants)
@@ -105,6 +100,14 @@ struct b2s_sim {
   PerturbItem* pert_item = nullptr;
   int pert_nitems = 0;
 };
+
+// Every entry point picks the handle's precision once: f(DModel<R>&, DState<R>&) runs with R = float or double, and
+// real_of<decltype(m)> names R inside a generic lambda.
+template <typename F> static auto with_real(b2s_sim* s, F&& f) { return s->precision == B2S_F32 ? f(s->mf, s->sf) : f(s->md, s->sd); }
+template <typename M> struct RealOf;
+template <typename R> struct RealOf<DModel<R>> { using type = R; };
+template <typename M> using real_of = typename RealOf<std::remove_cv_t<std::remove_reference_t<M>>>::type;
+static size_t real_size(const b2s_sim* s) { return s->precision == B2S_F32 ? sizeof(float) : sizeof(double); }
 
 static int launch_set_const(b2s_sim* s, const uint8_t* mask);  // the set-constants pass (no-op without model overrides)
 
@@ -311,7 +314,7 @@ template <typename R> static void build_model(b2s_sim* s, const Blob& b, DModel<
     for (int64_t i = 0; i < nm; i++) { int v = vn[i]; if (v > n1) { n2 = n1; n1 = v; } else if (v > n2) n2 = v; }
     int need = 24 + ((3 * n1 + 3) & ~3) + ((3 * n2 + 3) & ~3);  // two poses, two hulls
     int cap = (int)(56 * 1024 / sizeof(R));
-    m.stage_cap = getenv("B2S_NO_STAGE") ? 0 : std::min(need, cap);
+    m.stage_cap = std::min(need, cap);
   }
   m.site_bodyid = up_i(s, b, "site_bodyid"); m.site_pos = up_f<R>(s, b, "site_pos"); m.site_quat = up_f<R>(s, b, "site_quat");
   m.act_trnid = up_i(s, b, "actuator_trnid"); m.act_ctrllimited = up_i(s, b, "actuator_ctrllimited");
@@ -337,9 +340,18 @@ template <typename T> static T* dev_zeros(b2s_sim* s, size_t n) {
   s->allocs.push_back(d);
   return d;
 }
+// per precision: the dtype code of its arrays and its constant-memory descriptor banks
 template <typename R> struct DT;
-template <> struct DT<float> { static const int code = B2S_F32; };
-template <> struct DT<double> { static const int code = B2S_F64; };
+template <> struct DT<float> {
+  static const int code = B2S_F32;
+  static const void* model_bank() { return &c_model_f; }
+  static const void* state_bank() { return &c_state_f; }
+};
+template <> struct DT<double> {
+  static const int code = B2S_F64;
+  static const void* model_bank() { return &c_model_d; }
+  static const void* state_bank() { return &c_state_d; }
+};
 
 template <typename R>
 static R* state_arr(b2s_sim* s, const char* name, int64_t d1, int64_t d2 = 0, int64_t d3 = 0) {
@@ -562,7 +574,7 @@ static int fit_wpb(size_t per_warp, int cap) {
   return w;
 }
 static int choose_blocks(b2s_sim* s) {
-  size_t rsz = s->precision == B2S_F32 ? 4 : 8;
+  size_t rsz = real_size(s);
   size_t pw0 = s->lay[LAY_P0].total * rsz, pws = s->lay[LAY_TS].total * rsz, pwl = s->lay[LAY_TL].total * rsz, pwf = s->lay[LAY_FULL].fused_stride * rsz;
   if (std::max(std::max(pw0, pws), std::max(pwl, pwf)) > 226 * 1024) return fail(B2S_ERR_UNSUPPORTED, "model workspace exceeds shared memory");
   // warps per block: as many as the launch bounds allow while B2S_LBx_BLOCKS blocks still fit one SM's shared memory
@@ -575,8 +587,6 @@ static int choose_blocks(b2s_sim* s) {
   s->wpb0 = pick(pw0, B2S_LB0_THREADS, B2S_LB0_BLOCKS);
   s->wpb5s = pick(pws, B2S_LB5_THREADS, B2S_LB5_BLOCKS);
   s->wpb5l = fit_wpb(pwl, B2S_LB5_THREADS / 32);
-  if (const char* v = getenv("B2S_WPB0")) { int x = atoi(v); if (x >= 1 && x <= B2S_LB0_THREADS / 32 && pw0 * x <= 226 * 1024) s->wpb0 = x; }
-  if (const char* v = getenv("B2S_WPB5")) { int x = atoi(v); if (x >= 1 && x <= B2S_LB5_THREADS / 32 && pws * x <= 226 * 1024) s->wpb5s = x; }
   s->smem0 = pw0 * s->wpb0; s->smem5s = pws * s->wpb5s; s->smem5l = pwl * s->wpb5l;
   int wf = fit_wpb(pwf, 16);
   s->wpb_fused = wf; s->smem_fused = pwf * wf;
@@ -630,7 +640,7 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
   if (cudaGetDeviceCount(&ndev) != cudaSuccess || ndev == 0)
     return fail(B2S_ERR_CUDA, "b2s_create: no CUDA device available (this library has no CPU fallback)");
   CUDA_TRY(cudaSetDevice(device));
-  if (!getenv("B2S_NO_LMEM_FLAG")) keep_local_memory_pool();
+  keep_local_memory_pool();
   b2s_sim* s = new b2s_sim();
   s->n_env = n_env; s->device = device; s->precision = precision;
   if (cudaDeviceGetAttribute(&s->num_sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess) {
@@ -657,16 +667,16 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
       for (int64_t i = 0; i < nc; i++) { if (cp[i] == '\n') { v.push_back(cur); cur.clear(); } else cur.push_back((char)cp[i]); }
       if (nc > 0) v.push_back(cur);
     }
-    int ncg, hcs;
-    if (precision == B2S_F32) { build_model(s, b, s->mf); build_state(s, s->mf, s->sf); ncg = s->mf.ncg; hcs = s->mf.hc_stride; }
-    else { build_model(s, b, s->md); build_state(s, s->md, s->sd); ncg = s->md.ncg; hcs = s->md.hc_stride; }
-    s->ncg = ncg; s->hc_stride = hcs;
+    int nfl = 0;
+    with_real(s, [&](auto& m, auto& st) {
+      build_model(s, b, m);
+      build_state(s, m, st);
+      s->ncg = m.ncg; s->hc_stride = m.hc_stride; nfl = m.nfl;
+    });
     // small tail tier: capacities almost every environment of this task stays within (compiled into the model blob by the task
-    // class, B2S_TIER_SMALL="mc,me" overrides); environments that need more are re-run by the large tier
-    int nfl = precision == B2S_F32 ? s->mf.nfl : s->md.nfl;
+    // class); environments that need more are re-run by the large tier
     s->mc_small = b.has("opt_maxcon_small") ? b.scalar_i("opt_maxcon_small") : s->maxcon;
     s->me_small = b.has("opt_maxefc_small") ? b.scalar_i("opt_maxefc_small") : s->maxefc;
-    if (const char* v = getenv("B2S_TIER_SMALL")) { int a_ = 0, b_ = 0; if (sscanf(v, "%d,%d", &a_, &b_) == 2 && a_ > 0 && b_ > 0) { s->mc_small = a_; s->me_small = b_; } }
     s->mc_small = std::min(std::max(s->mc_small, 4), s->maxcon);
     s->me_small = std::min(std::max(s->me_small, nfl + 8), s->maxefc);  // friction-loss rows are always present
     if (s->maxefc < nfl + 8) throw std::string("opt_maxefc too small for the model's friction-loss rows");
@@ -674,7 +684,7 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
     for (int k = 0; k < B2S_NSLOT && s->slot < 0; k++)
       if (!g_slots[device & 63][k]) { g_slots[device & 63][k] = s; s->slot = k; }
     if (s->slot < 0) throw std::string("more than 8 live handles on one device");
-    build_layouts(s, ncg, hcs);
+    build_layouts(s, s->ncg, s->hc_stride);
   } catch (const std::string& e) {
     b2s_destroy(s);
     return fail(B2S_ERR_MODEL, "b2s_create: " + e);
@@ -683,18 +693,14 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
   {
     // the attribute belongs to the FUNCTION, not to the handle: always opt in to the device maximum (a later handle with a
     // smaller workspace must not lower the limit of an earlier one - that broke mixed-task batches in round 1)
-    cudaError_t e1;
-    if (precision == B2S_F32) {
-      e1 = optin_max_smem(step_kernel<float>, device);
-      if (e1 == cudaSuccess) e1 = optin_max_smem(phase0_kernel<float>, device);
-      if (e1 == cudaSuccess) e1 = optin_max_smem(tail_kernel<float>, device);
-      if (e1 == cudaSuccess) e1 = optin_max_smem(phase1_kernel<float>, device);
-    } else {
-      e1 = optin_max_smem(step_kernel<double>, device);
-      if (e1 == cudaSuccess) e1 = optin_max_smem(phase0_kernel<double>, device);
-      if (e1 == cudaSuccess) e1 = optin_max_smem(tail_kernel<double>, device);
-      if (e1 == cudaSuccess) e1 = optin_max_smem(phase1_kernel<double>, device);
-    }
+    cudaError_t e1 = with_real(s, [&](auto& m, auto&) {
+      using R = real_of<decltype(m)>;
+      cudaError_t e = optin_max_smem(step_kernel<R>, device);
+      if (e == cudaSuccess) e = optin_max_smem(phase0_kernel<R>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R>, device);
+      if (e == cudaSuccess) e = optin_max_smem(phase1_kernel<R>, device);
+      return e;
+    });
     if (e1 != cudaSuccess) { std::string msg = cudaGetErrorString(e1); b2s_destroy(s); return fail(B2S_ERR_CUDA, "cudaFuncSetAttribute: " + msg); }
   }
   *out = s;
@@ -721,28 +727,14 @@ void b2s_destroy(b2s_sim* s) {
   for (void* p : s->allocs) cudaFree(p);
   for (auto q : s->gstreams) cudaStreamDestroy(q);
   for (auto ev : s->gevents) cudaEventDestroy(ev);
-  if (s->fork_event) cudaEventDestroy(s->fork_event);
   if (s->in_event) cudaEventDestroy(s->in_event);
-  if (s->out_event) cudaEventDestroy(s->out_event);
   for (auto& kv : s->graphs) cudaGraphExecDestroy(kv.second);
-  if (s->pstream) cudaStreamDestroy(s->pstream);
   delete s;
 }
 
 int b2s_set_stream(b2s_sim* s, void* stream) {
   if (!s) return fail(B2S_ERR_ARG, "null handle");
   s->stream = (cudaStream_t)stream;
-  return B2S_OK;
-}
-
-int b2s_timeline(b2s_sim* s, int enable, double mean_us[8], int count[8]) {
-  if (!s) return fail(B2S_ERR_ARG, "null handle");
-  if (mean_us) for (int k = 0; k < 8; k++) mean_us[k] = s->tl_mean_us[k];
-  if (count) for (int k = 0; k < 8; k++) count[k] = s->tl_count[k];
-  if (enable >= 0) {
-    s->timeline = enable ? (getenv("B2S_TIMELINE") ? 2 : 1) : 0;
-    s->use_graph = enable ? 0 : (getenv("B2S_NO_GRAPH") ? 0 : 1);
-  }
   return B2S_OK;
 }
 
@@ -768,13 +760,13 @@ static int bind_constants(b2s_sim* s) {
   CUDA_TRY(cudaSetDevice(s->device));
   if (!s->dirty) return B2S_OK;
   const size_t k = (size_t)s->slot;
-  if (s->precision == B2S_F32) {
-    CUDA_TRY(cudaMemcpyToSymbolAsync(c_model_f, &s->mf, sizeof(s->mf), k * sizeof(s->mf), cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyToSymbolAsync(c_state_f, &s->sf, sizeof(s->sf), k * sizeof(s->sf), cudaMemcpyHostToDevice, s->stream));
-  } else {
-    CUDA_TRY(cudaMemcpyToSymbolAsync(c_model_d, &s->md, sizeof(s->md), k * sizeof(s->md), cudaMemcpyHostToDevice, s->stream));
-    CUDA_TRY(cudaMemcpyToSymbolAsync(c_state_d, &s->sd, sizeof(s->sd), k * sizeof(s->sd), cudaMemcpyHostToDevice, s->stream));
-  }
+  int rc = with_real(s, [&](auto& m, auto& st) -> int {
+    using D = DT<real_of<decltype(m)>>;
+    CUDA_TRY(cudaMemcpyToSymbolAsync(D::model_bank(), &m, sizeof(m), k * sizeof(m), cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyToSymbolAsync(D::state_bank(), &st, sizeof(st), k * sizeof(st), cudaMemcpyHostToDevice, s->stream));
+    return B2S_OK;
+  });
+  if (rc != B2S_OK) return rc;
   CUDA_TRY(cudaMemcpyToSymbolAsync(c_lay, s->lay, sizeof(s->lay), k * sizeof(s->lay), cudaMemcpyHostToDevice, s->stream));
   CUDA_TRY(cudaMemcpyToSymbolAsync(c_cc, &s->ctrl, sizeof(s->ctrl), k * sizeof(s->ctrl), cudaMemcpyHostToDevice, s->stream));
   CUDA_TRY(cudaMemcpyToSymbolAsync(c_pio, s->pio, sizeof(s->pio), k * sizeof(s->pio), cudaMemcpyHostToDevice, s->stream));
@@ -793,8 +785,7 @@ static int rebuild_layouts(b2s_sim* s) {
   try { build_layouts(s, s->ncg, s->hc_stride); } catch (const std::string& e) { return fail(B2S_ERR_MODEL, e); }
   int rc = choose_blocks(s);
   if (rc != B2S_OK) return rc;
-  bool have_ws = s->precision == B2S_F32 ? s->sf.wsg != nullptr : s->sd.wsg != nullptr;
-  if (have_ws) { cudaSetDevice(s->device); cudaDeviceSynchronize(); }
+  if (with_real(s, [](auto&, auto& st) { return st.wsg != nullptr; })) { cudaSetDevice(s->device); cudaDeviceSynchronize(); }
   for (auto& kv : s->graphs) cudaGraphExecDestroy(kv.second);
   s->graphs.clear();
   s->dirty = 1;
@@ -805,10 +796,10 @@ static int launch(b2s_sim* s, int phases, int nsub, const void* action = nullptr
   int rc = bind_constants(s);
   if (rc != B2S_OK) return rc;
   int blocks = (s->n_env + s->wpb_fused - 1) / s->wpb_fused;
-  if (s->precision == B2S_F32)
-    step_kernel<float><<<blocks, s->wpb_fused * 32, s->smem_fused, s->stream>>>(phases, nsub, (const float*)action, s->slot, mask);
-  else
-    step_kernel<double><<<blocks, s->wpb_fused * 32, s->smem_fused, s->stream>>>(phases, nsub, (const double*)action, s->slot, mask);
+  with_real(s, [&](auto& m, auto&) {
+    using R = real_of<decltype(m)>;
+    step_kernel<R><<<blocks, s->wpb_fused * 32, s->smem_fused, s->stream>>>(phases, nsub, (const R*)action, s->slot, mask);
+  });
   s->launches++;
   CUDA_TRY(cudaGetLastError());
   return B2S_OK;
@@ -816,77 +807,40 @@ static int launch(b2s_sim* s, int phases, int nsub, const void* action = nullptr
 
 }  // extern "C"
 
-// enqueue the launches of `nsub` substeps for every environment group; `q0` is the stream the caller forks from / joins to
 // the launches of `nsub` substeps of ONE environment group on stream q
-template <typename R> static int enqueue_group(b2s_sim* s, DState<R>& st, int phases, int nsub, const R* action, int gi, int G, cudaStream_t q) {
-  const int epaw = (EPA_PIPE_WORDS + (s->precision == B2S_F32 ? s->mf.stage_cap : s->md.stage_cap)) * (int)sizeof(R);
+template <typename R>
+static int enqueue_group(b2s_sim* s, const DModel<R>& m, const DState<R>& st, int phases, int nsub, const R* action, int gi, int G, cudaStream_t q) {
+  const int epaw = (EPA_PIPE_WORDS + m.stage_cap) * (int)sizeof(R);
   const int p1smem = std::max(epaw, (int)osc_smem_bytes<R>());  // one block shape for the three roles of phase 1
   const bool tiered = s->mc_small < s->maxcon || s->me_small < s->maxefc;
-  {
-    int e0 = (int)((long long)s->n_env * gi / G), e1 = (int)((long long)s->n_env * (gi + 1) / G);
-    Grp g{e0, e1 - e0, gi, 0, s->slot};
-    int blocks0 = (g.nenv + s->wpb0 - 1) / s->wpb0, blocks5 = (g.nenv + s->wpb5s - 1) / s->wpb5s;
-    int blocksL = std::min((g.nenv + s->wpb5l - 1) / s->wpb5l, 2 * s->num_sms);  // large tier: warps claim overflowed environments
-    int nA = g.nenv * st.cl_maxa, nG = g.nenv * st.cl_maxg;
-    // convex role: one warp per block, items claimed through a counter.  ~1.6 items per environment are queued per substep (Lift), most of
-    // them dismissed in a few microseconds: half a block per environment keeps every slow item on its own warp without flooding the
-    // block scheduler with thousands of empty blocks per launch (B2S_CVX_BLOCKS overrides)
-    int cvx_blocks = std::max(s->num_sms, g.nenv / 2);
-    if (const char* v = getenv("B2S_CVX_BLOCKS")) { int x = atoi(v); if (x > 0) cvx_blocks = x; }
-    const bool ctrl_ext = (phases & PH_CTRL_EXT) != 0;
-    // B2S_TIMELINE=1 (with B2S_NO_GRAPH=1): timing events between the launches, per-kernel means on stderr (debug aid)
-    auto mark = [&](int type) {
-      if (!s->timeline) return;
-      cudaEvent_t ev; cudaEventCreate(&ev); cudaEventRecord(ev, q);
-      s->tl_events.push_back({gi, type, ev});
-    };
-    for (int sub = 0; sub < nsub; sub++) {
-      g.sub = sub;
-      mark(0);
-      CUDA_TRY(cudaMemsetAsync(st.cl_cnt + 8 * gi, 0, 8 * sizeof(int), q));
-      mark(1);
-      phase0_kernel<R><<<blocks0, s->wpb0 * 32, s->smem0, q>>>(phases, g);
-      mark(2);
-      // phase 1: convex narrow phase | controller | analytic narrow phase as block roles of ONE launch (no forks in the graph).
-      // Upper bounds of the candidate counts size the grid; warps / threads beyond the device-side counts exit at once.
-      {
-        P1Cfg c{(s->debug_skip & 2) ? 0 : std::min(nG, cvx_blocks), ctrl_ext ? (g.nenv + OSC_TPB - 1) / OSC_TPB : 0, sub};
-        int nAb = (s->debug_skip & 1) ? 0 : (nA + 31) / 32;
-        if (c.nG + c.nC + nAb > 0) phase1_kernel<R><<<c.nG + c.nC + nAb, 32, p1smem, q>>>(action, g, c);
-      }
-      mark(4);
-      tail_kernel<R><<<blocks5, s->wpb5s * 32, s->smem5s, q>>>(phases, nsub, action, g, 0);
-      mark(5);
-      if (tiered) {
-        tail_kernel<R><<<blocksL, s->wpb5l * 32, s->smem5l, q>>>(phases, nsub, action, g, 1);
-        mark(6);
-      }
-    }
+  int e0 = (int)((long long)s->n_env * gi / G), e1 = (int)((long long)s->n_env * (gi + 1) / G);
+  Grp g{e0, e1 - e0, gi, 0, s->slot};
+  int blocks0 = (g.nenv + s->wpb0 - 1) / s->wpb0, blocks5 = (g.nenv + s->wpb5s - 1) / s->wpb5s;
+  int blocksL = std::min((g.nenv + s->wpb5l - 1) / s->wpb5l, 2 * s->num_sms);  // large tier: warps claim overflowed environments
+  int nA = g.nenv * st.cl_maxa, nG = g.nenv * st.cl_maxg;
+  // convex role: one warp per block, items claimed through a counter.  ~1.6 items per environment are queued per substep (Lift), most of
+  // them dismissed in a few microseconds: half a block per environment keeps every slow item on its own warp without flooding the
+  // block scheduler with thousands of empty blocks per launch
+  const int cvx_blocks = std::max(s->num_sms, g.nenv / 2);
+  const bool ctrl_ext = (phases & PH_CTRL_EXT) != 0;
+  for (int sub = 0; sub < nsub; sub++) {
+    g.sub = sub;
+    CUDA_TRY(cudaMemsetAsync(st.cl_cnt + 8 * gi, 0, 8 * sizeof(int), q));
+    phase0_kernel<R><<<blocks0, s->wpb0 * 32, s->smem0, q>>>(phases, g);
+    // phase 1: convex narrow phase | controller | analytic narrow phase as block roles of ONE launch (no forks in the graph).
+    // Upper bounds of the candidate counts size the grid; warps / threads beyond the device-side counts exit at once.
+    P1Cfg c{std::min(nG, cvx_blocks), ctrl_ext ? (g.nenv + OSC_TPB - 1) / OSC_TPB : 0, sub};
+    int nAb = (nA + 31) / 32;
+    if (c.nG + c.nC + nAb > 0) phase1_kernel<R><<<c.nG + c.nC + nAb, 32, p1smem, q>>>(action, g, c);
+    tail_kernel<R><<<blocks5, s->wpb5s * 32, s->smem5s, q>>>(phases, nsub, action, g, 0);
+    if (tiered) tail_kernel<R><<<blocksL, s->wpb5l * 32, s->smem5l, q>>>(phases, nsub, action, g, 1);
   }
   CUDA_TRY(cudaGetLastError());
   return B2S_OK;
 }
 
-// all groups, forked from / joined to q0 (eager mode and the single-graph capture)
-template <typename R> static int enqueue_pipeline(b2s_sim* s, DState<R>& st, int phases, int nsub, const R* action, cudaStream_t q0) {
-  int G = s->ngroups;
-  if (G > s->n_env) G = s->n_env;
-  CUDA_TRY(cudaEventRecord(s->fork_event, q0));
-  for (int gi = 0; gi < G; gi++) {
-    cudaStream_t q = G == 1 ? q0 : s->gstreams[gi];
-    if (G > 1) CUDA_TRY(cudaStreamWaitEvent(q, s->fork_event, 0));
-    int rc = enqueue_group<R>(s, st, phases, nsub, action, gi, G, q);
-    if (rc != B2S_OK) return rc;
-    if (G > 1) {
-      CUDA_TRY(cudaEventRecord(s->gevents[gi], q));
-      CUDA_TRY(cudaStreamWaitEvent(q0, s->gevents[gi], 0));
-    }
-  }
-  return B2S_OK;
-}
-
 // global workspace rows + per-environment candidate tables / narrow-phase output slots (pipeline and unit-queue modes)
-template <typename R> static int ensure_ws(b2s_sim* s, DState<R>& st) {
+template <typename R> static int ensure_ws(b2s_sim* s, const DModel<R>& m, DState<R>& st) {
   if (!st.wsg) {
     R* p = nullptr;
     if (cudaMalloc(&p, (size_t)s->n_env * s->lay[LAY_ROW].total * sizeof(R)) != cudaSuccess) return fail(B2S_ERR_CUDA, "cudaMalloc(pipeline workspace) failed");
@@ -899,12 +853,10 @@ template <typename R> static int ensure_ws(b2s_sim* s, DState<R>& st) {
     // candidate capacity per environment: small models keep small grids (the narrow-phase grids are sized by these bounds)
     st.cl_maxa = s->maxcon <= 32 ? 8 : (s->maxcon <= 48 ? 16 : CL_MAXA);
     st.cl_maxg = s->maxcon <= 32 ? 16 : CL_MAXG;
-    if (const char* v = getenv("B2S_CL_MAXA")) { int x = atoi(v); if (x >= 1 && x <= CL_MAXA) st.cl_maxa = x; }
-    if (const char* v = getenv("B2S_CL_MAXG")) { int x = atoi(v); if (x >= 1 && x <= CL_MAXG) st.cl_maxg = x; }
     st.cl_listA = dev_zeros<int>(s, ne * st.cl_maxa); st.cl_listG = dev_zeros<int>(s, ne * st.cl_maxg);
     st.cl_outA = dev_zeros<R>(s, ne * st.cl_maxa * CL_RECA); st.cl_outG = dev_zeros<R>(s, ne * st.cl_maxg * 8);
     st.cl_env = dev_zeros<int>(s, ne * CL_ENVW(st));
-    st.gjk_cache = getenv("B2S_NO_GJK_CACHE") ? nullptr : dev_zeros<R>(s, ne * (size_t)(s->precision == B2S_F32 ? s->mf.npair : s->md.npair) * 3);
+    st.gjk_cache = getenv("B2S_NO_GJK_CACHE") ? nullptr : dev_zeros<R>(s, ne * (size_t)m.npair * 3);
     s->action_buf = dev_zeros<R>(s, ne * 16);
 #ifdef B2S_INSTR
     st.st_begin = dev_zeros<unsigned long long>(s, 64 * 32 * 8); st.st_end = dev_zeros<unsigned long long>(s, 64 * 32 * 8);
@@ -921,73 +873,42 @@ template <typename R> static int ensure_ws(b2s_sim* s, DState<R>& st) {
   return B2S_OK;
 }
 
-template <typename R> static int launch_pipeline_t(b2s_sim* s, DState<R>& st, int phases, int nsub, const R* action) {
-  { int rc0 = ensure_ws<R>(s, st); if (rc0 != B2S_OK) return rc0; }
+// ---- pipeline mode: CUDA-graph replay.  The launch sequence of one environment group (nsub substeps x 3-4 kernels) is captured
+// once per (phases, nsub, action given) and replayed on the group's own stream, forked from and joined to the handle's stream: the
+// groups' chains then overlap freely (inside ONE graph, parallel branches were observed to share a limited number of execution
+// lanes).  The action rows are staged into a fixed buffer so kernel arguments never change.
+static int launch_pipeline(b2s_sim* s, int phases, int nsub, const void* action) {
+  return with_real(s, [&](auto& m, auto& st) -> int {
+    using R = real_of<decltype(m)>;
+    { int rc0 = ensure_ws(s, m, st); if (rc0 != B2S_OK) return rc0; }
 #ifdef B2S_INSTR
-  cudaMemsetAsync(st.st_begin, 0xff, sizeof(unsigned long long) * 64 * 32 * 8, s->stream);
-  cudaMemsetAsync(st.st_end, 0, sizeof(unsigned long long) * 64 * 32 * 8, s->stream);
+    cudaMemsetAsync(st.st_begin, 0xff, sizeof(unsigned long long) * 64 * 32 * 8, s->stream);
+    cudaMemsetAsync(st.st_end, 0, sizeof(unsigned long long) * 64 * 32 * 8, s->stream);
 #endif
-  phases |= PH_WORKLIST;
-  const bool osc = s->ctrl.kind == B2S_CTRL_OSC_POSE || s->ctrl.kind == B2S_CTRL_OSC_POSITION;
-  if ((phases & PH_CTRL) && osc && s->ctrl_split) phases |= PH_CTRL_EXT;
-  { int rc2 = rebuild_layouts(s); if (rc2 != B2S_OK) return rc2; }  // before the descriptors are (re)uploaded
-  int rc = bind_constants(s);
-  if (rc != B2S_OK) return rc;
-  int G = s->ngroups;
-  if (G > s->n_env) G = s->n_env;
-  while ((int)s->gstreams.size() < G) {
-    cudaStream_t st2; cudaEvent_t ev;
-    CUDA_TRY(cudaStreamCreateWithFlags(&st2, cudaStreamNonBlocking));
-    CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-    s->gstreams.push_back(st2); s->gevents.push_back(ev);
-  }
-  if (!s->fork_event) {
-    CUDA_TRY(cudaEventCreateWithFlags(&s->fork_event, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventCreateWithFlags(&s->in_event, cudaEventDisableTiming));
-    CUDA_TRY(cudaEventCreateWithFlags(&s->out_event, cudaEventDisableTiming));
-    CUDA_TRY(cudaStreamCreateWithFlags(&s->pstream, cudaStreamNonBlocking));
-  }
-  // kernels per group-substep: phase 0, analytic + convex narrow phase, then the merged tail (or phases 2, [3], 4)
-  const bool tiered = s->mc_small < s->maxcon || s->me_small < s->maxefc;
-  int launches_per_call = G * nsub * (3 + (tiered ? 1 : 0));  // phase 0, phase 1 (narrow phase + controller), tail, [tail large tier]
-  if (!s->use_graph) {
-    rc = enqueue_pipeline<R>(s, st, phases, nsub, action, s->stream);
-    s->launches += launches_per_call;
-    if (s->timeline && rc == B2S_OK) {
-      cudaStreamSynchronize(s->stream);
-      static const char* names[8] = {"(prev->memset)", "memset", "P0", "narrowA", "narrowG", "tail", "tail(large tier)", "-"};
-      double sum[8] = {0}; int cnt[8] = {0};
-      for (size_t i = 1; i < s->tl_events.size(); i++) {
-        auto &a = s->tl_events[i - 1], &b = s->tl_events[i];
-        if (a.group != b.group) continue;
-        float ms = 0; cudaEventElapsedTime(&ms, a.ev, b.ev);
-        sum[b.type] += ms; cnt[b.type]++;
-      }
-      double tot = 0;
-      for (int k = 0; k < 8; k++) {
-        s->tl_mean_us[k] = cnt[k] ? 1e3 * sum[k] / cnt[k] : 0.0; s->tl_count[k] = cnt[k];
-        if (cnt[k]) tot += sum[k];
-        if (cnt[k] && s->timeline > 1) fprintf(stderr, "[timeline] %-16s n=%4d mean %8.1f us\n", names[k], cnt[k], s->tl_mean_us[k]);
-      }
-      if (s->timeline > 1) fprintf(stderr, "[timeline] sum over one call %.3f ms (all groups)\n", tot);
-      for (auto& t : s->tl_events) cudaEventDestroy(t.ev);
-      s->tl_events.clear();
+    phases |= PH_WORKLIST;
+    const bool osc = s->ctrl.kind == B2S_CTRL_OSC_POSE || s->ctrl.kind == B2S_CTRL_OSC_POSITION;
+    if ((phases & PH_CTRL) && osc && s->ctrl_split) phases |= PH_CTRL_EXT;
+    { int rc2 = rebuild_layouts(s); if (rc2 != B2S_OK) return rc2; }  // before the descriptors are (re)uploaded
+    int rc = bind_constants(s);
+    if (rc != B2S_OK) return rc;
+    const int G = std::min(s->ngroups, s->n_env);
+    while ((int)s->gstreams.size() < G) {
+      cudaStream_t st2; cudaEvent_t ev;
+      CUDA_TRY(cudaStreamCreateWithFlags(&st2, cudaStreamNonBlocking));
+      CUDA_TRY(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+      s->gstreams.push_back(st2); s->gevents.push_back(ev);
     }
-    return rc;
-  }
-  // CUDA-graph replay: the launch sequence of one call (G groups x nsub substeps x 6 kernels) is captured once per
-  // (phases, nsub) on an internal stream; the action rows are staged into a fixed buffer so kernel arguments never change
-  const R* act_in = action;
-  if (action) {
-    int ad = s->ctrl.action_dim > 0 ? s->ctrl.action_dim : 1;
-    if (ad > 16) return fail(B2S_ERR_UNSUPPORTED, "action_dim > 16");
-    CUDA_TRY(cudaMemcpyAsync(s->action_buf, action, (size_t)s->n_env * ad * sizeof(R), cudaMemcpyDeviceToDevice, s->stream));
-    act_in = (const R*)s->action_buf;
-  }
-  CUDA_TRY(cudaEventRecord(s->in_event, s->stream));
-  if (s->graph_per_group && G > 1) {
-    // one graph per environment group, each a plain chain replayed on its own stream: the groups' chains then overlap freely
-    // (inside ONE graph, parallel branches were observed to share a limited number of execution lanes)
+    if (!s->in_event) CUDA_TRY(cudaEventCreateWithFlags(&s->in_event, cudaEventDisableTiming));
+    const bool tiered = s->mc_small < s->maxcon || s->me_small < s->maxefc;
+    const int launches_per_call = G * nsub * (3 + (tiered ? 1 : 0));  // phase 0, phase 1 (narrow phase + controller), tail, [tail large tier]
+    const R* act_in = (const R*)action;
+    if (action) {
+      int ad = s->ctrl.action_dim > 0 ? s->ctrl.action_dim : 1;
+      if (ad > 16) return fail(B2S_ERR_UNSUPPORTED, "action_dim > 16");
+      CUDA_TRY(cudaMemcpyAsync(s->action_buf, action, (size_t)s->n_env * ad * sizeof(R), cudaMemcpyDeviceToDevice, s->stream));
+      act_in = (const R*)s->action_buf;
+    }
+    CUDA_TRY(cudaEventRecord(s->in_event, s->stream));
     for (int gi = 0; gi < G; gi++) {
       long long key = ((long long)phases << 28) | ((long long)(gi + 1) << 20) | (long long)nsub << 4 | (action ? 1 : 0);
       cudaStream_t q = s->gstreams[gi];
@@ -996,7 +917,7 @@ template <typename R> static int launch_pipeline_t(b2s_sim* s, DState<R>& st, in
         cudaGraph_t graph = nullptr;
         cudaGraphExec_t exec = nullptr;
         CUDA_TRY(cudaStreamBeginCapture(q, cudaStreamCaptureModeRelaxed));
-        rc = enqueue_group<R>(s, st, phases, nsub, act_in, gi, G, q);
+        rc = enqueue_group(s, m, st, phases, nsub, act_in, gi, G, q);
         cudaError_t ce = cudaStreamEndCapture(q, &graph);
         if (rc != B2S_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
         if (ce != cudaSuccess) return fail(B2S_ERR_CUDA, std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce));
@@ -1011,107 +932,74 @@ template <typename R> static int launch_pipeline_t(b2s_sim* s, DState<R>& st, in
     }
     s->launches += launches_per_call;
     return B2S_OK;
-  }
-  CUDA_TRY(cudaStreamWaitEvent(s->pstream, s->in_event, 0));
-  long long key = ((long long)phases << 28) | (long long)nsub << 4 | (action ? 1 : 0);
-  auto it = s->graphs.find(key);
-  if (it == s->graphs.end()) {
-    cudaGraph_t graph = nullptr;
-    cudaGraphExec_t exec = nullptr;
-    CUDA_TRY(cudaStreamBeginCapture(s->pstream, cudaStreamCaptureModeRelaxed));
-    rc = enqueue_pipeline<R>(s, st, phases, nsub, act_in, s->pstream);
-    cudaError_t ce = cudaStreamEndCapture(s->pstream, &graph);
-    if (rc != B2S_OK) { if (graph) cudaGraphDestroy(graph); return rc; }
-    if (ce != cudaSuccess) return fail(B2S_ERR_CUDA, std::string("cudaStreamEndCapture: ") + cudaGetErrorString(ce));
-    CUDA_TRY(cudaGraphInstantiate(&exec, graph, 0));
-    cudaGraphDestroy(graph);
-    it = s->graphs.emplace(key, exec).first;
-  }
-  CUDA_TRY(cudaGraphLaunch(it->second, s->pstream));
-  CUDA_TRY(cudaEventRecord(s->out_event, s->pstream));
-  CUDA_TRY(cudaStreamWaitEvent(s->stream, s->out_event, 0));
-  s->launches += launches_per_call;
-  return B2S_OK;
-}
-static int launch_pipeline(b2s_sim* s, int phases, int nsub, const void* action) {
-  return s->precision == B2S_F32 ? launch_pipeline_t<float>(s, s->sf, phases, nsub, (const float*)action)
-                                 : launch_pipeline_t<double>(s, s->sd, phases, nsub, (const double*)action);
+  });
 }
 
 // ---- unit-queue mode: one persistent kernel per control step (b2s_unit.cuh)
-template <typename R> static int launch_unit_t(b2s_sim* s, DState<R>& st, int phases, int nsub, const R* action) {
-  { int rc0 = ensure_ws<R>(s, st); if (rc0 != B2S_OK) return rc0; }
-  { int rc2 = rebuild_layouts(s); if (rc2 != B2S_OK) return rc2; }
-  const int total = s->n_env * nsub;
-  if ((long long)s->n_env * nsub > (1ll << 30)) return fail(B2S_ERR_UNSUPPORTED, "unit-queue mode: n_env * nsub too large");
-  if (total > s->uq_cap) {
-    cudaStreamSynchronize(s->stream);
-    int* p = nullptr;
-    if (cudaMalloc(&p, sizeof(int) * (2 * (size_t)total + 8)) != cudaSuccess) return fail(B2S_ERR_CUDA, "cudaMalloc(unit ring) failed");
-    s->allocs.push_back(p);
-    s->uq_ring = p; s->uq_ovf = p + total; s->uq_ctr = p + 2 * (size_t)total; s->uq_cap = total;
-  }
-  if (s->uq_wpb == 0) {
-    // block shape: the warp's one workspace area holds phase 0's layout, then the EPA polytope + vertex staging, then the small tail tier
-    const size_t rsz = sizeof(R);
-    const bool tiered = s->mc_small < s->maxcon || s->me_small < s->maxefc;
-    int stride = std::max(std::max(s->lay[LAY_P0].total, s->lay[LAY_TS].total), EPA_PIPE_WORDS + 24 + 384);
-    stride = (stride + 3) & ~3;
-    int stride_l = (s->lay[LAY_TL].total + 3) & ~3;
-    CUDA_TRY(optin_max_smem(unit_kernel<R>, s->device));
-    int best_w = 0, best_b = 0, best = 0;
-    int wcap = B2S_LBU_THREADS / 32;
-    if (const char* v = getenv("B2S_UNIT_WPB")) { int x = atoi(v); if (x >= 1 && x <= wcap) wcap = x; }
-    for (int w = wcap; w >= 1; w--) {
-      size_t sm = std::max((size_t)w * stride, tiered ? (size_t)stride_l : 0) * rsz;
-      if (sm > 226 * 1024) continue;
-      int b = 0;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, unit_kernel<R>, w * 32, sm) != cudaSuccess) { cudaGetLastError(); continue; }
-      if (w * b > best) { best = w * b; best_w = w; best_b = b; }
-    }
-    if (best == 0) return fail(B2S_ERR_UNSUPPORTED, "unit-queue mode: workspace does not fit shared memory");
-    cudaDeviceProp prop;
-    CUDA_TRY(cudaGetDeviceProperties(&prop, s->device));
-    s->uq_wpb = best_w; s->uq_bps = best_b; s->uq_stride = stride; s->uq_stride_large = stride_l;
-    s->uq_smem = std::max((size_t)best_w * stride, tiered ? (size_t)stride_l : 0) * rsz;
-    s->uq_wpb_large = tiered ? std::min(best_w, (int)(s->uq_smem / rsz / stride_l)) : 0;
-    int slots = best_b * prop.multiProcessorCount;
-    int nl = 0;
-    if (tiered) {
-      nl = std::max(1, std::min(slots / 64, 12));  // a large-role block occupies a block slot (a whole SM at one block per SM)
-      if (const char* v = getenv("B2S_UNIT_LARGE_BLOCKS")) { int x = atoi(v); if (x >= 1 && x < slots) nl = x; }
-    }
-    s->uq_nlarge = nl;
-    if (best_w > s->n_env) best_w = s->n_env;  // the lockstep rounds need n_env >= warps per block (b2s_unit.cuh)
-    s->uq_wpb = best_w;
-    int small_blocks = std::min(std::max(slots - nl, 1), (s->n_env + best_w - 1) / best_w);
-    if (const char* v = getenv("B2S_UNIT_BLOCKS")) { int x = atoi(v); if (x >= 1) small_blocks = x; }
-    s->uq_grid = nl + small_blocks;
-    if (getenv("B2S_VERBOSE"))
-      fprintf(stderr, "[b2s] unit-queue: %d warps/block x %d blocks/SM, %d words/warp (large role: %d words, %d warps/block, %d blocks), grid %d, smem %zu B\n",
-              best_w, best_b, stride, stride_l, s->uq_wpb_large, nl, s->uq_grid, s->uq_smem);
-  }
-  int rc = bind_constants(s);
-  if (rc != B2S_OK) return rc;
-  if (getenv("B2S_UNIT_PROF") && !s->uq_prof) s->uq_prof = dev_zeros<unsigned long long>(s, 16);
-  UnitQ q{s->uq_ring, s->uq_ovf, s->uq_ctr, total, s->uq_nlarge, s->uq_wpb_large, s->uq_stride, s->uq_stride_large, s->uq_prof};
-  unit_init_kernel<R><<<(total + 255) / 256, 256, 0, s->stream>>>(q, s->n_env);
-  unit_kernel<R><<<s->uq_grid, s->uq_wpb * 32, s->uq_smem, s->stream>>>(phases, nsub, action, s->slot, q);
-  unit_check_kernel<R><<<8, 256, 0, s->stream>>>(q, s->slot);
-  s->launches += 3;
-  CUDA_TRY(cudaGetLastError());
-  if (getenv("B2S_UNIT_DEBUG")) {
-    int c[8];
-    CUDA_TRY(cudaStreamSynchronize(s->stream));
-    CUDA_TRY(cudaMemcpy(c, s->uq_ctr, sizeof(c), cudaMemcpyDeviceToHost));
-    fprintf(stderr, "[b2s] unit ctr: head %d tail %d done %d ovf_head %d ovf_tail %d | watchdog ticket %d tail_then %d flag %d (total %d)\n", c[0], c[1], c[2], c[3], c[4], c[5], c[6], c[7], total);
-    if (c[7]) return fail(B2S_ERR_CUDA, "unit-queue watchdog: a ticket was never produced");
-  }
-  return B2S_OK;
-}
 static int launch_unit(b2s_sim* s, int phases, int nsub, const void* action) {
-  return s->precision == B2S_F32 ? launch_unit_t<float>(s, s->sf, phases, nsub, (const float*)action)
-                                 : launch_unit_t<double>(s, s->sd, phases, nsub, (const double*)action);
+  return with_real(s, [&](auto& m, auto& st) -> int {
+    using R = real_of<decltype(m)>;
+    { int rc0 = ensure_ws(s, m, st); if (rc0 != B2S_OK) return rc0; }
+    { int rc2 = rebuild_layouts(s); if (rc2 != B2S_OK) return rc2; }
+    const int total = s->n_env * nsub;
+    if ((long long)s->n_env * nsub > (1ll << 30)) return fail(B2S_ERR_UNSUPPORTED, "unit-queue mode: n_env * nsub too large");
+    if (total > s->uq_cap) {
+      cudaStreamSynchronize(s->stream);
+      int* p = nullptr;
+      if (cudaMalloc(&p, sizeof(int) * (2 * (size_t)total + 8)) != cudaSuccess) return fail(B2S_ERR_CUDA, "cudaMalloc(unit ring) failed");
+      s->allocs.push_back(p);
+      s->uq_ring = p; s->uq_ovf = p + total; s->uq_ctr = p + 2 * (size_t)total; s->uq_cap = total;
+    }
+    if (s->uq_wpb == 0) {
+      // block shape: the warp's one workspace area holds phase 0's layout, then the EPA polytope + vertex staging, then the small tail tier
+      const size_t rsz = sizeof(R);
+      const bool tiered = s->mc_small < s->maxcon || s->me_small < s->maxefc;
+      int stride = std::max(std::max(s->lay[LAY_P0].total, s->lay[LAY_TS].total), EPA_PIPE_WORDS + 24 + 384);
+      stride = (stride + 3) & ~3;
+      int stride_l = (s->lay[LAY_TL].total + 3) & ~3;
+      CUDA_TRY(optin_max_smem(unit_kernel<R>, s->device));
+      int best_w = 0, best_b = 0, best = 0;
+      for (int w = B2S_LBU_THREADS / 32; w >= 1; w--) {
+        size_t sm = std::max((size_t)w * stride, tiered ? (size_t)stride_l : 0) * rsz;
+        if (sm > 226 * 1024) continue;
+        int b = 0;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, unit_kernel<R>, w * 32, sm) != cudaSuccess) { cudaGetLastError(); continue; }
+        if (w * b > best) { best = w * b; best_w = w; best_b = b; }
+      }
+      if (best == 0) return fail(B2S_ERR_UNSUPPORTED, "unit-queue mode: workspace does not fit shared memory");
+      s->uq_stride = stride; s->uq_stride_large = stride_l;
+      s->uq_smem = std::max((size_t)best_w * stride, tiered ? (size_t)stride_l : 0) * rsz;
+      s->uq_wpb_large = tiered ? std::min(best_w, (int)(s->uq_smem / rsz / stride_l)) : 0;
+      int slots = best_b * s->num_sms;
+      // a large-role block occupies a block slot (a whole SM at one block per SM)
+      int nl = tiered ? std::max(1, std::min(slots / 64, 12)) : 0;
+      s->uq_nlarge = nl;
+      if (best_w > s->n_env) best_w = s->n_env;  // the lockstep rounds need n_env >= warps per block (b2s_unit.cuh)
+      s->uq_wpb = best_w;
+      int small_blocks = std::min(std::max(slots - nl, 1), (s->n_env + best_w - 1) / best_w);
+      s->uq_grid = nl + small_blocks;
+      if (getenv("B2S_VERBOSE"))
+        fprintf(stderr, "[b2s] unit-queue: %d warps/block x %d blocks/SM, %d words/warp (large role: %d words, %d warps/block, %d blocks), grid %d, smem %zu B\n",
+                best_w, best_b, stride, stride_l, s->uq_wpb_large, nl, s->uq_grid, s->uq_smem);
+    }
+    int rc = bind_constants(s);
+    if (rc != B2S_OK) return rc;
+    if (getenv("B2S_UNIT_PROF") && !s->uq_prof) s->uq_prof = dev_zeros<unsigned long long>(s, 16);
+    UnitQ q{s->uq_ring, s->uq_ovf, s->uq_ctr, total, s->uq_nlarge, s->uq_wpb_large, s->uq_stride, s->uq_stride_large, s->uq_prof};
+    unit_init_kernel<R><<<(total + 255) / 256, 256, 0, s->stream>>>(q, s->n_env);
+    unit_kernel<R><<<s->uq_grid, s->uq_wpb * 32, s->uq_smem, s->stream>>>(phases, nsub, (const R*)action, s->slot, q);
+    unit_check_kernel<R><<<8, 256, 0, s->stream>>>(q, s->slot);
+    s->launches += 3;
+    CUDA_TRY(cudaGetLastError());
+    if (getenv("B2S_UNIT_DEBUG")) {
+      int c[8];
+      CUDA_TRY(cudaStreamSynchronize(s->stream));
+      CUDA_TRY(cudaMemcpy(c, s->uq_ctr, sizeof(c), cudaMemcpyDeviceToHost));
+      fprintf(stderr, "[b2s] unit ctr: head %d tail %d done %d ovf_head %d ovf_tail %d | watchdog ticket %d tail_then %d flag %d (total %d)\n", c[0], c[1], c[2], c[3], c[4], c[5], c[6], c[7], total);
+      if (c[7]) return fail(B2S_ERR_CUDA, "unit-queue watchdog: a ticket was never produced");
+    }
+    return B2S_OK;
+  });
 }
 
 extern "C" {
@@ -1146,30 +1034,28 @@ int b2s_set_mode(b2s_sim* s, int mode) {
   s->mode = mode;
   const char* eg = getenv("B2S_GROUPS");
   if (eg) { int v = atoi(eg); if (v >= 1 && v <= 64) s->ngroups = v; }
-  if (getenv("B2S_NO_GRAPH")) s->use_graph = 0;
-  if (const char* ds = getenv("B2S_DEBUG_SKIP")) s->debug_skip = atoi(ds);
-  if (getenv("B2S_TIMELINE")) { s->timeline = 2; s->use_graph = 0; }
   if (const char* v = getenv("B2S_CTRL_SPLIT")) s->ctrl_split = atoi(v) != 0;
-  if (const char* v = getenv("B2S_GRAPH_PER_GROUP")) s->graph_per_group = atoi(v) != 0;
   return B2S_OK;
 }
 
 static void clear_warm_start(b2s_sim* s, const uint8_t* mask) {
-  int npair = s->precision == B2S_F32 ? s->mf.npair : s->md.npair;
-  bool have = s->precision == B2S_F32 ? s->sf.gjk_cache != nullptr : s->sd.gjk_cache != nullptr;
-  if (!have || npair == 0) return;
-  size_t total = (size_t)s->n_env * npair * 3;
-  int blocks = (int)((total + 255) / 256);
-  if (s->precision == B2S_F32) cache_reset_kernel<float><<<blocks, 256, 0, s->stream>>>(mask, s->slot);
-  else cache_reset_kernel<double><<<blocks, 256, 0, s->stream>>>(mask, s->slot);
-  s->launches++;
+  with_real(s, [&](auto& m, auto& st) {
+    using R = real_of<decltype(m)>;
+    if (!st.gjk_cache || m.npair == 0) return;
+    size_t total = (size_t)s->n_env * m.npair * 3;
+    int blocks = (int)((total + 255) / 256);
+    cache_reset_kernel<R><<<blocks, 256, 0, s->stream>>>(mask, s->slot);
+    s->launches++;
+  });
 }
 
 int b2s_reset(b2s_sim* s, const uint8_t* mask) {
   if (!s) return fail(B2S_ERR_ARG, "null handle");
   { int rc = bind_constants(s); if (rc != B2S_OK) return rc; }
-  if (s->precision == B2S_F32) reset_kernel<float><<<(s->n_env + 127) / 128, 128, 0, s->stream>>>(mask, s->slot);
-  else reset_kernel<double><<<(s->n_env + 127) / 128, 128, 0, s->stream>>>(mask, s->slot);
+  with_real(s, [&](auto& m, auto&) {
+    using R = real_of<decltype(m)>;
+    reset_kernel<R><<<(s->n_env + 127) / 128, 128, 0, s->stream>>>(mask, s->slot);
+  });
   clear_warm_start(s, mask);
   s->launches++;
   CUDA_TRY(cudaGetLastError());
@@ -1190,8 +1076,10 @@ int b2s_jac_site(b2s_sim* s, int site_id, void* jacp, void* jacr) {
   if (!s || site_id < 0 || site_id >= s->nsite) return fail(B2S_ERR_ARG, "b2s_jac_site: bad argument");
   { int rc = bind_constants(s); if (rc != B2S_OK) return rc; }
   int threads = 128, blocks = (s->n_env * s->nv + threads - 1) / threads;
-  if (s->precision == B2S_F32) jac_site_kernel<float><<<blocks, threads, 0, s->stream>>>(site_id, (float*)jacp, (float*)jacr, s->slot);
-  else jac_site_kernel<double><<<blocks, threads, 0, s->stream>>>(site_id, (double*)jacp, (double*)jacr, s->slot);
+  with_real(s, [&](auto& m, auto&) {
+    using R = real_of<decltype(m)>;
+    jac_site_kernel<R><<<blocks, threads, 0, s->stream>>>(site_id, (R*)jacp, (R*)jacr, s->slot);
+  });
   s->launches++;
   CUDA_TRY(cudaGetLastError());
   return B2S_OK;
@@ -1202,8 +1090,10 @@ int b2s_get_state(b2s_sim* s, void* out) {
   { int rc = bind_constants(s); if (rc != B2S_OK) return rc; }
   size_t total = (size_t)s->n_env * (1 + s->nq + s->nv);
   int blocks = (int)((total + 255) / 256);
-  if (s->precision == B2S_F32) state_io_kernel<float><<<blocks, 256, 0, s->stream>>>((float*)out, 0, s->slot);
-  else state_io_kernel<double><<<blocks, 256, 0, s->stream>>>((double*)out, 0, s->slot);
+  with_real(s, [&](auto& m, auto&) {
+    using R = real_of<decltype(m)>;
+    state_io_kernel<R><<<blocks, 256, 0, s->stream>>>((R*)out, 0, s->slot);
+  });
   s->launches++;
   CUDA_TRY(cudaGetLastError());
   return B2S_OK;
@@ -1213,8 +1103,10 @@ int b2s_set_state(b2s_sim* s, const void* in) {
   { int rc = bind_constants(s); if (rc != B2S_OK) return rc; }
   size_t total = (size_t)s->n_env * (1 + s->nq + s->nv);
   int blocks = (int)((total + 255) / 256);
-  if (s->precision == B2S_F32) state_io_kernel<float><<<blocks, 256, 0, s->stream>>>((float*)in, 1, s->slot);
-  else state_io_kernel<double><<<blocks, 256, 0, s->stream>>>((double*)in, 1, s->slot);
+  with_real(s, [&](auto& m, auto&) {
+    using R = real_of<decltype(m)>;
+    state_io_kernel<R><<<blocks, 256, 0, s->stream>>>((R*)in, 1, s->slot);
+  });
   s->launches++;
   CUDA_TRY(cudaGetLastError());
   return B2S_OK;
@@ -1234,16 +1126,17 @@ const char* b2s_id2name(const b2s_sim* s, const char* type, int id) {
 }
 int b2s_full_m(b2s_sim* s, void* out) {
   if (!s || !out) return fail(B2S_ERR_ARG, "b2s_full_m: bad argument");
-  size_t rsz = s->precision == B2S_F32 ? 4 : 8;
-  const void* src = s->precision == B2S_F32 ? (const void*)s->sf.qM : (const void*)s->sd.qM;
-  CUDA_TRY(cudaMemcpyAsync(out, src, (size_t)s->n_env * s->nv * s->nv * rsz, cudaMemcpyDeviceToDevice, s->stream));
+  const void* src = with_real(s, [](auto&, auto& st) -> const void* { return st.qM; });
+  CUDA_TRY(cudaMemcpyAsync(out, src, (size_t)s->n_env * s->nv * s->nv * real_size(s), cudaMemcpyDeviceToDevice, s->stream));
   return B2S_OK;
 }
 static int jac_point(b2s_sim* s, int kind, int id, void* jacp, void* jacr) {
   { int rc = bind_constants(s); if (rc != B2S_OK) return rc; }
   int threads = 128, blocks = (s->n_env * s->nv + threads - 1) / threads;
-  if (s->precision == B2S_F32) jac_point_kernel<float><<<blocks, threads, 0, s->stream>>>(kind, id, (float*)jacp, (float*)jacr, s->slot);
-  else jac_point_kernel<double><<<blocks, threads, 0, s->stream>>>(kind, id, (double*)jacp, (double*)jacr, s->slot);
+  with_real(s, [&](auto& m, auto&) {
+    using R = real_of<decltype(m)>;
+    jac_point_kernel<R><<<blocks, threads, 0, s->stream>>>(kind, id, (R*)jacp, (R*)jacr, s->slot);
+  });
   s->launches++;
   CUDA_TRY(cudaGetLastError());
   return B2S_OK;
@@ -1288,8 +1181,10 @@ int b2s_ctrl_reset(b2s_sim* s, const uint8_t* mask) {
   if (!s || !s->has_ctrl) return fail(B2S_ERR_ARG, "b2s_ctrl_reset: controller not configured");
   { int rc = bind_constants(s); if (rc != B2S_OK) return rc; }
   int threads = 128, blocks = (s->n_env + threads - 1) / threads;
-  if (s->precision == B2S_F32) ctrl_reset_kernel<float><<<blocks, threads, 0, s->stream>>>(mask, s->slot);
-  else ctrl_reset_kernel<double><<<blocks, threads, 0, s->stream>>>(mask, s->slot);
+  with_real(s, [&](auto& m, auto&) {
+    using R = real_of<decltype(m)>;
+    ctrl_reset_kernel<R><<<blocks, threads, 0, s->stream>>>(mask, s->slot);
+  });
   clear_warm_start(s, mask);  // an environment whose controller is rebuilt starts a new episode
   s->launches++;
   CUDA_TRY(cudaGetLastError());
@@ -1300,8 +1195,10 @@ int b2s_reset_envs(b2s_sim* s, const uint8_t* mask, const void* qpos_new) {
   if (!s) return fail(B2S_ERR_ARG, "null handle");
   { int rc = bind_constants(s); if (rc != B2S_OK) return rc; }
   int threads = 128, blocks = (s->n_env + threads - 1) / threads;
-  if (s->precision == B2S_F32) reset_envs_kernel<float><<<blocks, threads, 0, s->stream>>>(mask, (const float*)qpos_new, s->slot);
-  else reset_envs_kernel<double><<<blocks, threads, 0, s->stream>>>(mask, (const double*)qpos_new, s->slot);
+  with_real(s, [&](auto& m, auto&) {
+    using R = real_of<decltype(m)>;
+    reset_envs_kernel<R><<<blocks, threads, 0, s->stream>>>(mask, (const R*)qpos_new, s->slot);
+  });
   s->launches++;
   CUDA_TRY(cudaGetLastError());
   { int rc = launch_set_const(s, mask); if (rc != B2S_OK) return rc; }  // after the warn bits were cleared: bit 128 survives
@@ -1325,14 +1222,14 @@ template <typename R> static int body_pose_override_t(b2s_sim* s, DState<R>& st,
   try { st.ov_pos[k] = dev_upload(s, hp); st.ov_quat[k] = dev_upload(s, hq); } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
   st.ov_body[k] = body;
   st.n_ov = k + 1;
-  const int code = s->precision == B2S_F32 ? B2S_F32 : B2S_F64;
+  const int code = DT<R>::code;
   s->arrays["body_xpos_ov:" + std::to_string(body)] = ArrayInfo{st.ov_pos[k], code, 2, {s->n_env, 3, 0, 0}};
   s->arrays["body_xquat_ov:" + std::to_string(body)] = ArrayInfo{st.ov_quat[k], code, 2, {s->n_env, 4, 0, 0}};
   s->dirty = 1;
   return B2S_OK;
 }
 // ---- per-environment model values (b2s_model_override) and the set-constants pass
-static bool has_model_overrides(const b2s_sim* s) { return s->precision == B2S_F32 ? s->sf.dof_iw != nullptr : s->sd.dof_iw != nullptr; }
+static bool has_model_overrides(b2s_sim* s) { return with_real(s, [](auto&, auto& st) { return st.dof_iw != nullptr; }); }
 
 template <typename R> static void upload_rows(R* dst, const double* src, int k, size_t n_env) {  // n_env copies of src[0..k)
   std::vector<R> h(n_env * k);
@@ -1417,18 +1314,19 @@ template <typename R> static int model_override_t(b2s_sim* s, DState<R>& st, con
 static int launch_set_const(b2s_sim* s, const uint8_t* mask) {
   if (!has_model_overrides(s)) return B2S_OK;
   { int rc = bind_constants(s); if (rc != B2S_OK) return rc; }
-  const size_t rsz = s->precision == B2S_F32 ? 4 : 8;
-  if (s->sc_words == 0) {
-    CUDA_TRY(s->precision == B2S_F32 ? optin_max_smem(set_const_kernel<float>, s->device) : optin_max_smem(set_const_kernel<double>, s->device));
-    s->sc_words = s->lay[LAY_FULL].total + ((s->nv * s->nv + 3) & ~3);
-  }
-  const int wpb = fit_wpb((size_t)s->sc_words * rsz, 16), blocks = (s->n_env + wpb - 1) / wpb;
-  const size_t smem = (size_t)s->sc_words * rsz * wpb;
-  if (s->precision == B2S_F32) set_const_kernel<float><<<blocks, wpb * 32, smem, s->stream>>>(mask, s->slot, s->sc_words);
-  else set_const_kernel<double><<<blocks, wpb * 32, smem, s->stream>>>(mask, s->slot, s->sc_words);
-  s->launches++;
-  CUDA_TRY(cudaGetLastError());
-  return B2S_OK;
+  return with_real(s, [&](auto& m, auto&) -> int {
+    using R = real_of<decltype(m)>;
+    if (s->sc_words == 0) {
+      CUDA_TRY(optin_max_smem(set_const_kernel<R>, s->device));
+      s->sc_words = s->lay[LAY_FULL].total + ((s->nv * s->nv + 3) & ~3);
+    }
+    const int wpb = fit_wpb((size_t)s->sc_words * sizeof(R), 16), blocks = (s->n_env + wpb - 1) / wpb;
+    const size_t smem = (size_t)s->sc_words * sizeof(R) * wpb;
+    set_const_kernel<R><<<blocks, wpb * 32, smem, s->stream>>>(mask, s->slot, s->sc_words);
+    s->launches++;
+    CUDA_TRY(cudaGetLastError());
+    return B2S_OK;
+  });
 }
 
 extern "C" {
@@ -1453,7 +1351,7 @@ int b2s_model_override(b2s_sim* s, const char* field, int id) {
                              "dof_damping, dof_armature, dof_frictionloss; a declared geom's solref / solimp come with its slot)");
   }
   CUDA_TRY(cudaSetDevice(s->device));
-  return s->precision == B2S_F32 ? model_override_t<float>(s, s->sf, f, id) : model_override_t<double>(s, s->sd, f, id);
+  return with_real(s, [&](auto&, auto& st) { return model_override_t(s, st, f, id); });
 }
 
 int b2s_set_const(b2s_sim* s, const uint8_t* env_mask) {
@@ -1477,7 +1375,7 @@ int b2s_perturb_config(b2s_sim* s, const b2s_perturb* spec, int n) {
     if (dof && (p.id < -1 || p.id >= s->nv)) return fail(B2S_ERR_ARG, at + "dof id out of range");
     auto it = s->arrays.find(override_key(f, p.id));
     if (it == s->arrays.end()) return fail(B2S_ERR_ARG, at + "the field is not declared (b2s_model_override)");
-    const size_t rsz = s->precision == B2S_F32 ? 4 : 8;
+    const size_t rsz = real_size(s);
     PerturbEntry e{};
     e.mode = p.mode; e.one_draw = p.one_draw != 0; e.amp = p.amplitude;
     const double* model;
@@ -1518,10 +1416,10 @@ int b2s_perturb_model(b2s_sim* s, const uint8_t* env_mask, uint64_t seed, uint64
   const long long total = (long long)s->n_env * s->pert_nitems;
   const int threads = 256;
   const unsigned blocks = (unsigned)((total + threads - 1) / threads);
-  if (s->precision == B2S_F32)
-    perturb_kernel<float><<<blocks, threads, 0, s->stream>>>(s->pert_ent, s->pert_item, s->pert_nitems, s->n_env, env_mask, seed, (unsigned)counter);
-  else
-    perturb_kernel<double><<<blocks, threads, 0, s->stream>>>(s->pert_ent, s->pert_item, s->pert_nitems, s->n_env, env_mask, seed, (unsigned)counter);
+  with_real(s, [&](auto& m, auto&) {
+    using R = real_of<decltype(m)>;
+    perturb_kernel<R><<<blocks, threads, 0, s->stream>>>(s->pert_ent, s->pert_item, s->pert_nitems, s->n_env, env_mask, seed, (unsigned)counter);
+  });
   s->launches++;
   CUDA_TRY(cudaGetLastError());
   return B2S_OK;
@@ -1531,7 +1429,7 @@ int b2s_body_pose_override(b2s_sim* s, int body_id) {
   if (!s || body_id <= 0 || body_id >= s->nbody) return fail(B2S_ERR_ARG, "b2s_body_pose_override: bad argument");
   if (s->body_weldid_h[body_id] != 0) return fail(B2S_ERR_UNSUPPORTED, "b2s_body_pose_override: the body is not welded to the world (move it through qpos)");
   CUDA_TRY(cudaSetDevice(s->device));
-  return s->precision == B2S_F32 ? body_pose_override_t<float>(s, s->sf, body_id) : body_pose_override_t<double>(s, s->sd, body_id);
+  return with_real(s, [&](auto&, auto& st) { return body_pose_override_t(s, st, body_id); });
 }
 
 int b2s_env_step(b2s_sim* s, const void* action, int nsub) {
@@ -1557,8 +1455,10 @@ int b2s_obs_config(b2s_sim* s, int obs_dim, const int* op, const int* a, const i
       if (cudaMemcpy(fresh, ones.data(), sizeof(int) * s->n_env, cudaMemcpyHostToDevice) != cudaSuccess) throw std::string("obs_fresh upload failed");
       cudaStreamSynchronize(cudaStreamLegacy);
     }
-    if (s->precision == B2S_F32) { s->sf.obs = state_arr<float>(s, "obs", obs_dim); s->sf.task_out = state_arr<float>(s, "task_out", 8); s->sf.obs_fresh = fresh; }
-    else { s->sd.obs = state_arr<double>(s, "obs", obs_dim); s->sd.task_out = state_arr<double>(s, "task_out", 8); s->sd.obs_fresh = fresh; }
+    with_real(s, [&](auto& m, auto& st) {
+      using R = real_of<decltype(m)>;
+      st.obs = state_arr<R>(s, "obs", obs_dim); st.task_out = state_arr<R>(s, "task_out", 8); st.obs_fresh = fresh;
+    });
   } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
   s->has_obs = 1;
   s->dirty = 1;
@@ -1584,8 +1484,7 @@ int b2s_task_table(b2s_sim* s, int n, const int* op, const int* a, const int* b)
     std::vector<int> vo(op, op + n), va(a, a + n), vb(b, b + n);
     s->ctrl.task_dim = n;
     s->ctrl.task_op = dev_upload(s, vo); s->ctrl.task_a = dev_upload(s, va); s->ctrl.task_b = dev_upload(s, vb);
-    if (s->precision == B2S_F32) s->sf.task_vec = state_arr<float>(s, "task_vec", n);
-    else s->sd.task_vec = state_arr<double>(s, "task_vec", n);
+    with_real(s, [&](auto& m, auto& st) { st.task_vec = state_arr<real_of<decltype(m)>>(s, "task_vec", n); });
   } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
   s->dirty = 1;
   return B2S_OK;

@@ -101,7 +101,6 @@ def lib():
         L.b2s_task_config.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.b2s_task_config2.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.b2s_task_objects.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
-        L.b2s_timeline.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         L.b2s_task_table.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.b2s_set_export.argtypes = [C.c_void_p, C.c_int]
         L.b2s_set_profile.argtypes = [C.c_void_p, C.c_int]
@@ -331,13 +330,6 @@ class BatchedSim:
         """0 = fused single kernel, 1 = pipelined phase kernels, 2 = unit queue (one persistent kernel per control step);
         identical results"""
         self._check(self._L.b2s_set_mode(self._h, int(mode)))
-
-    def timeline(self, enable=-1):
-        """(mean_us[8], count[8]) of the last timed call; enable=1/0 switches event-timed eager launches on/off"""
-        m = (C.c_double * 8)()
-        n = (C.c_int * 8)()
-        self._check(self._L.b2s_timeline(self._h, int(enable), m, n))
-        return list(m), list(n)
 
     def set_profile(self, flag):
         self._check(self._L.b2s_set_profile(self._h, int(bool(flag))))

@@ -220,19 +220,19 @@ def test_env_step_f32_100_control_steps():
     assert eq < 5e-3 and ev < 1e-2
 
 
-def _scripted_rollout(mode, steps, no_cache, ctrl_split=False, tier_small=None):
+def _scripted_rollout(mode, steps, no_cache, ctrl_split=False, tier_small=None, n=16, groups=None):
+    """groups: B2S_GROUPS for the pipeline (None: the library's default)"""
     import os
     import torch
     from robosuite_b200 import controller_config as cc
     from robosuite_b200.engine import BatchedSim, CtrlCfg
 
     model = load("Lift_Panda")
-    n = 16
     q, v = lift_states(model, n, seed=21)
     rng = np.random.default_rng(3)
     actions = rng.uniform(-1, 1, size=(steps, n, 7))
     actions[:, :, 6] = 1.0  # keep closing the gripper: sliding / sticking finger contacts exercise the friction cones
-    actions[8:, : n // 2, :3] = [0.0, 0.0, -1.0]  # half of the arms push down onto the table / cube
+    actions[8:, : (n + 1) // 2, :3] = [0.0, 0.0, -1.0]  # half of the arms (at least one) push down onto the table / cube
     if no_cache:
         os.environ["B2S_NO_GJK_CACHE"] = "1"
     else:
@@ -243,7 +243,11 @@ def _scripted_rollout(mode, steps, no_cache, ctrl_split=False, tier_small=None):
     sim = BatchedSim(model, n, precision="f32", tier_small=tier_small)
     sim.ctrl_config(cc.resolve(model, cc.default_composite_config(), CtrlCfg))
     sim.set_export(False)
-    sim.set_mode(mode)
+    if groups is not None:
+        os.environ["B2S_GROUPS"] = str(groups)
+    sim.set_mode(mode)  # reads B2S_GROUPS
+    if groups is not None:
+        os.environ.pop("B2S_GROUPS")
     sim.qpos.copy_(torch.as_tensor(q, dtype=torch.float32))
     sim.forward()
     sim.ctrl_reset()

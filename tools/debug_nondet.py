@@ -28,16 +28,12 @@ acts[:, : n // 2, 2] = -1.0
 acts[:, :, 6] = 1.0
 acts_d = torch.as_tensor(acts, dtype=torch.float32, device="cuda")
 NAMES = ["qpos", "qvel", "qacc_warmstart", "ctrl", "ctrl_goal_pos", "ctrl_goal_ori", "ctrl_torque", "warn", "time"]
-KEYS = ["B2S_GROUPS", "B2S_TIER_SMALL", "B2S_CTRL_SPLIT", "B2S_NO_GRAPH", "B2S_NO_STAGE", "B2S_GRAPH_PER_GROUP", "B2S_NO_GJK_CACHE", "B2S_CVX_BLOCKS"]
+KEYS = ["B2S_GROUPS", "B2S_CTRL_SPLIT", "B2S_NO_GJK_CACHE"]
 CONFIGS = [
     ("default", {"B2S_NO_GJK_CACHE": "1"}),
     ("G1", {"B2S_NO_GJK_CACHE": "1", "B2S_GROUPS": "1"}),
-    ("notier", {"B2S_NO_GJK_CACHE": "1", "B2S_TIER_SMALL": "96,288"}),
     ("nosplit", {"B2S_NO_GJK_CACHE": "1", "B2S_CTRL_SPLIT": "0"}),
-    ("nograph", {"B2S_NO_GJK_CACHE": "1", "B2S_NO_GRAPH": "1"}),
-    ("nostage", {"B2S_NO_GJK_CACHE": "1", "B2S_NO_STAGE": "1"}),
-    ("onegraph", {"B2S_NO_GJK_CACHE": "1", "B2S_GRAPH_PER_GROUP": "0"}),
-    ("G1_notier_nosplit", {"B2S_NO_GJK_CACHE": "1", "B2S_GROUPS": "1", "B2S_TIER_SMALL": "96,288", "B2S_CTRL_SPLIT": "0"}),
+    ("G1_nosplit", {"B2S_NO_GJK_CACHE": "1", "B2S_GROUPS": "1", "B2S_CTRL_SPLIT": "0"}),
 ]
 only = os.environ.get("ONLY")
 
