@@ -188,6 +188,38 @@ int b2s_task_objects(b2s_sim* sim, int nobjects, const int* geoms, const int* co
  * (manipulation/door.py:219-266, nut_assembly.py:247-400, pick_place.py:275-425). Requires b2s_obs_config first. */
 int b2s_task_table(b2s_sim* sim, int n, const int* op, const int* a, const int* b);
 
+/* Whole-environment snapshots: everything that decides an environment's next control step, as one opaque byte row per environment,
+ * so that an environment can be saved mid-episode and resumed, or cloned into others, bit-exactly.  A row is made of named SECTIONS
+ * in a fixed order, each 16-byte aligned; the row length is a multiple of 16 bytes.  Sections, each the environment's row of the
+ * handle's own array:
+ *   always           qpos qvel qacc qacc_warmstart ctrl time, warn (i32), ctrl_goal_pos ctrl_goal_ori ctrl_initial_joint ctrl_grip_state
+ *                    ctrl_jv_state ctrl_torque, gjk_cache (npair x 3; written as zeros and ignored on restore while the handle has no
+ *                    cache: fused mode before the pipeline's first use, or B2S_NO_GJK_CACHE)
+ *   b2s_obs_config   obs, obs_fresh (i32), task_out
+ *   b2s_task_table   task_vec
+ *   overrides        body_xpos_ov:<id> body_xquat_ov:<id> per pose override; geom_{size,friction,rbound,aabb,solref,solimp}:<id> per geom
+ *                    slot; body_mass:<id> body_inertia:<id> per body slot; the declared dof vectors; dof_invweight0 body_invweight0
+ *                    meaninertia (copied, not recomputed: a snapshot taken while they were stale restores them stale)
+ * Not in a row: the exported derived arrays (xpos, contacts, efc_*, ...), ncon / nefc / solver_niter, prof / dbg, pipeline workspaces,
+ * and handle configuration (controller gains, obs / task tables, perturbation tables).
+ * The SIGNATURE is a 64-bit FNV-1a hash of the section table (names, counts, dtypes), the precision, the controller kind, the obs and
+ * task op tables and the model blob without its capacity records (opt_maxcon, opt_maxefc and the small-tier pair): rows restore only
+ * into a handle with the same signature (the Python layer checks it; the C layer does not).
+ * A restored environment continues bit-identically to its source under the same actions given the same library build, precision,
+ * mode (b2s_set_mode), B2S_CTRL_SPLIT and B2S_NO_GJK_CACHE, whatever n_env, group count, small tier or neighbours either handle has.
+ * b2s_snapshot_info / b2s_snapshot_section describe the layout (name: valid until the next call that changes it). */
+int b2s_snapshot_info(b2s_sim* sim, size_t* row_bytes, uint64_t* signature, int* nsections);
+int b2s_snapshot_section(b2s_sim* sim, int k, const char** name, int64_t* offset_bytes, int64_t* count, int* dtype);
+/* rows_dev [n_rows, row_bytes] <- environment env_index_host[r] for row r (NULL: every environment in order, n_rows == n_env).
+ * Indices are checked on the host: one out of range returns B2S_ERR_ARG and enqueues nothing. */
+int b2s_snapshot(b2s_sim* sim, void* rows_dev, const int* env_index_host, int n_rows);
+/* environment e <- row src_row_dev[e] (device int32 [n_env], e.g. an argmax computed on the device; NULL: row e, n_rows == n_env).
+ * -1 leaves the environment untouched; an index >= n_rows or < -1 leaves it untouched and sets warn bit 256.  No physics runs: the
+ * exported derived arrays stay stale until the next forward / step (a forward pass would also rewrite qacc, which is observed).  In
+ * pipeline / unit-queue mode the call first creates the GJK cache if the handle has none yet, so that it is restored.  Clone = snapshot
+ * every environment, then restore with a source map.  Both calls are enqueued on the handle's stream without a host synchronisation. */
+int b2s_restore(b2s_sim* sim, const void* rows_dev, int n_rows, const int* src_row_dev);
+
 /* b2s_env_step also exports the derived arrays of its last substep (xpos, contacts, efc ...) when flag != 0 (default 1);
  * the throughput path switches it off so that per-step HBM traffic is state + action + obs only */
 int b2s_set_export(b2s_sim* sim, int flag);

@@ -2,6 +2,7 @@
 // Entry points are declared in include/b2s.h; each cites the reference call it replaces.
 #include "../../include/b2s.h"
 #include "b2s_unit.cuh"
+#include "b2s_snapshot.cuh"
 
 #include <cmath>
 #include <cstdio>
@@ -28,6 +29,9 @@ struct Blob {
     return nullptr;
   }
   bool has(const char* name) const { return find(name) != nullptr; }
+  // FNV-1a of every record (name, dtype, shape, data) except the capacity records: tier choices are bit-exact, so two handles that
+  // differ only in capacities accept each other's snapshots
+  uint64_t hash() const;
   const double* f64(const char* name, int64_t* count = nullptr) const {
     const BlobRec* r = find(name);
     if (!r || r->dtype != 0) throw std::string("model blob: missing f64 field ") + name;
@@ -43,9 +47,30 @@ struct Blob {
   int scalar_i(const char* name) const { return i32(name)[0]; }
   double scalar_f(const char* name) const { return f64(name)[0]; }
 };
+static const uint64_t FNV_BASIS = 1469598103934665603ull;
+static uint64_t fnv1a(uint64_t h, const void* p, size_t n) {
+  const unsigned char* c = (const unsigned char*)p;
+  for (size_t i = 0; i < n; i++) { h ^= c[i]; h *= 1099511628211ull; }
+  return h;
+}
+uint64_t Blob::hash() const {
+  int64_t cnt; memcpy(&cnt, p + 8, 8);
+  const BlobRec* r = (const BlobRec*)(p + 16);
+  uint64_t h = FNV_BASIS;
+  for (int64_t i = 0; i < cnt; i++) {
+    const char* nm = r[i].name;
+    if (!strcmp(nm, "opt_maxcon") || !strcmp(nm, "opt_maxefc") || !strcmp(nm, "opt_maxcon_small") || !strcmp(nm, "opt_maxefc_small")) continue;
+    h = fnv1a(h, nm, strnlen(nm, sizeof(r[i].name)) + 1);
+    h = fnv1a(h, &r[i].dtype, sizeof(int32_t) * 6);  // dtype, ndim, shape
+    h = fnv1a(h, p + r[i].off, (size_t)r[i].nbytes);
+  }
+  return h;
+}
 
 // ------------------------------------------------------------------------------------------------ sim object
 struct ArrayInfo { void* ptr; int dtype; int ndim; int64_t shape[4]; };
+struct SnapSecHost { std::string name; int64_t off, count; int dtype; void* ptr; };  // off: bytes into the row; count: elements per env
+#define SNAP_MAXSEC 128
 
 struct b2s_sim {
   int n_env = 0, device = 0, precision = B2S_F32;
@@ -99,6 +124,14 @@ struct b2s_sim {
   PerturbEntry* pert_ent = nullptr;
   PerturbItem* pert_item = nullptr;
   int pert_nitems = 0;
+  // snapshots (b2s_snapshot / b2s_restore): every entry point that allocates a per-environment array or changes what the signature
+  // covers bumps layout_version; the section table is rebuilt when it differs from snap_version
+  int layout_version = 0, snap_version = -1;
+  std::vector<SnapSecHost> snap;
+  size_t snap_row_bytes = 0;
+  uint64_t snap_sig = 0, blob_hash = 0;  // blob_hash: the model blob without its capacity records
+  SnapSec* snap_dev = nullptr;           // device copy of the section table (capacity SNAP_MAXSEC)
+  std::vector<int> obs_tab_h, task_tab_h;  // host copies of the observation / task op tables (signature)
 };
 
 // Every entry point picks the handle's precision once: f(DModel<R>&, DState<R>&) runs with R = float or double, and
@@ -651,6 +684,7 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
   try {
     s->nq = b.scalar_i("nq"); s->nv = b.scalar_i("nv"); s->nu = b.scalar_i("nu"); s->nbody = b.scalar_i("nbody");
     s->ngeom = b.scalar_i("ngeom"); s->nsite = b.scalar_i("nsite");
+    s->blob_hash = b.hash();
     s->maxcon = b.has("opt_maxcon") ? b.scalar_i("opt_maxcon") : 32;
     s->maxefc = b.has("opt_maxefc") ? b.scalar_i("opt_maxefc") : 64;
     if (s->maxcon > 128) throw std::string("opt_maxcon > 128 not supported");
@@ -869,6 +903,7 @@ template <typename R> static int ensure_ws(b2s_sim* s, const DModel<R>& m, DStat
     s->arrays["slowlog"] = ArrayInfo{st.slowlog, B2S_I32, 2, {64, 12, 0, 0}};
 #endif
     s->dirty = 1;
+    s->layout_version++;  // the GJK cache now exists
   }
   return B2S_OK;
 }
@@ -1174,6 +1209,7 @@ int b2s_ctrl_config(b2s_sim* s, const b2s_ctrl_cfg* c) {
   d.jv_vel_lo = c->jv_vel_lo; d.jv_vel_hi = c->jv_vel_hi; d.jv_use_vel_limits = c->jv_use_vel_limits; d.jv_torque_comp = c->jv_torque_comp;
   s->has_ctrl = c->kind != B2S_CTRL_NONE;
   s->dirty = 1;
+  s->layout_version++;  // the controller kind is part of the snapshot signature
   return B2S_OK;
 }
 
@@ -1226,6 +1262,7 @@ template <typename R> static int body_pose_override_t(b2s_sim* s, DState<R>& st,
   s->arrays["body_xpos_ov:" + std::to_string(body)] = ArrayInfo{st.ov_pos[k], code, 2, {s->n_env, 3, 0, 0}};
   s->arrays["body_xquat_ov:" + std::to_string(body)] = ArrayInfo{st.ov_quat[k], code, 2, {s->n_env, 4, 0, 0}};
   s->dirty = 1;
+  s->layout_version++;
   return B2S_OK;
 }
 // ---- per-environment model values (b2s_model_override) and the set-constants pass
@@ -1308,6 +1345,7 @@ template <typename R> static int model_override_t(b2s_sim* s, DState<R>& st, con
     }
   } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
   s->dirty = 1;
+  s->layout_version++;
   return B2S_OK;
 }
 
@@ -1447,6 +1485,7 @@ int b2s_obs_config(b2s_sim* s, int obs_dim, const int* op, const int* a, const i
   try {
     std::vector<int> vo(op, op + obs_dim), va(a, a + obs_dim), vb(b, b + obs_dim);
     s->ctrl.obs_dim = obs_dim;
+    s->obs_tab_h = vo; s->obs_tab_h.insert(s->obs_tab_h.end(), va.begin(), va.end()); s->obs_tab_h.insert(s->obs_tab_h.end(), vb.begin(), vb.end());
     s->ctrl.obs_op = dev_upload(s, vo); s->ctrl.obs_a = dev_upload(s, va); s->ctrl.obs_b = dev_upload(s, vb);
     if (obs_dim > 128) throw std::string("obs_dim > 128 not supported");
     int* fresh = state_arr_i(s, "obs_fresh", 0);
@@ -1462,6 +1501,7 @@ int b2s_obs_config(b2s_sim* s, int obs_dim, const int* op, const int* a, const i
   } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
   s->has_obs = 1;
   s->dirty = 1;
+  s->layout_version++;
   return B2S_OK;
 }
 
@@ -1483,10 +1523,12 @@ int b2s_task_table(b2s_sim* s, int n, const int* op, const int* a, const int* b)
   try {
     std::vector<int> vo(op, op + n), va(a, a + n), vb(b, b + n);
     s->ctrl.task_dim = n;
+    s->task_tab_h = vo; s->task_tab_h.insert(s->task_tab_h.end(), va.begin(), va.end()); s->task_tab_h.insert(s->task_tab_h.end(), vb.begin(), vb.end());
     s->ctrl.task_op = dev_upload(s, vo); s->ctrl.task_a = dev_upload(s, va); s->ctrl.task_b = dev_upload(s, vb);
     with_real(s, [&](auto& m, auto& st) { st.task_vec = state_arr<real_of<decltype(m)>>(s, "task_vec", n); });
   } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
   s->dirty = 1;
+  s->layout_version++;
   return B2S_OK;
 }
 
@@ -1520,6 +1562,155 @@ int b2s_task_config(b2s_sim* s, int body, int site, const int* left, int nl, con
   s->ctrl.task_body = body; s->ctrl.task_site = site;
   if (s->ctrl.mask_obj2 == 0) s->ctrl.task_body2 = -1;
   s->dirty = 1;
+  return B2S_OK;
+}
+
+}  // extern "C"
+
+// ---- whole-environment snapshots.  The row is the handle's per-environment arrays in a fixed section order, each section 16-byte
+// aligned; the table (and the signature) is rebuilt when an entry point changed what it covers (layout_version).
+static int ensure_snap(b2s_sim* s) {
+  if (s->snap_dev && s->snap_version == s->layout_version) return B2S_OK;
+  std::vector<SnapSecHost> v;
+  int64_t off = 0;
+  auto add = [&](const std::string& name, const void* p, int64_t count, int dtype) {
+    v.push_back(SnapSecHost{name, off, count, dtype, const_cast<void*>(p)});
+    const int64_t es = (dtype == B2S_F64 || dtype == B2S_I64) ? 8 : 4;
+    off += (count * es + 15) & ~(int64_t)15;
+  };
+  with_real(s, [&](auto& m, auto& st) {
+    const int R = DT<real_of<decltype(m)>>::code;
+    const size_t N = s->n_env;
+    add("qpos", st.qpos, m.nq, R); add("qvel", st.qvel, m.nv, R); add("qacc", st.qacc, m.nv, R);
+    add("qacc_warmstart", st.qacc_ws, m.nv, R); add("ctrl", st.ctrl, m.nu, R); add("time", st.time, 1, R);
+    add("warn", st.warn, 1, B2S_I32);
+    add("ctrl_goal_pos", st.goal_pos, 3, R); add("ctrl_goal_ori", st.goal_ori, 9, R); add("ctrl_initial_joint", st.init_qpos_arm, 8, R);
+    add("ctrl_grip_state", st.grip_state, 4, R); add("ctrl_jv_state", st.jv_state, 72, R); add("ctrl_torque", st.ctrl_torque, 8, R);
+    add("gjk_cache", st.gjk_cache, (int64_t)m.npair * 3, R);  // null until the pipeline's first use, or with B2S_NO_GJK_CACHE
+    if (s->has_obs) { add("obs", st.obs, s->ctrl.obs_dim, R); add("obs_fresh", st.obs_fresh, 1, B2S_I32); add("task_out", st.task_out, 8, R); }
+    if (st.task_vec) add("task_vec", st.task_vec, s->ctrl.task_dim, R);
+    for (int k = 0; k < st.n_ov; k++) {
+      const std::string id = std::to_string(st.ov_body[k]);
+      add("body_xpos_ov:" + id, st.ov_pos[k], 3, R); add("body_xquat_ov:" + id, st.ov_quat[k], 4, R);
+    }
+    for (int k = 0; k < st.n_mg; k++) {  // a geom slot carries all six values, whichever field declared it
+      const std::string id = std::to_string(st.mg_id[k]);
+      add("geom_size:" + id, st.mg_size + k * N * 3, 3, R); add("geom_friction:" + id, st.mg_fric + k * N * 3, 3, R);
+      add("geom_rbound:" + id, st.mg_rbound + k * N, 1, R); add("geom_aabb:" + id, st.mg_aabb + k * N * 6, 6, R);
+      add("geom_solref:" + id, st.mg_solref + k * N * 2, 2, R); add("geom_solimp:" + id, st.mg_solimp + k * N * 5, 5, R);
+    }
+    for (int k = 0; k < st.n_mb; k++) {
+      const std::string id = std::to_string(st.mb_id[k]);
+      add("body_mass:" + id, st.mb_mass + k * N, 1, R); add("body_inertia:" + id, st.mb_inertia + k * N * 3, 3, R);
+    }
+    if (st.dof_damp) add("dof_damping", st.dof_damp, m.nv, R);
+    if (st.dof_arm) add("dof_armature", st.dof_arm, m.nv, R);
+    if (st.dof_floss) add("dof_frictionloss", st.dof_floss, m.nv, R);
+    if (st.dof_iw) {  // copied, not recomputed: a snapshot taken while they were stale restores them stale
+      add("dof_invweight0", st.dof_iw, m.nv, R); add("body_invweight0", st.body_iw, 2 * (int64_t)m.nbody, R);
+      add("meaninertia", st.mean_inertia, 1, R);
+    }
+  });
+  if (v.size() > SNAP_MAXSEC) return fail(B2S_ERR_UNSUPPORTED, "snapshot: too many sections");
+  std::vector<SnapSec> dev(v.size());
+  uint64_t h = FNV_BASIS;
+  for (size_t k = 0; k < v.size(); k++) {
+    const SnapSecHost& x = v[k];
+    const int64_t bytes = x.count * ((x.dtype == B2S_F64 || x.dtype == B2S_I64) ? 8 : 4);
+    const int64_t next = k + 1 < v.size() ? v[k + 1].off : off;
+    dev[k] = SnapSec{(char*)x.ptr, (long long)bytes, (int)(x.off / 4), (int)(bytes / 4), (int)((next - x.off) / 4),
+                     ((uintptr_t)x.ptr % 16 == 0 && bytes % 16 == 0) ? 1 : 0};
+    h = fnv1a(h, x.name.c_str(), x.name.size() + 1);
+    h = fnv1a(h, &x.count, sizeof(x.count));
+    h = fnv1a(h, &x.dtype, sizeof(x.dtype));
+  }
+  h = fnv1a(h, &s->precision, sizeof(int));
+  h = fnv1a(h, &s->ctrl.kind, sizeof(int));
+  const int no = (int)s->obs_tab_h.size(), nt = (int)s->task_tab_h.size();
+  h = fnv1a(h, &no, sizeof(int)); h = fnv1a(h, s->obs_tab_h.data(), sizeof(int) * no);
+  h = fnv1a(h, &nt, sizeof(int)); h = fnv1a(h, s->task_tab_h.data(), sizeof(int) * nt);
+  h = fnv1a(h, &s->blob_hash, sizeof(uint64_t));
+  CUDA_TRY(cudaSetDevice(s->device));
+  if (!s->snap_dev) {
+    try { s->snap_dev = dev_zeros<SnapSec>(s, SNAP_MAXSEC); } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
+  }
+  // stream-ordered behind every earlier snapshot / restore of this handle that read the old table
+  if (!dev.empty()) CUDA_TRY(cudaMemcpyAsync(s->snap_dev, dev.data(), dev.size() * sizeof(SnapSec), cudaMemcpyHostToDevice, s->stream));
+  s->snap = v;
+  s->snap_row_bytes = (size_t)off;
+  s->snap_sig = h;
+  s->snap_version = s->layout_version;
+  return B2S_OK;
+}
+
+extern "C" {
+
+int b2s_snapshot_info(b2s_sim* s, size_t* row_bytes, uint64_t* signature, int* nsections) {
+  if (!s) return fail(B2S_ERR_ARG, "null handle");
+  int rc = ensure_snap(s);
+  if (rc != B2S_OK) return rc;
+  if (row_bytes) *row_bytes = s->snap_row_bytes;
+  if (signature) *signature = s->snap_sig;
+  if (nsections) *nsections = (int)s->snap.size();
+  return B2S_OK;
+}
+
+int b2s_snapshot_section(b2s_sim* s, int k, const char** name, int64_t* offset_bytes, int64_t* count, int* dtype) {
+  if (!s) return fail(B2S_ERR_ARG, "null handle");
+  int rc = ensure_snap(s);
+  if (rc != B2S_OK) return rc;
+  if (k < 0 || k >= (int)s->snap.size()) return fail(B2S_ERR_ARG, "b2s_snapshot_section: section index out of range");
+  const SnapSecHost& x = s->snap[k];
+  if (name) *name = x.name.c_str();
+  if (offset_bytes) *offset_bytes = x.off;
+  if (count) *count = x.count;
+  if (dtype) *dtype = x.dtype;
+  return B2S_OK;
+}
+
+int b2s_snapshot(b2s_sim* s, void* rows, const int* env_index, int n_rows) {
+  if (!s || n_rows < 0 || (n_rows > 0 && !rows)) return fail(B2S_ERR_ARG, "b2s_snapshot: bad argument");
+  if (!env_index && n_rows != s->n_env) return fail(B2S_ERR_ARG, "b2s_snapshot: without an index list n_rows must equal n_env");
+  if (env_index)
+    for (int r = 0; r < n_rows; r++)
+      if (env_index[r] < 0 || env_index[r] >= s->n_env)
+        return fail(B2S_ERR_ARG, "b2s_snapshot: environment index " + std::to_string(env_index[r]) + " out of range [0, " + std::to_string(s->n_env) + ")");
+  CUDA_TRY(cudaSetDevice(s->device));
+  int rc = ensure_snap(s);
+  if (rc != B2S_OK) return rc;
+  if (n_rows == 0) return B2S_OK;
+  const int nsec = (int)s->snap.size(), row_words = (int)(s->snap_row_bytes / 4);
+  if (!env_index) {
+    snapshot_kernel<<<(n_rows + 7) / 8, 256, 0, s->stream>>>(s->snap_dev, nsec, row_words, (unsigned char*)rows, n_rows);
+    s->launches++;
+  } else {
+    for (int first = 0; first < n_rows; first += SNAP_IDX) {
+      const int n = std::min(SNAP_IDX, n_rows - first);
+      SnapIdx ix;
+      memcpy(ix.idx, env_index + first, sizeof(int) * n);
+      snapshot_list_kernel<<<(n + 7) / 8, 256, 0, s->stream>>>(s->snap_dev, nsec, row_words, (unsigned char*)rows, first, n, ix);
+      s->launches++;
+    }
+  }
+  CUDA_TRY(cudaGetLastError());
+  return B2S_OK;
+}
+
+int b2s_restore(b2s_sim* s, const void* rows, int n_rows, const int* src_row) {
+  if (!s || n_rows < 0 || (n_rows > 0 && !rows)) return fail(B2S_ERR_ARG, "b2s_restore: bad argument");
+  if (!src_row && n_rows != s->n_env) return fail(B2S_ERR_ARG, "b2s_restore: without a source-row map n_rows must equal n_env");
+  CUDA_TRY(cudaSetDevice(s->device));
+  if (s->mode != 0) {  // the pipeline / unit queue would create a zero GJK cache at their first step: create it now, so it is restored
+    int rc0 = with_real(s, [&](auto& m, auto& st) { return ensure_ws(s, m, st); });
+    if (rc0 != B2S_OK) return rc0;
+  }
+  int rc = ensure_snap(s);
+  if (rc != B2S_OK) return rc;
+  int* warn = with_real(s, [](auto&, auto& st) { return st.warn; });
+  restore_kernel<<<(s->n_env + 7) / 8, 256, 0, s->stream>>>(s->snap_dev, (int)s->snap.size(), (int)(s->snap_row_bytes / 4),
+                                                             (const unsigned char*)rows, n_rows, src_row, s->n_env, warn);
+  s->launches++;
+  CUDA_TRY(cudaGetLastError());
   return B2S_OK;
 }
 

@@ -107,6 +107,11 @@ def lib():
         L.b2s_set_mode.argtypes = [C.c_void_p, C.c_int]
         L.b2s_launch_count.argtypes = [C.c_void_p]
         L.b2s_launch_count.restype = C.c_int64
+        L.b2s_snapshot_info.argtypes = [C.c_void_p, C.POINTER(C.c_size_t), C.POINTER(C.c_uint64), C.POINTER(C.c_int)]
+        L.b2s_snapshot_section.argtypes = [C.c_void_p, C.c_int, C.POINTER(C.c_char_p), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                           C.POINTER(C.c_int)]
+        L.b2s_snapshot.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
+        L.b2s_restore.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
         _LIB = L
     return _LIB
 
@@ -121,6 +126,46 @@ class _DevArray:
 
 
 _TYPESTR = {B2S_F32: "<f4", B2S_F64: "<f8", B2S_I32: "<i4", B2S_I64: "<i8"}
+
+
+_ITEMSIZE = {B2S_F32: 4, B2S_F64: 8, B2S_I32: 4, B2S_I64: 8}
+_PRECISION_NAME = {B2S_F32: "f32", B2S_F64: "f64"}
+
+
+class Snapshot:
+    """Whole-environment snapshot rows (b2s_snapshot): `rows` uint8 [k, row_bytes] (a device tensor, or a numpy array when loaded
+    from a file), `signature` (64-bit, see include/b2s.h), `precision` ("f32" / "f64") and `sections`, a list of
+    (name, offset_bytes, count, dtype code) in row order.  A row holds everything that decides an environment's next control step."""
+
+    def __init__(self, rows, signature, precision, sections):
+        self.rows, self.signature, self.precision = rows, int(signature), str(precision)
+        self.sections = [(str(n), int(o), int(c), int(d)) for n, o, c, d in sections]
+
+    def __len__(self):
+        return int(self.rows.shape[0])
+
+    @property
+    def names(self):
+        return [s[0] for s in self.sections]
+
+    def field(self, name):
+        """typed view [k, count] of one section of every row (a torch view of the device rows, or a numpy view)"""
+        for n, off, cnt, dt in self.sections:
+            if n == name:
+                raw = self.rows[:, off:off + cnt * _ITEMSIZE[dt]]
+                if isinstance(raw, np.ndarray):
+                    return raw.view(np.dtype(_TYPESTR[dt]))
+                import torch
+
+                return raw.view({B2S_F32: torch.float32, B2S_F64: torch.float64, B2S_I32: torch.int32, B2S_I64: torch.int64}[dt])
+        raise KeyError("snapshot has no section %r" % name)
+
+
+def snapshot_mismatch(a_sections, b_sections):
+    """names of the sections that differ (present in one table only, or with another count / dtype) between two section tables"""
+    a = {n: (c, d) for n, _, c, d in a_sections}
+    b = {n: (c, d) for n, _, c, d in b_sections}
+    return sorted(n for n in set(a) | set(b) if a.get(n) != b.get(n))
 
 
 _LIVE = None  # weak set of open BatchedSim objects (a device holds at most B2S_NSLOT = 8 live handles: descriptor slots)
@@ -337,6 +382,69 @@ class BatchedSim:
     @property
     def launch_count(self):
         return int(self._L.b2s_launch_count(self._h))
+
+    # ---- whole-environment snapshots (b2s_snapshot / b2s_restore)
+    def snapshot_layout(self):
+        """(row_bytes, signature, sections) of this handle's snapshot rows as they are now"""
+        rb, sig, ns = C.c_size_t(), C.c_uint64(), C.c_int()
+        self._check(self._L.b2s_snapshot_info(self._h, C.byref(rb), C.byref(sig), C.byref(ns)))
+        cached = self.__dict__.get("_snap_layout")
+        if cached is not None and cached[1] == sig.value:  # the signature covers the section table: unchanged
+            return cached
+        secs = []
+        for k in range(ns.value):
+            nm, off, cnt, dt = C.c_char_p(), C.c_int64(), C.c_int64(), C.c_int()
+            self._check(self._L.b2s_snapshot_section(self._h, k, C.byref(nm), C.byref(off), C.byref(cnt), C.byref(dt)))
+            secs.append((nm.value.decode(), off.value, cnt.value, dt.value))
+        self._snap_layout = (int(rb.value), int(sig.value), secs)
+        return self._snap_layout
+
+    def snapshot(self, env_ids=None):
+        """Snapshot of environments `env_ids` (host list / array of indices, None = all in order): row r holds environment env_ids[r].
+        Enqueued on the handle's stream; an index out of range raises B2SError."""
+        import torch
+
+        rb, sig, secs = self.snapshot_layout()
+        if env_ids is None:
+            idx, k = None, self.n_env
+        else:
+            idx = np.ascontiguousarray(np.asarray(env_ids.cpu() if torch.is_tensor(env_ids) else env_ids, dtype=np.int32).reshape(-1))
+            k = len(idx)
+        rows = torch.empty((k, rb), dtype=torch.uint8, device=self.torch_device)
+        self._check(self._L.b2s_snapshot(self._h, C.c_void_p(rows.data_ptr()), None if idx is None else idx.ctypes.data, k))
+        return Snapshot(rows, sig, _PRECISION_NAME[self.precision], secs)
+
+    def restore(self, snap, src=None):
+        """Environment e takes row src[e] of `snap` (-1 keeps it; src None: row e, needs len(snap) == n_env).  src: a device int32
+        tensor [n_env] (used as is, e.g. an argmax computed on the device) or host indices.  A device entry >= len(snap) or < -1
+        leaves its environment untouched and sets warn bit 256.  No physics runs: the exported derived arrays stay stale until the
+        next forward / step.  ValueError when the snapshot's signature differs from this handle's."""
+        import torch
+
+        rb, sig, secs = self.snapshot_layout()
+        if snap.signature != sig:
+            diff = snapshot_mismatch(snap.sections, secs)
+            why = ("sections differ: " + ", ".join(diff)) if diff else \
+                "same sections, but the model, precision, controller kind or observation / task tables differ"
+            raise ValueError("snapshot signature %#018x does not match this handle's %#018x (%s)" % (snap.signature, sig, why))
+        rows = snap.rows
+        if not torch.is_tensor(rows) or rows.device != self.torch_device:
+            rows = torch.as_tensor(np.asarray(rows) if not torch.is_tensor(rows) else rows, dtype=torch.uint8).to(self.torch_device)
+        rows = rows.contiguous()
+        assert rows.dtype == torch.uint8 and rows.ndim == 2 and rows.shape[1] == rb
+        if src is not None:
+            if torch.is_tensor(src) and src.is_cuda:
+                src = src.to(device=self.torch_device, dtype=torch.int32).contiguous()
+            else:
+                src = torch.as_tensor(np.asarray(src.cpu() if torch.is_tensor(src) else src, dtype=np.int32), device=self.torch_device)
+            assert src.shape == (self.n_env,), "src must hold one source row (or -1) per environment"
+        self._restore_keep = (rows, src)  # alive until the next restore: the copy runs asynchronously on the handle's stream
+        self._check(self._L.b2s_restore(self._h, C.c_void_p(rows.data_ptr()), int(rows.shape[0]),
+                                        None if src is None else C.c_void_p(src.data_ptr())))
+
+    def clone_envs(self, src):
+        """environment e takes the current state of environment src[e] (-1 keeps its own): snapshot of all, then restore"""
+        self.restore(self.snapshot(), src)
 
     # ---- MjSim-style state I/O (binding_utils.py:1155-1184): flattened [time, qpos, qvel] per env
     def get_state(self):

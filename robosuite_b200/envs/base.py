@@ -99,7 +99,8 @@ SIM_WARN_BITS = {1: "singular mass matrix", 2: "non-finite state in the integrat
                  64: "unit-queue watchdog fired: the control step is incomplete (mode 2 only; a library bug, please report)",
                  128: "invalid model override (non-finite or non-positive size, friction, mass or moment, moments violating the "
                       "triangle inequality, non-finite or negative damping, armature or friction loss, or a non-finite solref / "
-                      "solimp component)"}
+                      "solimp component)",
+                 256: "restore source row out of range (b2s_restore): the environment was left untouched"}
 
 
 class BatchedMujocoEnv:
@@ -110,6 +111,9 @@ class BatchedMujocoEnv:
     # capacities of the tail kernel's small tier (contacts, rows): what all but ~0.1 % of this task's environment-substeps stay within
     # under random actions (measured: tools/probe_instr.py); None = no tiering
     tier_small = None
+    # per-environment tensors of the task layer that a snapshot carries besides the engine rows, the episode clocks and `done`
+    # (attribute names; [N, ...] device tensors)
+    _task_state = ()
 
     def __init__(self, robots="Panda", num_envs=1, device=0, controller_configs=None, control_freq=20, horizon=500,
                  ignore_done=False, reward_scale=1.0, reward_shaping=False, use_object_obs=True, seed=None,
@@ -418,6 +422,57 @@ class BatchedMujocoEnv:
 
     def get_state(self):
         return self.sim.get_state()
+
+    # ---- whole-environment snapshots: engine rows (BatchedSim.snapshot) + the episode clocks, `done` and the task's tensors
+    def get_env_state(self, env_ids=None):
+        """Everything that decides the next control steps of environments `env_ids` (host indices, None = all in order), for
+        set_env_state / clone_envs / state_io.save_snapshot(extra=state["tensors"]).  Not included: `rng` and the domain-randomisation
+        counter, which belong to the handle, not to an environment; later draws stay keyed by the destination's index."""
+        import torch
+
+        idx = None if env_ids is None else np.asarray(env_ids.cpu() if torch.is_tensor(env_ids) else env_ids, dtype=np.int64).reshape(-1)
+        sel = slice(None) if idx is None else torch.as_tensor(idx, device=self.device)
+        tensors = {name: getattr(self, name)[sel].clone() for name in ("timestep", "done") + tuple(self._task_state)}
+        host = None if self._host_steps is None else self._host_steps[slice(None) if idx is None else idx].copy()
+        return {"sim": self.sim.snapshot(idx), "tensors": tensors, "host_steps": host, "max_steps": int(self._max_steps_since_reset)}
+
+    def set_env_state(self, state, src=None):
+        """Environment e takes entry src[e] of `state` (get_env_state; -1 keeps it, None: entry e).  src on the host (list / numpy)
+        keeps the host mirror of the episode clocks exact, so BatchedGymWrapper resets a restored environment on its source's
+        schedule; a device tensor (e.g. an argmax) avoids a host round trip, and the mirror becomes unknown as after a device-mask
+        reset.  An index out of range leaves its environment untouched and sets warn bit 256.  No physics runs: observations and task
+        outputs are the source's; the exported derived arrays follow at the next step."""
+        import torch
+
+        k = len(state["sim"])
+        self.sim.restore(state["sim"], src)
+        if src is None:
+            for name, t in state["tensors"].items():
+                getattr(self, name).copy_(t)
+            on_device = False
+            h = np.arange(self.num_envs)
+        else:
+            on_device = torch.is_tensor(src) and src.is_cuda
+            g = src.to(device=self.device, dtype=torch.long) if on_device else torch.as_tensor(
+                np.asarray(src.cpu() if torch.is_tensor(src) else src, dtype=np.int64), device=self.device)
+            ok = (g >= 0) & (g < k)
+            g = g.clamp(0, max(k - 1, 0))
+            for name, t in state["tensors"].items():
+                dst = getattr(self, name)
+                dst.copy_(torch.where(ok.view((-1,) + (1,) * (dst.ndim - 1)), t.to(dst.device)[g], dst))
+            h = None if on_device else np.asarray(src.cpu() if torch.is_tensor(src) else src, dtype=np.int64).reshape(self.num_envs)
+        if on_device or self._host_steps is None or state["host_steps"] is None:
+            self._host_steps = None  # `_max_steps_since_reset` stays an upper bound of every clock
+            self._max_steps_since_reset = max(self._max_steps_since_reset, int(state["max_steps"]))
+        else:
+            ok_h = (h >= 0) & (h < k)
+            self._host_steps[ok_h] = np.asarray(state["host_steps"])[h[ok_h]]
+            self._max_steps_since_reset = int(self._host_steps.max())
+        return self._get_observations()
+
+    def clone_envs(self, src):
+        """environment e continues from the current state of environment src[e] (-1 keeps its own): get_env_state + set_env_state"""
+        return self.set_env_state(self.get_env_state(), src)
 
     def close(self):
         self.sim.close()

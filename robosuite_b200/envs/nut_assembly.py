@@ -20,6 +20,7 @@ class _BatchedNutAssembly(BatchedMujocoEnv):
     nut_to_id = {"square": 0, "round": 1}
     single_object_mode = 0
     nut_id = 0
+    _task_state = ("objects_on_pegs",)  # carried by get_env_state / set_env_state
 
     def _load_model(self, xml):
         return load_task_model("NutAssemblyRound", self.robot_name, xml)  # same composed model for all variants

@@ -22,6 +22,7 @@ class BatchedPickPlace(BatchedMujocoEnv):
     obj_names = ("Milk", "Bread", "Cereal", "Can")
     maxcon, maxefc = 64, 224
     tier_small = (12, 56)  # small tail tier: see BatchedMujocoEnv.tier_small
+    _task_state = ("objects_in_bins",)  # carried by get_env_state / set_env_state
     bin1_pos = np.array([0.1, -0.25, 0.8])   # pick_place.py:186-187
     bin2_pos = np.array([0.1, 0.28, 0.8])
     bin_size = np.array([0.39, 0.49, 0.82])  # BinsArena table_full_size (pick_place.py:184)

@@ -6,6 +6,8 @@
   `state_*.npz` with `states` [T, 1 + nq + nv], `action_infos` (list of {"actions": a}), `successful`, `env`.
   `save_episodes` writes one such folder per environment of a batched rollout, `load_episode` reads one back (also folders
   written by the reference itself), so recorded demonstrations can be replayed on either side with `set_state`.
+* Whole-environment snapshots (`BatchedSim.snapshot`, include/b2s.h): `save_snapshot` / `load_snapshot` keep the rows, the
+  signature, the precision and the section table in one `.npz`, plus optional environment-layer arrays (`extra`).
 
 Host-side numpy only; nothing here touches the GPU."""
 import json
@@ -69,3 +71,65 @@ def load_episode(ep_directory):
     meta = json.load(open(meta_path)) if os.path.exists(meta_path) else {}
     return dict(model_xml=xml, states=np.concatenate(states, axis=0), actions=np.array(actions), successful=successful, env=env,
                 ep_meta=meta)
+
+
+SNAPSHOT_FORMAT = "b2s-snapshot-1"
+
+
+def _check_sections(row_bytes, names, offsets, counts, dtypes):
+    """section table sanity: 16-byte aligned, disjoint, inside the row"""
+    from .engine import _ITEMSIZE
+
+    if row_bytes % 16:
+        raise ValueError("snapshot rows are %d bytes, not a multiple of 16" % row_bytes)
+    end = 0
+    for n, o, c, d in zip(names, offsets, counts, dtypes):
+        if int(d) not in _ITEMSIZE or o % 16 or o < end or c < 0 or o + c * _ITEMSIZE[int(d)] > row_bytes:
+            raise ValueError("snapshot section %r (offset %d, count %d, dtype %d) does not fit the row layout" % (n, o, c, d))
+        end = o + c * _ITEMSIZE[int(d)]
+
+
+def save_snapshot(path, snap, extra=None):
+    """Write a Snapshot (rows copied to the host) and optional named arrays `extra` (e.g. the environment layer's episode clocks and
+    task tensors, numpy or torch) to one .npz file."""
+    rows = snap.rows.cpu().numpy() if hasattr(snap.rows, "cpu") else np.asarray(snap.rows)
+    rows = np.ascontiguousarray(rows, dtype=np.uint8)
+    names = [n for n, *_ in snap.sections]
+    if any("\n" in n for n in names):
+        raise ValueError("section names must not contain newlines")
+    arrays = {"format": np.array(SNAPSHOT_FORMAT), "rows": rows, "signature": np.array(snap.signature, dtype=np.uint64),
+              "precision": np.array(snap.precision), "section_names": np.array("\n".join(names)),
+              "section_offsets": np.array([s[1] for s in snap.sections], dtype=np.int64),
+              "section_counts": np.array([s[2] for s in snap.sections], dtype=np.int64),
+              "section_dtypes": np.array([s[3] for s in snap.sections], dtype=np.int32)}
+    for k, v in (extra or {}).items():
+        arrays["extra/" + k] = np.asarray(v.cpu() if hasattr(v, "cpu") else v)
+    with open(path, "wb") as f:
+        np.savez(f, **arrays)
+
+
+def load_snapshot(path):
+    """-> (Snapshot with host rows, dict of the `extra` arrays).  ValueError for a file that is truncated, not a snapshot, or whose rows
+    and section table disagree."""
+    import zipfile
+
+    from .engine import Snapshot
+
+    try:
+        with np.load(path, allow_pickle=False) as d:
+            z = {k: d[k] for k in d.files}
+    except (zipfile.BadZipFile, OSError, EOFError, ValueError) as e:
+        raise ValueError("%s is not a readable snapshot file: %s" % (path, e)) from None
+    need = ("format", "rows", "signature", "precision", "section_names", "section_offsets", "section_counts", "section_dtypes")
+    missing = [k for k in need if k not in z]
+    if missing or str(z["format"]) != SNAPSHOT_FORMAT:
+        raise ValueError("%s is not a %s file (missing: %s)" % (path, SNAPSHOT_FORMAT, ", ".join(missing) or "-"))
+    rows = z["rows"]
+    names = str(z["section_names"]).split("\n") if str(z["section_names"]) else []
+    offs, cnts, dts = (z[k].astype(np.int64).tolist() for k in ("section_offsets", "section_counts", "section_dtypes"))
+    if rows.dtype != np.uint8 or rows.ndim != 2 or not (len(names) == len(offs) == len(cnts) == len(dts)):
+        raise ValueError("%s: rows or section table malformed" % path)
+    _check_sections(int(rows.shape[1]), names, offs, cnts, dts)
+    snap = Snapshot(rows, int(z["signature"]), str(z["precision"]), list(zip(names, offs, cnts, dts)))
+    extra = {k[len("extra/"):]: v for k, v in z.items() if k.startswith("extra/")}
+    return snap, extra

@@ -112,6 +112,17 @@ class BatchedGymWrapper:
                 obs = self._format(env.reset(mask=done, host_mask=hd))
         return obs, reward, terminated, torch.zeros_like(terminated), info
 
+    def get_env_state(self, env_ids=None):
+        return self.env.get_env_state(env_ids)
+
+    def set_env_state(self, state, src=None):
+        """restore environments (BatchedMujocoEnv.set_env_state) -> the formatted observation.  A restored environment is auto-reset
+        on its source's schedule: exactly through the host mirror of the clocks for host-given `src`, by device mask otherwise."""
+        return self._format(self.env.set_env_state(state, src))
+
+    def clone_envs(self, src):
+        return self._format(self.env.clone_envs(src))
+
     def compute_reward(self, achieved_goal=None, desired_goal=None, info=None):
         return self.env.reward()
 
