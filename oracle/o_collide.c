@@ -1,5 +1,6 @@
 /* TEST INFRASTRUCTURE - CPU oracle, collision detection: static pair list + bounding-sphere cull, analytic narrow
- * phase for plane/sphere/box/cylinder pairs, box-box by separating axes + face clipping, everything else by
+ * phase for plane/sphere/box/cylinder pairs, plane-capsule / plane-ellipsoid, sphere-capsule and capsule-capsule (closest
+ * points of the cores), box-box by separating axes + face clipping, everything else by
  * GJK + EPA on convex supports (one contact per convex pair: the reference models run with multiccd off,
  * `robosuite/models/world.py:11,18`).  Restates SURVEY.md section 8 row a1 "collision"; parity unpinned. */
 #include "b2s_oracle.h"
@@ -175,6 +176,37 @@ static int plane_cylinder(const Shape* p, const Shape* c, OContact* out, int max
   }
   return cnt;
 }
+static int plane_capsule(const Shape* p, const Shape* c, OContact* out, int maxout) {
+  /* one contact per penetrating end sphere of the segment, + end first */
+  double n[3] = COL(p->mat, 2), axis[3] = COL(c->mat, 2), df[3], pos[3];
+  double r = c->size[0], h = c->size[1];
+  v3_sub(df, c->pos, p->pos);
+  double dist0 = v3_dot(df, n), prj = h * v3_dot(n, axis);
+  int cnt = 0;
+  for (int k = 0; k < 2; k++) {
+    double sg = k ? -1.0 : 1.0, dist = dist0 + sg * prj - r;
+    if (dist > 0) continue;
+    v3_addscl(pos, c->pos, axis, sg * h);
+    v3_addscl(pos, pos, n, -(r + 0.5 * dist));
+    cnt = add_contact(out, cnt, maxout, pos, n, dist);
+  }
+  return cnt;
+}
+static int plane_ellipsoid(const Shape* p, const Shape* e, OContact* out, int maxout) {
+  /* support point of the ellipsoid along -n: local -S^2 nl / |S nl| */
+  double n[3] = COL(p->mat, 2), nl[3], df[3], sp[3], w[3], pos[3];
+  m3_mulTv(nl, e->mat, n);
+  double t[3] = {nl[0] * e->size[0], nl[1] * e->size[1], nl[2] * e->size[2]};
+  double len = v3_norm(t);
+  for (int k = 0; k < 3; k++) sp[k] = -t[k] * e->size[k] / len;
+  m3_mulv(w, e->mat, sp);
+  v3_add(w, w, e->pos);
+  v3_sub(df, w, p->pos);
+  double dist = v3_dot(df, n);
+  if (dist > 0) return 0;
+  v3_addscl(pos, w, n, -0.5 * dist);
+  return add_contact(out, 0, maxout, pos, n, dist);
+}
 static int plane_mesh(const Shape* p, const Shape* s, OContact* out, int maxout) {
   /* deepest hull vertex first, then up to three more penetrating vertices chosen greedily far from those taken */
   double n[3] = COL(p->mat, 2), nl[3];
@@ -271,7 +303,8 @@ static int sphere_cylinder(const Shape* s, const Shape* c, OContact* out, int ma
   if (rho <= R && fabs(p[2]) <= h) { /* centre inside the solid cylinder */
     double dside = R - rho, dcap = h - fabs(p[2]);
     double nl[3] = {0, 0, 0};
-    if (dcap < dside || rho < 1e-12) { nl[2] = p[2] >= 0 ? -1 : 1; dist = -dcap - r; }
+    if (dcap < dside) { nl[2] = p[2] >= 0 ? -1 : 1; dist = -dcap - r; }
+    else if (rho < 1e-12) { nl[0] = 1; dist = -dside - r; } /* on the axis, nearer the side: a fixed perpendicular */
     else { nl[0] = -p[0] / rho; nl[1] = -p[1] / rho; dist = -dside - r; }
     m3_mulv(n, c->mat, nl);
   } else {
@@ -287,6 +320,51 @@ static int sphere_cylinder(const Shape* s, const Shape* c, OContact* out, int ma
   }
   v3_addscl(pos, s->pos, n, r + 0.5 * dist);
   return add_contact(out, 0, maxout, pos, n, dist);
+}
+
+/* ------------------------------------------------------------------------------------------------ capsule pairs */
+/* closest points of the segments a + s u (|s| <= ha) and b + t v (|t| <= hb), u and v unit; parallel segments take s = 0 */
+static void seg_seg(const double* a, const double* u, double ha, const double* b, const double* v, double hb, double* p, double* q) {
+  double r[3];
+  v3_sub(r, a, b);
+  double uv = v3_dot(u, v), c = v3_dot(u, r), f = v3_dot(v, r), den = 1 - uv * uv;
+  double s = den > 1e-12 ? fmin(fmax((uv * f - c) / den, -ha), ha) : 0.0;
+  double t = uv * s + f;
+  if (t < -hb || t > hb) {
+    t = fmin(fmax(t, -hb), hb);
+    s = fmin(fmax(uv * t - c, -ha), ha);
+  }
+  v3_addscl(p, a, u, s);
+  v3_addscl(q, b, v, t);
+}
+/* contact of two inflated cores with closest points p (on A's core) and q (on B's); nfb: normal when p == q */
+static int core_contact(const double* p, const double* q, double ra, double rb, const double* nfb, OContact* out, int maxout) {
+  double n[3], pos[3];
+  v3_sub(n, q, p);
+  double len = v3_norm(n), dist = len - ra - rb;
+  if (dist > 0) return 0;
+  if (len < 1e-12) v3_copy(n, nfb); else v3_scl(n, n, 1.0 / len);
+  v3_addscl(pos, p, n, ra + 0.5 * dist);
+  return add_contact(out, 0, maxout, pos, n, dist);
+}
+static int sphere_capsule(const Shape* s, const Shape* c, OContact* out, int maxout) {
+  double axis[3] = COL(c->mat, 2), nfb[3] = COL(c->mat, 0), df[3], q[3];
+  v3_sub(df, s->pos, c->pos);
+  v3_addscl(q, c->pos, axis, fmin(fmax(v3_dot(df, axis), -c->size[1]), c->size[1]));
+  return core_contact(s->pos, q, s->size[0], c->size[0], nfb, out, maxout); /* centre on the segment: a fixed perpendicular */
+}
+static int capsule_capsule(const Shape* A, const Shape* B, OContact* out, int maxout) {
+  double u[3] = COL(A->mat, 2), v[3] = COL(B->mat, 2), p[3], q[3], nfb[3], df[3];
+  seg_seg(A->pos, u, A->size[1], B->pos, v, B->size[1], p, q);
+  /* intersecting cores: crossing axes take their common perpendicular, pointing along the centre difference; collinear ones a
+   * fixed perpendicular of A's axis */
+  v3_cross(nfb, u, v);
+  double len = v3_norm(nfb);
+  if (len > 1e-6) {
+    v3_sub(df, B->pos, A->pos);
+    v3_scl(nfb, nfb, (v3_dot(nfb, df) < 0 ? -1.0 : 1.0) / len);
+  } else v3_set(nfb, A->mat[0], A->mat[3], A->mat[6]);
+  return core_contact(p, q, A->size[0], B->size[0], nfb, out, maxout);
 }
 
 /* ------------------------------------------------------------------------------------------------ box - box */
@@ -595,7 +673,7 @@ static int epa(const Shape* A, const Shape* B, SV* simplex, int ns, double* dept
   if (epa_trace < 0) epa_trace = getenv("B2S_EPA_TRACE") != NULL;
   int nV = 0, nF = 0;
   for (int k = 0; k < ns; k++) V[nV++] = simplex[k];
-  /* grow a degenerate simplex into a tetrahedron */
+  /* grow a degenerate simplex into a tetrahedron (acceptance thresholds relative to the simplex's size, as on the device) */
   static const double dirs[6][3] = {{1, 0, 0}, {-1, 0, 0}, {0, 1, 0}, {0, -1, 0}, {0, 0, 1}, {0, 0, -1}};
   if (nV == 1) {
     for (int k = 0; k < 6 && nV < 2; k++) {
@@ -603,7 +681,7 @@ static int epa(const Shape* A, const Shape* B, SV* simplex, int ns, double* dept
       sv_support(A, B, dirs[k], &w);
       double e[3];
       v3_sub(e, w.w, V[0].w);
-      if (v3_dot(e, e) > 1e-16) V[nV++] = w;
+      if (v3_dot(e, e) > 1e-12) V[nV++] = w;
     }
   }
   if (nV == 2) {
@@ -612,13 +690,13 @@ static int epa(const Shape* A, const Shape* B, SV* simplex, int ns, double* dept
     for (int k = 0; k < 6 && nV < 3; k++) {
       double dir[3];
       v3_cross(dir, ab, dirs[k]);
-      if (v3_dot(dir, dir) < 1e-12) continue;
+      if (v3_dot(dir, dir) < 1e-12 * v3_dot(ab, ab)) continue;
       SV w;
       sv_support(A, B, dir, &w);
       double e[3], cr[3];
       v3_sub(e, w.w, V[0].w);
       v3_cross(cr, ab, e);
-      if (v3_dot(cr, cr) > 1e-20) V[nV++] = w;
+      if (v3_dot(cr, cr) > 1e-12 * v3_dot(ab, ab) * v3_dot(ab, ab)) V[nV++] = w;
     }
   }
   if (nV == 3) {
@@ -633,7 +711,7 @@ static int epa(const Shape* A, const Shape* B, SV* simplex, int ns, double* dept
       sv_support(A, B, dir, &w);
       double e[3];
       v3_sub(e, w.w, V[0].w);
-      if (fabs(v3_dot(e, nrm)) > 1e-14 * (1 + v3_dot(nrm, nrm))) V[nV++] = w;
+      if (fabs(v3_dot(e, nrm)) > 1e-7 * v3_dot(nrm, nrm)) V[nV++] = w;
     }
   }
   if (nV < 4) return -1;
@@ -661,7 +739,7 @@ static int epa(const Shape* A, const Shape* B, SV* simplex, int ns, double* dept
       if (!F[f].alive) continue;
       double e[3];
       v3_sub(e, w.w, V[F[f].v[0]].w);
-      if (v3_dot(F[f].n, e) > 1e-14) {
+      if (v3_dot(F[f].n, e) > 1e-12) {
         F[f].alive = 0;
         for (int k = 0; k < 3; k++) {
           int a = F[f].v[k], b = F[f].v[(k + 1) % 3], found = 0;
@@ -768,10 +846,14 @@ int o_collide_pair(const OModel* m, const OData* d, int g1, int g2, OContact* ou
     else if (t2 == O_GEOM_BOX) n = plane_box(&A, &B, out, maxout);
     else if (t2 == O_GEOM_CYLINDER) n = plane_cylinder(&A, &B, out, maxout);
     else if (t2 == O_GEOM_MESH) n = plane_mesh(&A, &B, out, maxout);
+    else if (t2 == O_GEOM_CAPSULE) n = plane_capsule(&A, &B, out, maxout);
+    else if (t2 == O_GEOM_ELLIPSOID) n = plane_ellipsoid(&A, &B, out, maxout);
     else n = 0;
   } else if (t1 == O_GEOM_SPHERE && t2 == O_GEOM_SPHERE) n = sphere_sphere(&A, &B, out, maxout);
   else if (t1 == O_GEOM_SPHERE && t2 == O_GEOM_BOX) n = sphere_box(&A, &B, out, maxout);
   else if (t1 == O_GEOM_SPHERE && t2 == O_GEOM_CYLINDER) n = sphere_cylinder(&A, &B, out, maxout);
+  else if (t1 == O_GEOM_SPHERE && t2 == O_GEOM_CAPSULE) n = sphere_capsule(&A, &B, out, maxout);
+  else if (t1 == O_GEOM_CAPSULE && t2 == O_GEOM_CAPSULE) n = capsule_capsule(&A, &B, out, maxout);
   else if (t1 == O_GEOM_BOX && t2 == O_GEOM_BOX) n = box_box(&A, &B, out, maxout);
   else n = convex_convex(&A, &B, out, maxout);
   for (int k = 0; k < n; k++) {

@@ -1,5 +1,6 @@
 // Per-warp collision detection: lane-per-pair bounding-sphere + oriented-box culling over the static pair list,
-// lane-per-candidate analytic narrow phase (plane / sphere / box / cylinder), warp-cooperative GJK + EPA for
+// lane-per-candidate analytic narrow phase (plane / sphere / box / cylinder, plane_capsule and plane_ellipsoid, sphere_capsule and
+// capsule_capsule from the closest points of the cores), warp-cooperative GJK + EPA for
 // convex pairs (mesh support scans are split across the 32 lanes).  Contacts come out ordered by pair index.
 // Replaces the collision stage of mj_step1 (robosuite/utils/binding_utils.py:1101-1103), SURVEY.md section 8 a1.
 #pragma once
@@ -141,6 +142,37 @@ template <typename R> DEVN int plane_cylinder(const Shape<R>& p, const Shape<R>&
   }
   return cnt;
 }
+// one contact per penetrating end sphere of the segment, + end first
+template <typename R> DEVN int plane_capsule(const Shape<R>& p, const Shape<R>& c, R* out, int maxn) {
+  R n[3] = COLV(p.mat, 2), axis[3] = COLV(c.mat, 2), df[3], pos[3];
+  R r = c.size[0], h = c.size[1];
+  v3sub(df, c.pos, p.pos);
+  R dist0 = v3dot(df, n), prj = h * v3dot(n, axis);
+  int cnt = 0;
+  for (int k = 0; k < 2; k++) {
+    R sg = k ? R(-1) : R(1), dist = dist0 + sg * prj - r;
+    if (dist > 0) continue;
+    v3addscl(pos, c.pos, axis, sg * h);
+    v3addscl(pos, pos, n, -(r + R(0.5) * dist));
+    cnt = put(out, cnt, maxn, pos, n, dist);
+  }
+  return cnt;
+}
+// support point of the ellipsoid along -n: local -S^2 nl / |S nl|
+template <typename R> DEVN int plane_ellipsoid(const Shape<R>& p, const Shape<R>& e, R* out, int maxn) {
+  R n[3] = COLV(p.mat, 2), nl[3], df[3], sp[3], w[3], pos[3];
+  m3mulTv(nl, e.mat, n);
+  R t[3] = {nl[0] * e.size[0], nl[1] * e.size[1], nl[2] * e.size[2]};
+  R len = v3norm(t);
+  for (int k = 0; k < 3; k++) sp[k] = -t[k] * e.size[k] / len;
+  m3mulv(w, e.mat, sp);
+  v3add(w, w, e.pos);
+  v3sub(df, w, p.pos);
+  R dist = v3dot(df, n);
+  if (dist > 0) return 0;
+  v3addscl(pos, w, n, -R(0.5) * dist);
+  return put(out, 0, maxn, pos, n, dist);
+}
 template <typename R> DEVN int plane_mesh(const Shape<R>& p, const Shape<R>& s, R* out, int maxn) {
   R n[3] = COLV(p.mat, 2), nl[3], df[3];
   m3mulTv(nl, s.mat, n);
@@ -233,7 +265,8 @@ template <typename R> DEVN int sphere_cylinder(const Shape<R>& s, const Shape<R>
   if (rho <= Rc && r_abs(p[2]) <= h) {
     R dside = Rc - rho, dcap = h - r_abs(p[2]);
     R nl[3] = {0, 0, 0};
-    if (dcap < dside || rho < R(1e-12)) { nl[2] = p[2] >= 0 ? R(-1) : R(1); dist = -dcap - r; }
+    if (dcap < dside) { nl[2] = p[2] >= 0 ? R(-1) : R(1); dist = -dcap - r; }
+    else if (rho < R(1e-12)) { nl[0] = R(1); dist = -dside - r; }  // on the axis, nearer the side: a fixed perpendicular
     else { nl[0] = -p[0] / rho; nl[1] = -p[1] / rho; dist = -dside - r; }
     m3mulv(n, c.mat, nl);
   } else {
@@ -249,6 +282,51 @@ template <typename R> DEVN int sphere_cylinder(const Shape<R>& s, const Shape<R>
   }
   v3addscl(pos, s.pos, n, r + R(0.5) * dist);
   return put(out, 0, maxn, pos, n, dist);
+}
+
+// closest points of the segments a + s u (|s| <= ha) and b + t v (|t| <= hb), u and v unit; parallel segments take s = 0
+template <typename R> DEV void seg_seg(const R* a, const R* u, R ha, const R* b, const R* v, R hb, R* p, R* q) {
+  R r[3];
+  v3sub(r, a, b);
+  R uv = v3dot(u, v), c = v3dot(u, r), f = v3dot(v, r), den = 1 - uv * uv;
+  R s = den > R(1e-12) ? r_min(r_max((uv * f - c) / den, -ha), ha) : R(0);
+  R t = uv * s + f;
+  if (t < -hb || t > hb) {
+    t = r_min(r_max(t, -hb), hb);
+    s = r_min(r_max(uv * t - c, -ha), ha);
+  }
+  v3addscl(p, a, u, s);
+  v3addscl(q, b, v, t);
+}
+// contact of two inflated cores with closest points p (on A's core) and q (on B's); nfb: the normal where the cores meet.  fp32 takes
+// core distances below 1e-5 as meeting: at metre-scale coordinates the rounding of p - q is ~1e-7 and its direction is noise
+template <typename R> DEV int core_contact(const R* p, const R* q, R ra, R rb, const R* nfb, R* out, int maxn) {
+  R n[3], pos[3];
+  v3sub(n, q, p);
+  R len = v3norm(n), dist = len - ra - rb;
+  if (dist > 0) return 0;
+  if (len < (sizeof(R) == 4 ? R(1e-5) : R(1e-12))) v3copy(n, nfb); else v3scl(n, n, R(1) / len);
+  v3addscl(pos, p, n, ra + R(0.5) * dist);
+  return put(out, 0, maxn, pos, n, dist);
+}
+template <typename R> DEVN int sphere_capsule(const Shape<R>& s, const Shape<R>& c, R* out, int maxn) {
+  R axis[3] = COLV(c.mat, 2), nfb[3] = COLV(c.mat, 0), df[3], q[3];
+  v3sub(df, s.pos, c.pos);
+  v3addscl(q, c.pos, axis, r_min(r_max(v3dot(df, axis), -c.size[1]), c.size[1]));
+  return core_contact(s.pos, q, s.size[0], c.size[0], nfb, out, maxn);  // centre on the segment: a fixed perpendicular
+}
+template <typename R> DEVN int capsule_capsule(const Shape<R>& A, const Shape<R>& B, R* out, int maxn) {
+  R u[3] = COLV(A.mat, 2), v[3] = COLV(B.mat, 2), p[3], q[3], nfb[3], df[3];
+  seg_seg(A.pos, u, A.size[1], B.pos, v, B.size[1], p, q);
+  // intersecting cores: crossing axes take their common perpendicular, pointing along the centre difference; collinear ones a fixed
+  // perpendicular of A's axis
+  v3cross(nfb, u, v);
+  R len = v3norm(nfb);
+  if (len > R(1e-6)) {
+    v3sub(df, B.pos, A.pos);
+    v3scl(nfb, nfb, (v3dot(nfb, df) < 0 ? R(-1) : R(1)) / len);
+  } else v3set(nfb, A.mat[0], A.mat[3], A.mat[6]);
+  return core_contact(p, q, A.size[0], B.size[0], nfb, out, maxn);
 }
 
 // keep the part of the polygon with sign*coord[axis] <= lim
@@ -960,8 +1038,8 @@ template <typename R> DEVN bool obb_overlap(const Eng<R> e, int g1, int g2) {
 template <typename R> DEV bool is_gjk_pair(int t1, int t2) {
   if (t1 > t2) { int t = t1; t1 = t2; t2 = t; }
   if (t1 == G_PLANE) return false;
-  if (t1 == G_SPHERE && (t2 == G_SPHERE || t2 == G_BOX || t2 == G_CYLINDER)) return false;
-  if (t1 == G_BOX && t2 == G_BOX) return false;
+  if (t1 == G_SPHERE && (t2 == G_SPHERE || t2 == G_CAPSULE || t2 == G_BOX || t2 == G_CYLINDER)) return false;
+  if ((t1 == G_BOX && t2 == G_BOX) || (t1 == G_CAPSULE && t2 == G_CAPSULE)) return false;
   return true;
 }
 
@@ -986,9 +1064,13 @@ template <typename R> DEV int narrow_analytic(const Shape<R>& A, const Shape<R>&
     else if (t2 == G_BOX) n = plane_box(A, B, buf, 8);
     else if (t2 == G_CYLINDER) n = plane_cylinder(A, B, buf, 8);
     else if (t2 == G_MESH) n = plane_mesh(A, B, buf, 8);
+    else if (t2 == G_CAPSULE) n = plane_capsule(A, B, buf, 8);
+    else if (t2 == G_ELLIPSOID) n = plane_ellipsoid(A, B, buf, 8);
   } else if (t1 == G_SPHERE && t2 == G_SPHERE) n = sphere_sphere(A, B, buf, 8);
   else if (t1 == G_SPHERE && t2 == G_BOX) n = sphere_box(A, B, buf, 8);
   else if (t1 == G_SPHERE && t2 == G_CYLINDER) n = sphere_cylinder(A, B, buf, 8);
+  else if (t1 == G_SPHERE && t2 == G_CAPSULE) n = sphere_capsule(A, B, buf, 8);
+  else if (t1 == G_CAPSULE && t2 == G_CAPSULE) n = capsule_capsule(A, B, buf, 8);
   else if (t1 == G_BOX && t2 == G_BOX) n = box_box(A, B, buf, 8);
   return n;
 }
@@ -1110,16 +1192,7 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
       Shape<R> A, B;
       shape_get(e, g1, A);
       shape_get(e, g2, B);
-      int t1 = A.type, t2 = B.type;
-      if (t1 == G_PLANE) {
-        if (t2 == G_SPHERE) n = plane_sphere(A, B, buf, 8);
-        else if (t2 == G_BOX) n = plane_box(A, B, buf, 8);
-        else if (t2 == G_CYLINDER) n = plane_cylinder(A, B, buf, 8);
-        else if (t2 == G_MESH) n = plane_mesh(A, B, buf, 8);
-      } else if (t1 == G_SPHERE && t2 == G_SPHERE) n = sphere_sphere(A, B, buf, 8);
-      else if (t1 == G_SPHERE && t2 == G_BOX) n = sphere_box(A, B, buf, 8);
-      else if (t1 == G_SPHERE && t2 == G_CYLINDER) n = sphere_cylinder(A, B, buf, 8);
-      else if (t1 == G_BOX && t2 == G_BOX) n = box_box(A, B, buf, 8);
+      n = narrow_analytic(A, B, buf);
     }
     // ordered compaction
     int off = n;
