@@ -610,16 +610,16 @@ static int choose_blocks(b2s_sim* s) {
   size_t rsz = real_size(s);
   size_t pw0 = s->lay[LAY_P0].total * rsz, pws = s->lay[LAY_TS].total * rsz, pwl = s->lay[LAY_TL].total * rsz, pwf = s->lay[LAY_FULL].fused_stride * rsz;
   if (std::max(std::max(pw0, pws), std::max(pwl, pwf)) > 226 * 1024) return fail(B2S_ERR_UNSUPPORTED, "model workspace exceeds shared memory");
-  // warps per block: as many as the launch bounds allow while B2S_LBx_BLOCKS blocks still fit one SM's shared memory
+  // warps per block: as many as the launch bounds allow while the launch bounds' blocks per SM still fit one SM's shared memory
   auto pick = [&](size_t pw, int lb_threads, int lb_blocks) {
     int cap = lb_threads / 32, w = cap;
     while (w > 1 && (pw * w + 1024) * lb_blocks > 228 * 1024) w--;  // 1 KB per block is reserved by the system
     if ((pw * w + 1024) * lb_blocks > 228 * 1024) w = fit_wpb(pw, cap);  // cannot reach the block count: largest block that fits
     return w;
   };
-  s->wpb0 = pick(pw0, B2S_LB0_THREADS, B2S_LB0_BLOCKS);
-  s->wpb5s = pick(pws, B2S_LB5_THREADS, B2S_LB5_BLOCKS);
-  s->wpb5l = fit_wpb(pwl, B2S_LB5_THREADS / 32);
+  s->wpb0 = pick(pw0, P0_THREADS, P0_BLOCKS);
+  s->wpb5s = pick(pws, TAIL_THREADS, TAIL_BLOCKS);
+  s->wpb5l = fit_wpb(pwl, TAIL_THREADS / 32);
   s->smem0 = pw0 * s->wpb0; s->smem5s = pws * s->wpb5s; s->smem5l = pwl * s->wpb5l;
   int wf = fit_wpb(pwf, 16);
   s->wpb_fused = wf; s->smem_fused = pwf * wf;
@@ -844,7 +844,7 @@ static int launch(b2s_sim* s, int phases, int nsub, const void* action = nullptr
 // the launches of `nsub` substeps of ONE environment group on stream q
 template <typename R>
 static int enqueue_group(b2s_sim* s, const DModel<R>& m, const DState<R>& st, int phases, int nsub, const R* action, int gi, int G, cudaStream_t q) {
-  const int epaw = (EPA_PIPE_WORDS + m.stage_cap) * (int)sizeof(R);
+  const int epaw = (EPA_AREA_WORDS(EPA_MAXV, EPA_MAXF) + m.stage_cap) * (int)sizeof(R);
   const int p1smem = std::max(epaw, (int)osc_smem_bytes<R>());  // one block shape for the three roles of phase 1
   const bool tiered = s->mc_small < s->maxcon || s->me_small < s->maxefc;
   int e0 = (int)((long long)s->n_env * gi / G), e1 = (int)((long long)s->n_env * (gi + 1) / G);
@@ -989,12 +989,12 @@ static int launch_unit(b2s_sim* s, int phases, int nsub, const void* action) {
       // block shape: the warp's one workspace area holds phase 0's layout, then the EPA polytope + vertex staging, then the small tail tier
       const size_t rsz = sizeof(R);
       const bool tiered = s->mc_small < s->maxcon || s->me_small < s->maxefc;
-      int stride = std::max(std::max(s->lay[LAY_P0].total, s->lay[LAY_TS].total), EPA_PIPE_WORDS + 24 + 384);
+      int stride = std::max(std::max(s->lay[LAY_P0].total, s->lay[LAY_TS].total), EPA_AREA_WORDS(EPA_MAXV, EPA_MAXF) + 24 + 384);
       stride = (stride + 3) & ~3;
       int stride_l = (s->lay[LAY_TL].total + 3) & ~3;
       CUDA_TRY(optin_max_smem(unit_kernel<R>, s->device));
       int best_w = 0, best_b = 0, best = 0;
-      for (int w = B2S_LBU_THREADS / 32; w >= 1; w--) {
+      for (int w = UNIT_THREADS / 32; w >= 1; w--) {
         size_t sm = std::max((size_t)w * stride, tiered ? (size_t)stride_l : 0) * rsz;
         if (sm > 226 * 1024) continue;
         int b = 0;

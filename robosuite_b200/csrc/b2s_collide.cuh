@@ -18,23 +18,6 @@ struct Shape {
 };
 
 template <typename R>
-DEV void shape_get(const Eng<R>& e, int g, Shape<R>& s) {
-  const DModel<R>& m = e.model();
-  int k = m.geom_cgid[g];
-  s.type = m.geom_type[g];
-  s.pos = e.p(e.lay().gpos) + 3 * k;
-  s.mat = e.p(e.lay().gmat) + 9 * k;
-  const R* sz = geom_size_of(m, e.state(), g, e.env);
-  s.size[0] = sz[0]; s.size[1] = sz[1]; s.size[2] = sz[2];
-  s.vert = nullptr; s.nvert = 0;
-  if (s.type == G_MESH) {
-    int id = m.geom_dataid[g];
-    s.vert = m.mesh_vert + 3 * m.mesh_vertadr[id];
-    s.nvert = m.mesh_vertnum[id];
-  }
-}
-
-template <typename R>
 DEV void shape_from(const DModel<R>& m, const DState<R>& st, int env, int g, const R* gpos, const R* gmat, Shape<R>& s) {
   int k = m.geom_cgid[g];
   s.type = m.geom_type[g];
@@ -888,9 +871,6 @@ DEVN int epa(const Shape<R>& A, const Shape<R>& B, R* sx, int ns, R& depth, R* n
 #ifdef B2S_INSTR
   if (lane == 0) { edges[64] = nV; edges[65] = nF; }
 #endif
-#ifdef B2S_CVX_STATS
-  if (lane == 0 && (nF >= maxf - 16 || nV >= maxv - 1)) printf("EPA cap: nV %d nF %d types %d %d depth %.6g\n", nV, nF, A.type, B.type, (double)(bestf >= 0 ? Fn[4 * bestf + 3] : -1));
-#endif
   if (bestf < 0) return -1;
   int fi = Fi[bestf];
   int ia = fi & 255, ib = (fi >> 8) & 255, ic = (fi >> 16) & 255;
@@ -1075,8 +1055,64 @@ template <typename R> DEV int narrow_analytic(const Shape<R>& A, const Shape<R>&
   return n;
 }
 
+// ---- one narrow-phase pair, for all three schedules: the shapes come from the geom poses `gpos` / `gmat` (the fused kernel's workspace,
+// or the environment's workspace row), the contacts are counted and returned as records in `buf`
+
+// the pair's geoms in type order (the narrow-phase routines take the lower type first; contacts carry the geoms in this order)
+template <typename R> DEV void pair_geoms(const DModel<R>& m, int pidx, int& g1, int& g2) {
+  g1 = m.pair_geom[2 * pidx]; g2 = m.pair_geom[2 * pidx + 1];
+  if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
+}
+
+// one analytic pair, one lane: up to 8 records
+template <typename R>
+DEV int narrow_pair_analytic(const DModel<R>& m, const DState<R>& s, int env, int pidx, const R* gpos, const R* gmat, R* buf) {
+  int g1, g2;
+  pair_geoms(m, pidx, g1, g2);
+  Shape<R> A, B;
+  shape_from(m, s, env, g1, gpos, gmat, A);
+  shape_from(m, s, env, g2, gpos, gmat, B);
+  return narrow_analytic(A, B, buf);
+}
+
+// one convex pair, the whole warp: at most one record.  `scratch` holds the EPA polytope; `cache` is the pair's GJK warm-start
+// direction and `stage` (stage_cap words) the hull staging area, or nullptr - the fused kernel passes nullptr for both, so that its
+// results never depend on earlier substeps.  item_stats: -DB2S_INSTR per-item cost histogram and slow-item log (the phase-1 convex role)
+template <typename R>
+DEV int narrow_pair_convex(const DModel<R>& m, const DState<R>& s, int env, int pidx, const R* gpos, const R* gmat, R* buf, R* scratch,
+                           R* cache, R* stage, int stage_cap, int lane, bool item_stats) {
+  int g1, g2;
+  pair_geoms(m, pidx, g1, g2);
+  Shape<R> A, B;
+  shape_from(m, s, env, g1, gpos, gmat, A);
+  shape_from(m, s, env, g2, gpos, gmat, B);
+#ifdef B2S_INSTR
+  long long it0 = clock64();
+#endif
+  int n = convex_convex(A, B, buf, 1, scratch, lane, cache, EPA_MAXV, EPA_MAXF, stage, stage_cap);
+#ifdef B2S_INSTR
+  if (item_stats && lane == 0 && s.stats) {  // bucket k = cycles in [2^(k+8), 2^(k+9)), by shape types (mesh-mesh / other)
+    long long dt = clock64() - it0;
+    int k = 0;
+    while (k < 11 && (dt >> (k + 9)) > 0) k++;
+    atomicAdd(s.stats + 500 - 12 * ((A.type == G_MESH && B.type == G_MESH) ? 2 : 1) + k, 1);
+    if (n > 0) atomicAdd(s.stats + 18, 1);
+    if (dt > (1 << 19) && s.slowlog) {  // items above 524 k cycles (~270 us): what are they?
+      int j = atomicAdd(s.stats + 20, 1);
+      if (j < 64) {
+        const int* sp = reinterpret_cast<const int*>(scratch + 9 * EPA_MAXV + 4 * EPA_MAXF) + EPA_MAXF + 64;
+        int* o = s.slowlog + 12 * j;
+        o[0] = (int)dt; o[1] = A.type; o[2] = B.type; o[3] = A.nvert; o[4] = B.nvert; o[5] = sp[0]; o[6] = sp[1]; o[7] = sp[2]; o[8] = sp[3];
+        o[9] = sp[4]; o[10] = g1; o[11] = g2;
+      }
+    }
+  }
+#endif
+  return n;
+}
+
 // Cull the static pair list (bounding spheres, then oriented boxes); candidate pair indices in pair order.
-template <typename R> DEVN void cull_pairs(Eng<R> e, int* cand, int* cand_g, int maxa, int maxg, int& na_out, int& ng_out) {
+template <typename R> DEV void cull_pairs(Eng<R> e, int* cand, int* cand_g, int maxa, int maxg, int& na_out, int& ng_out) {
   const DModel<R>& m = e.model();
   const DState<R>& st = e.state();
   const WSLayout& L = e.lay();
@@ -1131,52 +1167,26 @@ template <typename R> DEV void finish_contacts(const Eng<R>& e, int ncon) {
   __syncwarp();
 }
 
-// Fills the contact arrays in the workspace; returns ncon (warp-uniform).  warn bit 4 on overflow.
+// The fused kernel's collision stage, composed of the shared pieces: broad phase (at most 96 analytic and 96 convex candidates),
+// analytic candidates one lane each, convex candidates the whole warp each, contacts ordered by pair index, friction / condim mixing.
+// Fills the contact arrays in the workspace; returns ncon (warp-uniform).  warn bit 4 on candidate or contact overflow (the contacts
+// kept are the first maxcon found, analytic before convex).  dbg3: candidate and convex-contact counts; pc: profiler slots 8-10.
 template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc = nullptr) {
   long long tp0 = pc ? clock64() : 0;
 #define CTICK(slot) if (pc) { __syncwarp(); long long tp1 = clock64(); pc[slot] += (float)(tp1 - tp0); tp0 = tp1; }
   const DModel<R>& m = e.model();
   const DState<R>& st = e.state();
   const WSLayout& L = e.lay();
-  int lane = e.lane;
-  int* cand = reinterpret_cast<int*>(e.p(L.scratch));  // candidate pair indices, analytic first then gjk
-  int* cand_g = cand + 96;
-  const int MAXC = 96;
-  int na = 0, ng = 0;
+  const int lane = e.lane, MAXC = 96;
   const R* gpos = e.p(L.gpos); const R* gmat = e.p(L.gmat);
-  for (int base = 0; base < m.npair; base += 32) {
-    int pidx = base + lane;
-    int pass = 0, isg = 0;
-    if (pidx < m.npair) {
-      int g1 = m.pair_geom[2 * pidx], g2 = m.pair_geom[2 * pidx + 1];
-      int t1 = m.geom_type[g1], t2 = m.geom_type[g2];
-      int k1 = m.geom_cgid[g1], k2 = m.geom_cgid[g2];
-      if (t1 != G_PLANE && t2 != G_PLANE) {
-        R df[3];
-        v3sub(df, gpos + 3 * k1, gpos + 3 * k2);
-        R bound = geom_rbound_of(m, st, g1, e.env) + geom_rbound_of(m, st, g2, e.env);
-        pass = v3dot(df, df) <= bound * bound;
-      } else {
-        int kp = t1 == G_PLANE ? k1 : k2, ko = t1 == G_PLANE ? k2 : k1, go = t1 == G_PLANE ? g2 : g1;
-        R nrm[3] = COLV(gmat + 9 * kp, 2), df[3];
-        v3sub(df, gpos + 3 * ko, gpos + 3 * kp);
-        pass = v3dot(df, nrm) <= geom_rbound_of(m, st, go, e.env);
-      }
-      if (pass) pass = obb_overlap(e, g1, g2);
-      isg = is_gjk_pair<R>(t1, t2);
-    }
-    unsigned ma = __ballot_sync(B2S_FULL, pass && !isg), mg = __ballot_sync(B2S_FULL, pass && isg);
-    unsigned lt = (1u << lane) - 1;
-    if (pass && !isg) { int r = na + __popc(ma & lt); if (r < MAXC) cand[r] = pidx; }
-    if (pass && isg) { int r = ng + __popc(mg & lt); if (r < MAXC) cand_g[r] = pidx; }
-    na += __popc(ma);
-    ng += __popc(mg);
-  }
+  int* cand = e.pi(L.scratch);  // candidate pair indices: analytic, convex at +MAXC
+  int* cand_g = cand + MAXC;
+  int na, ng;
+  cull_pairs(e, cand, cand_g, MAXC, MAXC, na, ng);
   dbg3[0] += na; dbg3[1] += ng;
   CTICK(8)
   if (na > MAXC) { na = MAXC; warn |= 4; }
   if (ng > MAXC) { ng = MAXC; warn |= 4; }
-  __syncwarp();
   R* cpos = e.p(L.c_pos); R* cfr = e.p(L.c_frame); R* cdist = e.p(L.c_dist);
   int* cint = e.pi(L.c_int);
   int ncon = 0;
@@ -1187,12 +1197,8 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
     int n = 0, g1 = 0, g2 = 0, pidx = 0;
     if (ci < na) {
       pidx = cand[ci];
-      g1 = m.pair_geom[2 * pidx]; g2 = m.pair_geom[2 * pidx + 1];
-      if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
-      Shape<R> A, B;
-      shape_get(e, g1, A);
-      shape_get(e, g2, B);
-      n = narrow_analytic(A, B, buf);
+      pair_geoms(m, pidx, g1, g2);
+      n = narrow_pair_analytic(m, st, e.env, pidx, gpos, gmat, buf);
     }
     // ordered compaction
     int off = n;
@@ -1214,17 +1220,13 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
   if (ncon > L.mc) { ncon = L.mc; warn |= 4; }
   __syncwarp();
   CTICK(9)
-  // --- convex candidates: the whole warp per pair (scratch beyond the candidate lists holds the EPA polytope)
-  R* epa_scratch = e.ws + L.total;  // the fused kernel appends the EPA polytope area to every warp's workspace
+  // --- convex candidates: the whole warp per pair (the fused kernel appends the EPA polytope area to every warp's workspace)
+  R* epa_scratch = e.ws + L.total;
   for (int ci = 0; ci < ng; ci++) {
-    int pidx = cand_g[ci];
-    int g1 = m.pair_geom[2 * pidx], g2 = m.pair_geom[2 * pidx + 1];
-    if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
-    Shape<R> A, B;
-    shape_get(e, g1, A);
-    shape_get(e, g2, B);
+    int pidx = cand_g[ci], g1, g2;
+    pair_geoms(m, pidx, g1, g2);
     R buf[CREC];
-    int n = convex_convex(A, B, buf, 1, epa_scratch, lane);
+    int n = narrow_pair_convex(m, st, e.env, pidx, gpos, gmat, buf, epa_scratch, (R*)nullptr, (R*)nullptr, 0, lane, false);
     if (n > 0) {
       dbg3[2]++;
       if (ncon < L.mc) {
@@ -1242,12 +1244,8 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
   }
   __syncwarp();
   CTICK(10)
-  // --- order contacts by pair index (stable): rank = #contacts with smaller key
+  // --- order contacts by pair index (stable): up to 32 by rank = #contacts with a smaller key, more by insertion on lane 0
   if (ng > 0 && ncon > 1) {
-    for (int base = 0; base < ncon; base += 32) {
-      // ncon <= 32 is the common case; larger sets are sorted with a simple insertion pass by lane 0
-      if (ncon > 32) break;
-    }
     if (ncon <= 32) {
       int c = lane;
       R rec[7];
@@ -1281,16 +1279,6 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
     }
     __syncwarp();
   }
-  // --- per contact: condim + friction mixing
-  R* cfric = e.p(L.c_fric);
-  for (int c = lane; c < ncon; c += 32) {
-    R f3[3];
-    int dim;
-    mix_contact(m, e.state(), e.env, cint[5 * c], cint[5 * c + 1], f3, dim);
-    cfric[3 * c] = f3[0]; cfric[3 * c + 1] = f3[1]; cfric[3 * c + 2] = f3[2];
-    cint[5 * c + 2] = dim;
-    cint[5 * c + 3] = -1;
-  }
-  __syncwarp();
+  finish_contacts(e, ncon);
   return ncon;
 }

@@ -3,16 +3,28 @@
 #pragma once
 #include "b2s_ctrl.cuh"
 
-#ifndef B2S_BARRIERS
-#define B2S_BARRIERS 4  // block barriers per substep that keep the warps of an SM in the same code region
-#endif
-
 template <typename R> DEV void load_row(R* dst, const R* src, int n, int lane) {
   for (int i = lane; i < n; i += 32) dst[i] = src[i];
 }
 
-// end of an environment's substep(s): state rows, time and warn bits -> global memory (b2s_pipeline.cuh, with the other shared stages)
-template <typename R> DEV void store_state(const Eng<R>& e, int env, R time, int warn);
+// Write-back at the end of step_kernel and of the pipeline's / unit queue's tail: state rows, time and the warn bits of the whole warp -> global memory
+template <typename R> DEV void store_state(const Eng<R>& e, int env, R time, int warn) {
+  const DModel<R>& m = e.model();
+  const DState<R>& s = e.state();
+  const WSLayout& L = e.lay();
+  const int lane = e.lane;
+  const size_t E = env;
+  for (int i = lane; i < m.nq; i += 32) s.qpos[E * m.nq + i] = e.p(L.qpos)[i];
+  for (int i = lane; i < m.nv; i += 32) {
+    s.qvel[E * m.nv + i] = e.p(L.qvel)[i];
+    s.qacc[E * m.nv + i] = e.p(L.qacc)[i];
+    s.qacc_ws[E * m.nv + i] = e.p(L.qacc_ws)[i];
+  }
+  warn = warp_or_i(warn);  // some flags (a dropped contact's rows) are raised on the lane that owns the item
+  if (lane == 0) { s.time[env] = time; s.warn[env] |= warn; }
+  __syncwarp();
+}
+
 
 template <typename R>
 DEVN void export_step1(const Eng<R> e, int env, int ncon) {
@@ -132,12 +144,12 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
   int dbgc[3] = {0, 0, 0};
   long long t0 = 0;
 #define TICK(slot) if (prof) { long long t1 = clock64(); pc[slot] += (float)(t1 - t0); t0 = t1; }
-#define BAR(level, slot) if (B2S_BARRIERS >= level) { __syncthreads(); TICK(slot) }
+#define BAR { __syncthreads(); TICK(11) }
   for (int sub = 0; sub < nsub; sub++) {
     int ncon = 0, nefc = 0, niter = 0;
     bool ex = live && (phases & PH_EXPORT) && sub == nsub - 1;
     if (prof) t0 = clock64();
-    BAR(1, 11)
+    BAR
     if (phases & PH_STEP1) {
       if (e.kinematics()) {  // diverged state reset to the model defaults (mj_checkPos / mj_checkVel)
         for (int i = lane; i < m.nv; i += 32) { e.p(L.qacc)[i] = 0; e.p(L.qacc_ws)[i] = 0; }
@@ -148,27 +160,25 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
       e.velocity();
       e.crb();
       TICK(1)
-      BAR(3, 11)
+      BAR
       ncon = collide(e, warn, dbgc, prof ? pc : (float*)nullptr);
       TICK(2)
       if (ex) export_step1(e, env, ncon);
-      BAR(4, 11)
+      BAR
       nefc = make_constraint(e, ncon, warn);
       TICK(3)
       if (ex) export_efc(e, env, nefc);
     }
-    BAR(5, 11)
     if (phases & PH_CTRL) ctrl_run(e, cs, env, sub == 0 ? action : (const R*)nullptr);
     TICK(4)
     if (phases & PH_STEP2) {
       e.actuation(ex ? s.actuator_force + E * m.nu : nullptr);
       if (e.acceleration()) warn |= 1;
       TICK(5)
-      BAR(2, 11)
+      BAR
       niter = solve(e, nefc, ncon, warn);
       TICK(6)
       if (ex) export_step2(e, env, nefc, niter);
-      BAR(6, 11)
       if (!(phases & PH_NOINTEGRATE)) {
         { int eb = e.euler(&time); if (eb & 32) warn |= 32; else if (eb) warn |= 2; }
       }

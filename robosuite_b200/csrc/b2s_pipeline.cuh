@@ -1,28 +1,13 @@
 // Pipeline mode: one substep = phase 0 (kinematics + dynamics + broad phase) | work-list narrow phase (analytic, convex) beside the
 // thread-per-environment controller kernel | tail (contact gather, constraint rows, solve, integrate, observations), exchanging a
-// per-environment workspace row through L2.  Same device functions as the fused kernel, and the stage sequences (phase 0, one narrow-
-// phase pair, the tail stages) are defined here once for this pipeline and the unit queue; what changes is scheduling and MEMORY:
+// per-environment workspace row through L2.  Same device functions as the fused kernel (the narrow phase of one pair included,
+// b2s_collide.cuh), and the stage sequences (phase 0, the tail stages) are defined here once for this pipeline and the unit queue; what
+// changes is scheduling and MEMORY:
 // every kernel has its own compact shared-memory layout (LAY_P0 / LAY_TS / LAY_TL), so 24-28 warps are resident per SM instead of
 // the 14 the one-size-fits-all layout allowed, and the tail kernel runs in two capacity tiers: the small tier holds the contact /
 // row counts almost every environment has, the few that need more are re-run by the large tier (same results, no truncation).
 #pragma once
 #include "b2s_kernel.cuh"
-
-template <typename R> DEV void row_copy(R* dst, const R* src, int n, int lane) {
-  for (int i = lane; i < n; i += 32) dst[i] = src[i];
-}
-template <> DEV void row_copy<float>(float* dst, const float* src, int n, int lane) {
-  // offsets and lengths of workspace regions are even: move 8 bytes per lane
-  const float2* s2 = reinterpret_cast<const float2*>(src);
-  float2* d2 = reinterpret_cast<float2*>(dst);
-  int n2 = n >> 1;
-  for (int i = lane; i < n2; i += 32) d2[i] = s2[i];
-  if ((n & 1) && lane == 0) dst[n - 1] = src[n - 1];
-}
-
-#ifndef B2S_TMA
-#define B2S_TMA 1  // move workspace regions with the TMA bulk-copy engine (cp.async.bulk + mbarrier)
-#endif
 
 // ---- TMA 1-D bulk copies (SASS: UBLKCP).  One elected lane per warp issues the copies; completion of loads is signalled on
 // the warp's mbarrier (transaction bytes), stores are tracked with a bulk async-group.
@@ -59,7 +44,6 @@ DEV void tma_store_1d(void* gdst, const void* smem_src, unsigned bytes) {
 // a handful of bulk copies: lane k issues span k.
 template <typename R> DEV void ws_load(const Eng<R>& e, const R* row, const PhaseIO& io, unsigned long long* bar, unsigned& parity) {
   if (io.nload == 0) return;
-#if B2S_TMA
   // the destination may have been read / written through the generic proxy before (the constraint Jacobian under the late poses, the
   // previous environment of a large-tier warp): order those accesses before the async-proxy writes of the bulk copies
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
@@ -72,13 +56,8 @@ template <typename R> DEV void ws_load(const Eng<R>& e, const R* row, const Phas
   }
   mbar_wait(bar, parity);
   parity ^= 1u;
-#else
-  for (int k = 0; k < io.nload; k++) row_copy(e.ws + io.load[k].off, row + io.load[k].goff, io.load[k].len, e.lane);
-  __syncwarp();
-#endif
 }
 template <typename R> DEV void ws_store(const Eng<R>& e, R* row, const PhaseIO& io) {
-#if B2S_TMA
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // this lane's generic-proxy writes -> visible to the async proxy
   __syncwarp();
   if (e.lane < io.nstore) {
@@ -88,17 +67,11 @@ template <typename R> DEV void ws_store(const Eng<R>& e, R* row, const PhaseIO& 
     asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
   }
   __syncwarp();
-#else
-  for (int k = 0; k < io.nstore; k++) row_copy(row + io.store[k].goff, e.ws + io.store[k].off, io.store[k].len, e.lane);
-#endif
 }
 
 // A launch covers one group of environments [env0, env0 + nenv); groups run on separate streams so that the tail of one
 // group's kernel (its slowest environment) overlaps with other groups' work.  slot = descriptor slot of the owning handle.
 struct Grp { int env0, nenv, gid, sub, slot; };
-#define EPA_PIPE_MAXV EPA_MAXV
-#define EPA_PIPE_MAXF EPA_MAXF
-#define EPA_PIPE_WORDS EPA_AREA_WORDS(EPA_PIPE_MAXV, EPA_PIPE_MAXF)  // polytope area, then the vertex staging area
 #define CLC(s, g) ((s).cl_cnt + 8 * (g).gid)  // this group's counters: nA, nG, overflowed envs, next convex item, next overflow item
 
 // -DB2S_INSTR: every launch stamps its first / last %globaltimer into st_begin / st_end (device timeline of the CUDA-graph
@@ -121,64 +94,9 @@ DEV unsigned long long gtimer() { unsigned long long t; asm volatile("mov.u64 %0
 // the role with the longest single work item (a deep EPA) is scheduled first.  Every block is one warp.
 struct P1Cfg { int nG, nC, sub; };
 
-// ---- one narrow-phase pair of an environment, for the phase-1 roles and the unit queue alike: geoms in type order (what the fused
-// collide produces), shapes from the environment's workspace row, contact count + records -> the output record `out`
-template <typename R> DEV void narrow_pair_analytic(int slot, int env, const R* row, int pidx, R* out) {
-  const DModel<R>& m = cmodel<R>(slot);
-  const DState<R>& s = cstate<R>(slot);
-  const WSLayout& RL = c_lay[slot][LAY_ROW];
-  int g1 = m.pair_geom[2 * pidx], g2 = m.pair_geom[2 * pidx + 1];
-  if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
-  Shape<R> A, B;
-  shape_from(m, s, env, g1, row + RL.gpos, row + RL.gmat, A);
-  shape_from(m, s, env, g2, row + RL.gpos, row + RL.gmat, B);
-  R buf[8 * CREC];
-  int n = narrow_analytic(A, B, buf);
-  out[0] = R(n);
-  for (int k = 0; k < n * CREC; k++) out[1 + k] = buf[k];
-}
-
-// the whole warp on one convex pair: `scratch` holds the EPA polytope, `stage` (stage_cap words, or nullptr) the staged hull vertices.
-// item_stats: -DB2S_INSTR per-item cost histogram and slow-item log (the phase-1 convex role)
-template <typename R>
-DEV void narrow_pair_convex(int slot, int env, const R* row, int pidx, R* out, R* scratch, R* stage, int stage_cap, int lane, bool item_stats) {
-  const DModel<R>& m = cmodel<R>(slot);
-  const DState<R>& s = cstate<R>(slot);
-  const WSLayout& RL = c_lay[slot][LAY_ROW];
-  int g1 = m.pair_geom[2 * pidx], g2 = m.pair_geom[2 * pidx + 1];
-  if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
-  Shape<R> A, B;
-  shape_from(m, s, env, g1, row + RL.gpos, row + RL.gmat, A);
-  shape_from(m, s, env, g2, row + RL.gpos, row + RL.gmat, B);
-  R buf[CREC];
-#ifdef B2S_INSTR
-  long long it0 = clock64();
-#endif
-  int n = convex_convex(A, B, buf, 1, scratch, lane, s.gjk_cache ? s.gjk_cache + ((size_t)env * m.npair + pidx) * 3 : (R*)nullptr,
-                        EPA_PIPE_MAXV, EPA_PIPE_MAXF, stage, stage_cap);
-#ifdef B2S_INSTR
-  if (item_stats && lane == 0 && s.stats) {  // bucket k = cycles in [2^(k+8), 2^(k+9)), by shape types (mesh-mesh / other)
-    long long dt = clock64() - it0;
-    int k = 0;
-    while (k < 11 && (dt >> (k + 9)) > 0) k++;
-    atomicAdd(s.stats + 500 - 12 * ((A.type == G_MESH && B.type == G_MESH) ? 2 : 1) + k, 1);
-    if (n > 0) atomicAdd(s.stats + 18, 1);
-    if (dt > (1 << 19) && s.slowlog) {  // items above 524 k cycles (~270 us): what are they?
-      int j = atomicAdd(s.stats + 20, 1);
-      if (j < 64) {
-        const int* sp = reinterpret_cast<const int*>(scratch + 9 * EPA_PIPE_MAXV + 4 * EPA_PIPE_MAXF) + EPA_PIPE_MAXF + 64;
-        int* o = s.slowlog + 12 * j;
-        o[0] = (int)dt; o[1] = A.type; o[2] = B.type; o[3] = A.nvert; o[4] = B.nvert; o[5] = sp[0]; o[6] = sp[1]; o[7] = sp[2]; o[8] = sp[3];
-        o[9] = sp[4]; o[10] = g1; o[11] = g2;
-      }
-    }
-  }
-#endif
-  if (lane == 0) {
-    out[0] = R(n);
-    for (int k = 0; k < CREC; k++) out[1 + k] = n ? buf[k] : R(0);
-  }
-  __syncwarp();
+// the convex pair's GJK warm-start direction (the separating direction of its last test in this environment), nullptr without the cache
+template <typename R> DEV R* gjk_cache_of(const DModel<R>& m, const DState<R>& s, int env, int pidx) {
+  return s.gjk_cache ? s.gjk_cache + ((size_t)env * m.npair + pidx) * 3 : (R*)nullptr;
 }
 
 // analytic pairs: ONE THREAD per candidate pair of any environment (32 different pairs per warp)
@@ -190,7 +108,12 @@ template <typename R> DEV void narrow_analytic_block(const Grp& g, int rb) {
   tid += g.env0 * s.cl_maxa;  // this group's slice of the candidate list / output slots
   int code = s.cl_listA[tid];
   int env = code >> 12;
-  narrow_pair_analytic(g.slot, env, s.wsg + (size_t)env * RL.total, code & 4095, s.cl_outA + (size_t)tid * CL_RECA);
+  const R* row = s.wsg + (size_t)env * RL.total;
+  R buf[8 * CREC];
+  const int n = narrow_pair_analytic(cmodel<R>(g.slot), s, env, code & 4095, row + RL.gpos, row + RL.gmat, buf);
+  R* out = s.cl_outA + (size_t)tid * CL_RECA;
+  out[0] = R(n);
+  for (int k = 0; k < n * CREC; k++) out[1 + k] = buf[k];
 }
 
 // convex pairs: ONE WARP per candidate pair (mesh support scans split over the lanes).  The block owns one EPA polytope and the
@@ -209,10 +132,17 @@ template <typename R> DEV void narrow_convex_block(const Grp& g, unsigned char* 
     item = __shfl_sync(B2S_FULL, item, 0);
     if (item >= cnt) break;
     int wid = item + g.env0 * s.cl_maxg;
-    int code = s.cl_listG[wid];
-    int env = code >> 12;
-    narrow_pair_convex(g.slot, env, s.wsg + (size_t)env * RL.total, code & 4095, s.cl_outG + (size_t)wid * 8, scratch,
-                       m.stage_cap > 0 ? scratch + EPA_PIPE_WORDS : (R*)nullptr, m.stage_cap, lane, true);
+    int code = s.cl_listG[wid], env = code >> 12, pidx = code & 4095;
+    const R* row = s.wsg + (size_t)env * RL.total;
+    R buf[CREC];
+    const int n = narrow_pair_convex(m, s, env, pidx, row + RL.gpos, row + RL.gmat, buf, scratch, gjk_cache_of(m, s, env, pidx),
+                                     m.stage_cap > 0 ? scratch + EPA_AREA_WORDS(EPA_MAXV, EPA_MAXF) : (R*)nullptr, m.stage_cap, lane, true);
+    if (lane == 0) {
+      R* out = s.cl_outG + (size_t)wid * 8;
+      out[0] = R(n);
+      for (int k = 0; k < CREC; k++) out[1 + k] = n ? buf[k] : R(0);
+    }
+    __syncwarp();
   }
 }
 
@@ -220,10 +150,6 @@ template <typename R>
 __global__ void __launch_bounds__(32) phase1_kernel(const R* action, Grp g, P1Cfg c) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int b = blockIdx.x;
-#ifdef B2S_ZERO_SMEM
-  for (int i = threadIdx.x; i < 6000; i += 32) reinterpret_cast<int*>(smem_raw)[i] = 0;
-  __syncwarp();
-#endif
 #ifdef B2S_INSTR
   const DState<R>& s = cstate<R>(g.slot);
   const int kind = b < c.nG ? 2 : (b < c.nG + c.nC ? 4 : 1);
@@ -281,8 +207,8 @@ template <typename R> DEVN int gather_contacts(Eng<R> e, int env, int& warn) {
     if (lane + 32 * it >= nc) continue;
     int pair = pairv[it], slot = slotv[it], n = cntv[it], off = offv[it];
     const R* rec = isgv[it] ? s.cl_outG + (size_t)slot * 8 + 1 : s.cl_outA + (size_t)slot * CL_RECA + 1;
-    int g1 = m.pair_geom[2 * pair], g2 = m.pair_geom[2 * pair + 1];
-    if (m.geom_type[g1] > m.geom_type[g2]) { int t = g1; g1 = g2; g2 = t; }
+    int g1, g2;
+    pair_geoms(m, pair, g1, g2);
     for (int k = 0; k < n; k++) {
       int c = off + k;
       if (c >= L.mc) break;
@@ -416,24 +342,6 @@ template <typename R> DEV int tail_newton(Eng<R>& e, int nefc, int ncon) {
   return warn;
 }
 
-// Write-back, also the end of the fused step_kernel: state rows, time and the warn bits of the whole warp -> global memory
-template <typename R> DEV void store_state(const Eng<R>& e, int env, R time, int warn) {
-  const DModel<R>& m = e.model();
-  const DState<R>& s = e.state();
-  const WSLayout& L = e.lay();
-  const int lane = e.lane;
-  const size_t E = env;
-  for (int i = lane; i < m.nq; i += 32) s.qpos[E * m.nq + i] = e.p(L.qpos)[i];
-  for (int i = lane; i < m.nv; i += 32) {
-    s.qvel[E * m.nv + i] = e.p(L.qvel)[i];
-    s.qacc[E * m.nv + i] = e.p(L.qacc)[i];
-    s.qacc_ws[E * m.nv + i] = e.p(L.qacc_ws)[i];
-  }
-  warn = warp_or_i(warn);  // some flags (a dropped contact's rows) are raised on the lane that owns the item
-  if (lane == 0) { s.time[env] = time; s.warn[env] |= warn; }
-  __syncwarp();
-}
-
 // Finish: Euler, on the last substep of a control step the observation and task rows, state write-back.
 template <typename R>
 DEV void tail_finish(Eng<R>& e, int env, int sub, int nsub, int phases, int ncon, int warn, unsigned long long* bar, unsigned& parity) {
@@ -460,18 +368,12 @@ DEV void tail_finish(Eng<R>& e, int env, int sub, int nsub, int phases, int ncon
 // pointer, found with compute-sanitizer) - the same family of nvcc 12.9 stack-slot problems as DESIGN.md section 3 records.
 // The kernels are latency bound at 4096 environments (every environment's warp is resident either way), so the lost occupancy
 // costs nothing measurable (256 x 2 was the fastest of the launch-bound variants measured).
-#ifndef B2S_LB0_THREADS
-#define B2S_LB0_THREADS 256  // phase 0
-#define B2S_LB0_BLOCKS 2
-#endif
-#ifndef B2S_LB5_THREADS
-#define B2S_LB5_THREADS 256  // tail kernel
-#define B2S_LB5_BLOCKS 2
-#endif
+constexpr int P0_THREADS = 256, P0_BLOCKS = 2;      // phase 0
+constexpr int TAIL_THREADS = 256, TAIL_BLOCKS = 2;  // tail kernel
 
 // ---- phase 0: kinematics, velocity stage + RNE bias, CRB -> M, broad phase -> global candidate work lists
 template <typename R>
-__global__ void __launch_bounds__(B2S_LB0_THREADS, B2S_LB0_BLOCKS) phase0_kernel(int phases, Grp g) {
+__global__ void __launch_bounds__(P0_THREADS, P0_BLOCKS) phase0_kernel(int phases, Grp g) {
   const DState<R>& s = cstate<R>(g.slot);
   const WSLayout& L = c_lay[g.slot][LAY_P0];
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -485,10 +387,6 @@ __global__ void __launch_bounds__(B2S_LB0_THREADS, B2S_LB0_BLOCKS) phase0_kernel
   if (env >= g.nenv) return;
   env += g.env0;
   Eng<R> e(smem + (size_t)warp * L.total, lane, g.slot, LAY_P0);
-#ifdef B2S_ZERO_SMEM
-  for (int i = lane; i < L.total; i += 32) e.ws[i] = 0;
-  __syncwarp();
-#endif
   int na, ng;
   const int warn = phase0_env(e, env, na, ng);
   // output slots of the candidates: appended to the group's work lists (slots by warp-aggregated atomics)
@@ -510,7 +408,7 @@ __global__ void __launch_bounds__(B2S_LB0_THREADS, B2S_LB0_BLOCKS) phase0_kernel
 // tier 0: warp per environment of the group, small-capacity layout; an environment whose contacts / rows do not fit is appended to
 // the group's overflow list untouched.  tier 1: warps claim the overflowed environments and run them with the full-capacity layout.
 template <typename R>
-__global__ void __launch_bounds__(B2S_LB5_THREADS, B2S_LB5_BLOCKS) tail_kernel(int phases, int nsub, const R* action, Grp g, int tier) {
+__global__ void __launch_bounds__(TAIL_THREADS, TAIL_BLOCKS) tail_kernel(int phases, int nsub, const R* action, Grp g, int tier) {
   const DState<R>& s = cstate<R>(g.slot);
   const int lid = tier ? LAY_TL : LAY_TS;
   const WSLayout& L = c_lay[g.slot][lid];
@@ -523,10 +421,6 @@ __global__ void __launch_bounds__(B2S_LB5_THREADS, B2S_LB5_BLOCKS) tail_kernel(i
   __syncwarp();
   unsigned parity = 0;
   Eng<R> e(smem + (size_t)warp * L.total, lane, g.slot, lid);
-#ifdef B2S_ZERO_SMEM
-  for (int i = lane; i < L.total; i += 32) e.ws[i] = 0;
-  __syncwarp();
-#endif
   int* clc = CLC(s, g);
   for (int iter = 0;; iter++) {
     int env;

@@ -5,12 +5,8 @@
 #pragma once
 // B2S_LOOP: the loops of make_constraint / constraint_update / ls_eval / solve keep their rolled form.  Unrolled, `solve` alone
 // is 90 KB of SASS against a 32 KB instruction cache; rolled it is 31 KB and the whole step is 11.7 % faster (239 k -> 267 k
-// env-steps/s, Lift 4096 envs).  -DB2S_UNROLL_SOLVER restores the compiler default.
-#ifndef B2S_UNROLL_SOLVER
+// env-steps/s, Lift 4096 envs).
 #define B2S_LOOP _Pragma("unroll 1")
-#else
-#define B2S_LOOP
-#endif
 #include "b2s_collide.cuh"
 
 #define B2S_MINIMP 0.0001

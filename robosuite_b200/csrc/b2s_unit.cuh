@@ -64,19 +64,36 @@ template <typename R> DEVN int unit_phase0(R* area, int lane, int slot, int env)
 // narrow phase of ONE environment by its own warp: analytic pairs one per lane, convex pairs one after the other with the warp's whole
 // workspace area as EPA polytope + vertex staging scratch (phase 0's regions are in the global row by now)
 template <typename R> DEVN void unit_narrow(R* area, int area_words, int lane, int slot, int env, int na, int ng) {
+  const DModel<R>& m = cmodel<R>(slot);
   const DState<R>& s = cstate<R>(slot);
+  const WSLayout& RL = c_lay[slot][LAY_ROW];
   size_t E = env;
-  const R* row = s.wsg + E * c_lay[slot][LAY_ROW].total;
+  const R* row = s.wsg + E * RL.total;
   const int* tab = s.cl_env + E * CL_ENVW(s);
   for (int base = 0; base < na; base += 32) {
     int i = base + lane;
-    if (i < na) narrow_pair_analytic(slot, env, row, tab[2 + 2 * i], s.cl_outA + (E * s.cl_maxa + i) * CL_RECA);
+    if (i < na) {
+      R buf[8 * CREC];
+      const int n = narrow_pair_analytic(m, s, env, tab[2 + 2 * i], row + RL.gpos, row + RL.gmat, buf);
+      R* out = s.cl_outA + (E * s.cl_maxa + i) * CL_RECA;
+      out[0] = R(n);
+      for (int k = 0; k < n * CREC; k++) out[1 + k] = buf[k];
+    }
   }
   __syncwarp();
-  const int stage_cap = area_words - EPA_PIPE_WORDS;
-  for (int i = 0; i < ng; i++)
-    narrow_pair_convex(slot, env, row, tab[2 + 2 * (s.cl_maxa + i)], s.cl_outG + (E * s.cl_maxg + i) * 8, area,
-                       stage_cap >= 64 ? area + EPA_PIPE_WORDS : (R*)nullptr, stage_cap >= 64 ? stage_cap : 0, lane, false);
+  const int epa_words = EPA_AREA_WORDS(EPA_MAXV, EPA_MAXF), stage_cap = area_words - epa_words;
+  for (int i = 0; i < ng; i++) {
+    const int pidx = tab[2 + 2 * (s.cl_maxa + i)];
+    R buf[CREC];
+    const int n = narrow_pair_convex(m, s, env, pidx, row + RL.gpos, row + RL.gmat, buf, area, gjk_cache_of(m, s, env, pidx),
+                                     stage_cap >= 64 ? area + epa_words : (R*)nullptr, stage_cap >= 64 ? stage_cap : 0, lane, false);
+    if (lane == 0) {
+      R* out = s.cl_outG + (E * s.cl_maxg + i) * 8;
+      out[0] = R(n);
+      for (int k = 0; k < CREC; k++) out[1 + k] = n ? buf[k] : R(0);
+    }
+    __syncwarp();
+  }
   __syncwarp();
 }
 
@@ -122,13 +139,10 @@ DEV void unit_finish(const UnitQ& q, int n_env, int env, int sub, int nsub, int 
 // One block of 16 warps per SM: what counts is that an SM executes ONE code region at a time (the hot code is ~10x the instruction
 // cache).  Measured on 4096 Lift environments: 16 warps x 1 block 306 k env-steps/s, 8 warps x 2 blocks 248 k, 8 warps x 1 block 210 k,
 // 4 warps x 4 blocks 158 k, free-running warps (no block barriers) 80 k.
-#ifndef B2S_LBU_THREADS
-#define B2S_LBU_THREADS 512
-#define B2S_LBU_BLOCKS 1
-#endif
+constexpr int UNIT_THREADS = 512, UNIT_BLOCKS = 1;
 
 template <typename R>
-__global__ void __launch_bounds__(B2S_LBU_THREADS, B2S_LBU_BLOCKS) unit_kernel(int phases, int nsub, const R* action, int slot, UnitQ q) {
+__global__ void __launch_bounds__(UNIT_THREADS, UNIT_BLOCKS) unit_kernel(int phases, int nsub, const R* action, int slot, UnitQ q) {
   const DState<R>& s = cstate<R>(slot);
   extern __shared__ __align__(16) unsigned char smem_raw[];
   R* smem = reinterpret_cast<R*>(smem_raw);

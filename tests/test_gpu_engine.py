@@ -323,12 +323,8 @@ def test_split_controller_kernel_matches_in_kernel_controller():
     assert np.isfinite(b[0]).all() and dq < 1e-5
 
 
-@pytest.mark.parametrize("name", ["Stack_Panda", "NutAssemblyRound_Panda", "Door_Panda", "PickPlace_Panda", "Lift_Sawyer"])
-def test_engine_parity_other_task_models(name):
-    """engine-level parity (forward + 60 substeps, gravity-compensating torques) on the other BASELINE task models"""
-    import torch
-    from robosuite_b200.engine import BatchedSim
-
+def _task_states(name, n=2):
+    """a BASELINE task model and `n` seeded states of it: arm near its home pose, free objects spread out and dropped a little"""
     model = load(name)
     if name.startswith("Door"):
         # the composed MJCF leaves the door at the world origin (half inside the floor); the reference moves it at reset
@@ -337,7 +333,6 @@ def test_engine_parity_other_task_models(name):
         th = -np.pi / 2 - 0.125
         model.body_pos[b] = [-0.2 + 0.08, -0.35, 0.8 + 0.3]
         model.body_quat[b] = [np.cos(th / 2), 0, 0, np.sin(th / 2)]
-    n = 2
     rng = np.random.default_rng(0)
     q = np.tile(model.qpos0, (n, 1))
     arm = [i for i, nm in enumerate(model.names["joint"]) if nm and nm.startswith("robot0_") and model.jnt_type[i] == 3]
@@ -359,6 +354,41 @@ def test_engine_parity_other_task_models(name):
                 q[:, model.jnt_qposadr[j] + 1] += 0.12 * k - 0.12
             k += 1
             q[:, model.jnt_qposadr[j] + 2] += 0.02
+    return model, q
+
+
+def _same_contacts(tag, o, nd, cg, cd):
+    """the device's contacts (count nd, geoms cg, distances cd) against the oracle's after its forward().  The sets must agree except
+    for knife-edge contacts (|dist| below fp32 resolution: geoms that touch exactly in the model, where activation depends on the last
+    bit in any engine); without those, the sequences must be identical: ordered by pair index.  Returns False on a knife edge."""
+    dev = {}
+    for c in range(nd):
+        dev.setdefault((int(cg[c, 0]), int(cg[c, 1])), []).append(float(cd[c]))
+    ora = {}
+    for c in o.contacts():
+        ora.setdefault((c["geom1"], c["geom2"]), []).append(c["dist"])
+    knife = False
+    for key in set(dev) | set(ora):
+        a, b = dev.get(key, []), ora.get(key, [])
+        if len(a) != len(b):
+            knife = True
+            # a pair present on one side only must be a zero-depth touch; a pair present on both sides may differ in
+            # the NUMBER of manifold points when faces are exactly aligned (clipping keeps / drops boundary vertices)
+            if not a or not b:
+                assert all(abs(x) < 2e-6 for x in a + b), (tag, key, a, b)
+    if not knife:
+        assert [(int(a), int(b)) for a, b in cg[:nd]] == [(c["geom1"], c["geom2"]) for c in o.contacts()], tag
+    return not knife
+
+
+@pytest.mark.parametrize("name", ["Stack_Panda", "NutAssemblyRound_Panda", "Door_Panda", "PickPlace_Panda", "Lift_Sawyer"])
+def test_engine_parity_other_task_models(name):
+    """engine-level parity (forward + 60 substeps, gravity-compensating torques) on the other BASELINE task models"""
+    import torch
+    from robosuite_b200.engine import BatchedSim
+
+    model, q = _task_states(name)
+    n = len(q)
     sim = BatchedSim(model, n, precision="f32", maxcon=96, maxefc=288)
     sim.qpos.copy_(torch.as_tensor(q, dtype=torch.float32))
     sim.forward()
@@ -369,25 +399,7 @@ def test_engine_parity_other_task_models(name):
     qacc_h, nefc_h = sim.qacc.cpu().numpy(), sim.nefc.cpu().numpy()
     for e in range(n):
         o.reset_data(); o.qpos[:] = q[e]; o.forward()
-        # contact sets must agree except for knife-edge contacts (|dist| below fp32 resolution: geoms that touch exactly
-        # in the model, where activation depends on the last bit in any engine)
-        nd = int(ncon_h[e])
-        dev = {}
-        for c in range(nd):
-            dev.setdefault((int(cg_h[e, c, 0]), int(cg_h[e, c, 1])), []).append(float(cd_h[e, c]))
-        ora = {}
-        for c in o.contacts():
-            ora.setdefault((c["geom1"], c["geom2"]), []).append(c["dist"])
-        knife = False
-        for key in set(dev) | set(ora):
-            a, b = dev.get(key, []), ora.get(key, [])
-            if len(a) != len(b):
-                knife = True
-                # a pair present on one side only must be a zero-depth touch; a pair present on both sides may differ in
-                # the NUMBER of manifold points when faces are exactly aligned (clipping keeps / drops boundary vertices)
-                if not a or not b:
-                    assert all(abs(x) < 2e-6 for x in a + b), (name, e, key, a, b)
-        if not knife:
+        if _same_contacts((name, e), o, int(ncon_h[e]), cg_h[e], cd_h[e]):
             assert int(nefc_h[e]) == o.nefc
             errs.append(np.abs(qacc_h[e] - o.qacc).max() / max(np.abs(o.qacc).max(), 1e-9))
     assert not errs or max(errs) < 2e-2, (name, errs)  # Door: ~90 stiff rows at rest, fp32 solve
@@ -413,6 +425,50 @@ def test_engine_parity_other_task_models(name):
     print(name, "forward qacc rel err %.3g (%d of %d envs without knife-edge contacts), 60-substep qpos rel err %.3g" % (
         max(errs) if errs else float("nan"), len(errs), n, worst))
     assert worst < (1e-4 if len(errs) == n else 2e-3)
+    # the contact sequence once more with the objects settled, at the device's state: NutAssemblyRound's nut then rests on more than
+    # 32 contacts, which the fused kernel orders by insertion instead of by rank
+    sim.forward()
+    torch.cuda.synchronize()
+    ncon_h, cg_h, cd_h = sim.ncon.cpu().numpy(), sim.contact_geom.cpu().numpy(), sim.contact_dist.cpu().numpy()
+    longest = 0  # most contacts of an environment whose sequence was checked
+    for e in range(n):
+        o.reset_data(); o.qpos[:] = qd[e]; o.forward()
+        same = _same_contacts((name, "settled", e), o, int(ncon_h[e]), cg_h[e], cd_h[e])
+        print(name, "settled env %d: %d contacts, %s" % (e, int(ncon_h[e]), "sequence checked" if same else "knife edge"))
+        if same:
+            longest = max(longest, int(ncon_h[e]))
+    if name.startswith("NutAssembly"):
+        assert longest > 32, longest
+    sim.close()
+
+
+def test_contact_overflow_keeps_pair_ordered_subset():
+    """more contacts than maxcon: forward() sets warn bit 4 and exports exactly maxcon of them, in pair order, each one a contact of
+    the oracle (Stack: the cubes on the floor and the two finger pads pressed together, 15-16 contacts)"""
+    import torch
+    from robosuite_b200.engine import BatchedSim
+
+    model, q = _task_states("Stack_Panda")
+    n, maxcon = len(q), 4
+    sim = BatchedSim(model, n, precision="f32", maxcon=maxcon, maxefc=288)
+    sim.qpos.copy_(torch.as_tensor(q, dtype=torch.float32))
+    sim.forward()
+    torch.cuda.synchronize()
+    pair = {tuple(sorted(p)): i for i, p in enumerate(model.pair_geom.tolist())}
+    warn, ncon = sim.warn.cpu().numpy(), sim.ncon.cpu().numpy()
+    cg, cpos, cd = sim.contact_geom.cpu().numpy(), sim.contact_pos.cpu().numpy(), sim.contact_dist.cpu().numpy()
+    o = _oracle(model)
+    for e in range(n):
+        assert int(warn[e]) & 4 and int(ncon[e]) == maxcon, (e, int(warn[e]), int(ncon[e]))
+        pidx = [pair[tuple(sorted((int(a), int(b))))] for a, b in cg[e, :maxcon]]
+        assert pidx == sorted(pidx), (e, pidx)
+        o.reset_data(); o.qpos[:] = q[e]; o.forward()
+        oc = o.contacts()
+        assert len(oc) > maxcon
+        for c in range(maxcon):
+            g = (int(cg[e, c, 0]), int(cg[e, c, 1]))
+            assert any((x["geom1"], x["geom2"]) == g and np.abs(cpos[e, c] - x["pos"]).max() < 1e-3 and abs(cd[e, c] - x["dist"]) < 1e-4
+                       for x in oc), (e, c, g, cpos[e, c], cd[e, c])
     sim.close()
 
 
