@@ -200,7 +200,7 @@ int b2s_task_table(b2s_sim* sim, int n, const int* op, const int* a, const int* 
  *   overrides        body_xpos_ov:<id> body_xquat_ov:<id> per pose override; geom_{size,friction,rbound,aabb,solref,solimp}:<id> per geom
  *                    slot; body_mass:<id> body_inertia:<id> per body slot; the declared dof vectors; dof_invweight0 body_invweight0
  *                    meaninertia (copied, not recomputed: a snapshot taken while they were stale restores them stale)
- * Not in a row: the exported derived arrays (xpos, contacts, efc_*, ...), ncon / nefc / solver_niter, prof / dbg, pipeline workspaces,
+ * Not in a row: the exported derived arrays (xpos, contacts, efc_*, ...), ncon / nefc / solver_niter, pipeline workspaces,
  * and handle configuration (controller gains, obs / task tables, perturbation tables).
  * The SIGNATURE is a 64-bit FNV-1a hash of the section table (names, counts, dtypes), the precision, the controller kind, the obs and
  * task op tables and the model blob without its capacity records (opt_maxcon, opt_maxefc and the small-tier pair): rows restore only
@@ -230,11 +230,6 @@ int b2s_set_export(b2s_sim* sim, int flag);
  * replayed on the group's own stream), 2 = unit queue (one persistent kernel per control step).  Results are identical; see
  * DESIGN.md sections 4 and 5 for when each wins. */
 int b2s_set_mode(b2s_sim* sim, int mode);
-
-/* debugging aid: b2s_env_step accumulates per-phase clock cycles per environment into the array "prof" [n_env,12]
- * (0 kinematics, 1 velocity+crb, 2 collision, 3 constraint rows, 4 controller, 5 actuation+smooth acc, 6 solver,
- * 7 integrate, 11 time spent waiting at block barriers) and collision candidate counts into "dbg" [n_env,4] */
-int b2s_set_profile(b2s_sim* sim, int flag);
 
 /* number of kernels this handle has launched since creation (bench.py "gpu_launches") */
 int64_t b2s_launch_count(const b2s_sim* sim);

@@ -28,7 +28,8 @@ def build(force=False, verbose=False):
 
 def build_instr(force=False):
     """-DB2S_INSTR measurement build (device %globaltimer timeline + solver statistics; tools/probe_instr.py, bench.py's
-    `roofline.timeline`).  Never loaded by the product path: selected only through B2S_LIB."""
+    `roofline.timeline`; the unit queue's stage counters, tools/probe_unit.py).  Never loaded by the product path: selected only
+    through B2S_LIB."""
     out = os.path.join(_HERE, "variants", "libb2s_instr.so")
     if not force and os.path.exists(out) and all(os.path.getmtime(p) <= os.path.getmtime(out) for p in _deps()):
         return out

@@ -97,7 +97,7 @@ struct b2s_sim {
   std::vector<double> qpos0;
   std::vector<int> site_bodyid, cgid;
   std::map<std::string, std::vector<std::string>> names;  // object type -> names by id (MjModel name tables)
-  int has_obs = 0, export_env_step = 1, dirty = 1, profile = 0, mode = 0, ngroups = 8;
+  int has_obs = 0, export_env_step = 1, dirty = 1, mode = 0, ngroups = 8;
   int ctrl_split = 1;  // pipeline: OSC controller as its own thread-per-environment kernel (B2S_CTRL_SPLIT=0: inside the tail kernel)
   // pipeline: one CUDA graph per environment group, replayed on the group's stream and joined to `stream` through gevents
   std::vector<cudaStream_t> gstreams;
@@ -111,7 +111,9 @@ struct b2s_sim {
   int* uq_ring = nullptr; int* uq_ovf = nullptr; int* uq_ctr = nullptr; int uq_cap = 0;
   int uq_wpb = 0, uq_stride = 0, uq_stride_large = 0, uq_wpb_large = 0, uq_nlarge = 0, uq_grid = 0;
   size_t uq_smem = 0;
-  unsigned long long* uq_prof = nullptr;
+#ifdef B2S_INSTR
+  unsigned long long* uq_prof = nullptr;  // the unit queue's stage counters (UnitQ::prof)
+#endif
   std::vector<double> xpos0_h, xquat0_h;  // world poses of the bodies welded to the world (model constants)
   std::vector<int> body_weldid_h;
   // model values that b2s_model_override copies per environment, and the host-computed constants derived from them
@@ -429,12 +431,6 @@ template <typename R> static void build_state(b2s_sim* s, const DModel<R>& m, DS
   st.ctrl_torque = state_arr<R>(s, "ctrl_torque", 8);
   st.jv_state = state_arr<R>(s, "ctrl_jv_state", 72);
   st.wsg = nullptr;
-  {
-    float* p = dev_zeros<float>(s, (size_t)s->n_env * 12);
-    s->arrays["prof"] = ArrayInfo{p, B2S_F32, 2, {s->n_env, 12, 0, 0}};
-    st.prof = p;
-    st.dbg = state_arr_i(s, "dbg", 4);
-  }
 }
 
 // ---- workspace layouts.  Every region is 16-byte aligned in offset and length (TMA bulk copies).
@@ -745,16 +741,6 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
 
 void b2s_destroy(b2s_sim* s) {
   if (!s) return;
-  if (s->uq_prof) {
-    unsigned long long h[16];
-    cudaSetDevice(s->device); cudaDeviceSynchronize();
-    if (cudaMemcpy(h, s->uq_prof, sizeof(h), cudaMemcpyDeviceToHost) == cudaSuccess && h[15] > 0) {
-      static const char* nm[9] = {"take tickets", "ring slots", "phase 0", "narrow phase", "rows (gather, constraint)", "controller", "actuation + acceleration", "solve", "integrate, obs, publish"};
-      double tot = 0; for (int k = 0; k < 9; k++) tot += (double)h[k];
-      fprintf(stderr, "[b2s] unit-queue stage profile over %llu block rounds (mean cycles per round, share):\n", h[15]);
-      for (int k = 0; k < 9; k++) fprintf(stderr, "[b2s]   %-28s %9.0f  %5.1f %%\n", nm[k], (double)h[k] / (double)h[15], 100.0 * (double)h[k] / tot);
-    }
-  }
   if (s->slot >= 0 && g_slots[s->device & 63][s->slot] == s) g_slots[s->device & 63][s->slot] = nullptr;
   cudaSetDevice(s->device);
   cudaDeviceSynchronize();  // kernels of this handle may still be reading its buffers
@@ -771,8 +757,6 @@ int b2s_set_stream(b2s_sim* s, void* stream) {
   s->stream = (cudaStream_t)stream;
   return B2S_OK;
 }
-
-int b2s_set_profile(b2s_sim* s, int flag) { if (!s) return fail(B2S_ERR_ARG, "null handle"); s->profile = flag != 0; return B2S_OK; }
 
 int b2s_set_export(b2s_sim* s, int flag) { if (!s) return fail(B2S_ERR_ARG, "null handle"); s->export_env_step = flag != 0; return B2S_OK; }
 
@@ -901,6 +885,8 @@ template <typename R> static int ensure_ws(b2s_sim* s, const DModel<R>& m, DStat
     s->arrays["cyc"] = ArrayInfo{st.cyc, B2S_F32, 3, {(int64_t)ne, 32, 2, 0}};
     st.slowlog = dev_zeros<int>(s, 64 * 12);
     s->arrays["slowlog"] = ArrayInfo{st.slowlog, B2S_I32, 2, {64, 12, 0, 0}};
+    s->uq_prof = dev_zeros<unsigned long long>(s, 16);
+    s->arrays["unit_prof"] = ArrayInfo{s->uq_prof, B2S_I64, 1, {16, 0, 0, 0}};
 #endif
     s->dirty = 1;
     s->layout_version++;  // the GJK cache now exists
@@ -920,7 +906,6 @@ static int launch_pipeline(b2s_sim* s, int phases, int nsub, const void* action)
     cudaMemsetAsync(st.st_begin, 0xff, sizeof(unsigned long long) * 64 * 32 * 8, s->stream);
     cudaMemsetAsync(st.st_end, 0, sizeof(unsigned long long) * 64 * 32 * 8, s->stream);
 #endif
-    phases |= PH_WORKLIST;
     const bool osc = s->ctrl.kind == B2S_CTRL_OSC_POSE || s->ctrl.kind == B2S_CTRL_OSC_POSITION;
     if ((phases & PH_CTRL) && osc && s->ctrl_split) phases |= PH_CTRL_EXT;
     { int rc2 = rebuild_layouts(s); if (rc2 != B2S_OK) return rc2; }  // before the descriptors are (re)uploaded
@@ -984,6 +969,9 @@ static int launch_unit(b2s_sim* s, int phases, int nsub, const void* action) {
       if (cudaMalloc(&p, sizeof(int) * (2 * (size_t)total + 8)) != cudaSuccess) return fail(B2S_ERR_CUDA, "cudaMalloc(unit ring) failed");
       s->allocs.push_back(p);
       s->uq_ring = p; s->uq_ovf = p + total; s->uq_ctr = p + 2 * (size_t)total; s->uq_cap = total;
+#ifdef B2S_INSTR
+      s->arrays["unit_ctr"] = ArrayInfo{s->uq_ctr, B2S_I32, 1, {8, 0, 0, 0}};
+#endif
     }
     if (s->uq_wpb == 0) {
       // block shape: the warp's one workspace area holds phase 0's layout, then the EPA polytope + vertex staging, then the small tail tier
@@ -1019,20 +1007,15 @@ static int launch_unit(b2s_sim* s, int phases, int nsub, const void* action) {
     }
     int rc = bind_constants(s);
     if (rc != B2S_OK) return rc;
-    if (getenv("B2S_UNIT_PROF") && !s->uq_prof) s->uq_prof = dev_zeros<unsigned long long>(s, 16);
-    UnitQ q{s->uq_ring, s->uq_ovf, s->uq_ctr, total, s->uq_nlarge, s->uq_wpb_large, s->uq_stride, s->uq_stride_large, s->uq_prof};
+    UnitQ q{s->uq_ring, s->uq_ovf, s->uq_ctr, total, s->uq_nlarge, s->uq_wpb_large, s->uq_stride, s->uq_stride_large};
+#ifdef B2S_INSTR
+    q.prof = s->uq_prof;
+#endif
     unit_init_kernel<R><<<(total + 255) / 256, 256, 0, s->stream>>>(q, s->n_env);
     unit_kernel<R><<<s->uq_grid, s->uq_wpb * 32, s->uq_smem, s->stream>>>(phases, nsub, (const R*)action, s->slot, q);
     unit_check_kernel<R><<<8, 256, 0, s->stream>>>(q, s->slot);
     s->launches += 3;
     CUDA_TRY(cudaGetLastError());
-    if (getenv("B2S_UNIT_DEBUG")) {
-      int c[8];
-      CUDA_TRY(cudaStreamSynchronize(s->stream));
-      CUDA_TRY(cudaMemcpy(c, s->uq_ctr, sizeof(c), cudaMemcpyDeviceToHost));
-      fprintf(stderr, "[b2s] unit ctr: head %d tail %d done %d ovf_head %d ovf_tail %d | watchdog ticket %d tail_then %d flag %d (total %d)\n", c[0], c[1], c[2], c[3], c[4], c[5], c[6], c[7], total);
-      if (c[7]) return fail(B2S_ERR_CUDA, "unit-queue watchdog: a ticket was never produced");
-    }
     return B2S_OK;
   });
 }
@@ -1472,11 +1455,11 @@ int b2s_body_pose_override(b2s_sim* s, int body_id) {
 
 int b2s_env_step(b2s_sim* s, const void* action, int nsub) {
   if (!s || !s->has_ctrl || !action || nsub < 1) return fail(B2S_ERR_ARG, "b2s_env_step: bad argument / controller not configured");
-  if (s->mode == 2 && !s->export_env_step && !s->profile)
+  if (s->mode == 2 && !s->export_env_step)
     return launch_unit(s, PH_STEP1 | PH_STEP2 | PH_CTRL | (s->has_obs ? PH_OBS : 0), nsub, action);
-  if (s->mode == 1 && !s->export_env_step && !s->profile)
+  if (s->mode == 1 && !s->export_env_step)
     return launch_pipeline(s, PH_STEP1 | PH_STEP2 | PH_CTRL | (s->has_obs ? PH_OBS : 0), nsub, action);
-  return launch(s, PH_STEP1 | PH_STEP2 | PH_CTRL | (s->has_obs ? PH_OBS : 0) | (s->export_env_step ? PH_EXPORT : 0) | (s->profile ? PH_PROFILE : 0), nsub, action);
+  return launch(s, PH_STEP1 | PH_STEP2 | PH_CTRL | (s->has_obs ? PH_OBS : 0) | (s->export_env_step ? PH_EXPORT : 0), nsub, action);
 }
 
 int b2s_obs_config(b2s_sim* s, int obs_dim, const int* op, const int* a, const int* b) {

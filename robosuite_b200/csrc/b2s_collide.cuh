@@ -1170,10 +1170,8 @@ template <typename R> DEV void finish_contacts(const Eng<R>& e, int ncon) {
 // The fused kernel's collision stage, composed of the shared pieces: broad phase (at most 96 analytic and 96 convex candidates),
 // analytic candidates one lane each, convex candidates the whole warp each, contacts ordered by pair index, friction / condim mixing.
 // Fills the contact arrays in the workspace; returns ncon (warp-uniform).  warn bit 4 on candidate or contact overflow (the contacts
-// kept are the first maxcon found, analytic before convex).  dbg3: candidate and convex-contact counts; pc: profiler slots 8-10.
-template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc = nullptr) {
-  long long tp0 = pc ? clock64() : 0;
-#define CTICK(slot) if (pc) { __syncwarp(); long long tp1 = clock64(); pc[slot] += (float)(tp1 - tp0); tp0 = tp1; }
+// kept are the first maxcon found, analytic before convex).
+template <typename R> DEVN int collide(Eng<R> e, int& warn) {
   const DModel<R>& m = e.model();
   const DState<R>& st = e.state();
   const WSLayout& L = e.lay();
@@ -1183,8 +1181,6 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
   int* cand_g = cand + MAXC;
   int na, ng;
   cull_pairs(e, cand, cand_g, MAXC, MAXC, na, ng);
-  dbg3[0] += na; dbg3[1] += ng;
-  CTICK(8)
   if (na > MAXC) { na = MAXC; warn |= 4; }
   if (ng > MAXC) { ng = MAXC; warn |= 4; }
   R* cpos = e.p(L.c_pos); R* cfr = e.p(L.c_frame); R* cdist = e.p(L.c_dist);
@@ -1219,7 +1215,6 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
   }
   if (ncon > L.mc) { ncon = L.mc; warn |= 4; }
   __syncwarp();
-  CTICK(9)
   // --- convex candidates: the whole warp per pair (the fused kernel appends the EPA polytope area to every warp's workspace)
   R* epa_scratch = e.ws + L.total;
   for (int ci = 0; ci < ng; ci++) {
@@ -1228,7 +1223,6 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
     R buf[CREC];
     int n = narrow_pair_convex(m, st, e.env, pidx, gpos, gmat, buf, epa_scratch, (R*)nullptr, (R*)nullptr, 0, lane, false);
     if (n > 0) {
-      dbg3[2]++;
       if (ncon < L.mc) {
         int c = ncon;
         if (lane == 0) {
@@ -1243,7 +1237,6 @@ template <typename R> DEVN int collide(Eng<R> e, int& warn, int* dbg3, float* pc
     __syncwarp();
   }
   __syncwarp();
-  CTICK(10)
   // --- order contacts by pair index (stable): up to 32 by rank = #contacts with a smaller key, more by insertion on lane 0
   if (ng > 0 && ncon > 1) {
     if (ncon <= 32) {

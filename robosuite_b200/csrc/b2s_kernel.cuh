@@ -137,52 +137,35 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
   if (phases & PH_CTRL) ctrl_load(e, cs, env);
   __syncwarp();
   int warn = 0;
-  float pc[12];
-#pragma unroll
-  for (int i = 0; i < 12; i++) pc[i] = 0;
-  const bool prof = phases & PH_PROFILE;
-  int dbgc[3] = {0, 0, 0};
-  long long t0 = 0;
-#define TICK(slot) if (prof) { long long t1 = clock64(); pc[slot] += (float)(t1 - t0); t0 = t1; }
-#define BAR { __syncthreads(); TICK(11) }
   for (int sub = 0; sub < nsub; sub++) {
     int ncon = 0, nefc = 0, niter = 0;
     bool ex = live && (phases & PH_EXPORT) && sub == nsub - 1;
-    if (prof) t0 = clock64();
-    BAR
+    __syncthreads();
     if (phases & PH_STEP1) {
       if (e.kinematics()) {  // diverged state reset to the model defaults (mj_checkPos / mj_checkVel)
         for (int i = lane; i < m.nv; i += 32) { e.p(L.qacc)[i] = 0; e.p(L.qacc_ws)[i] = 0; }
         time = 0; warn |= 32;
         __syncwarp();
       }
-      TICK(0)
       e.velocity();
       e.crb();
-      TICK(1)
-      BAR
-      ncon = collide(e, warn, dbgc, prof ? pc : (float*)nullptr);
-      TICK(2)
+      __syncthreads();
+      ncon = collide(e, warn);
       if (ex) export_step1(e, env, ncon);
-      BAR
+      __syncthreads();
       nefc = make_constraint(e, ncon, warn);
-      TICK(3)
       if (ex) export_efc(e, env, nefc);
     }
     if (phases & PH_CTRL) ctrl_run(e, cs, env, sub == 0 ? action : (const R*)nullptr);
-    TICK(4)
     if (phases & PH_STEP2) {
       e.actuation(ex ? s.actuator_force + E * m.nu : nullptr);
       if (e.acceleration()) warn |= 1;
-      TICK(5)
-      BAR
+      __syncthreads();
       niter = solve(e, nefc, ncon, warn);
-      TICK(6)
       if (ex) export_step2(e, env, nefc, niter);
       if (!(phases & PH_NOINTEGRATE)) {
         { int eb = e.euler(&time); if (eb & 32) warn |= 32; else if (eb) warn |= 2; }
       }
-      TICK(7)
     }
     if (live && (phases & PH_OBS) && c_cc[slot].obs_dim > 0) {
       // The reference's observables sample on the LAST substep of a control step: reset()'s forced update already
@@ -191,11 +174,6 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
       if (sub == nsub - 1) { write_obs(e, env, (phases & PH_NOINTEGRATE) != 0); write_task(e, env, ncon); }
     }
     __syncwarp();
-  }
-  if (prof && live && lane == 0)
-  {
-    for (int i = 0; i < 12; i++) s.prof[E * 12 + i] = pc[i];
-    s.dbg[E * 4] = dbgc[0]; s.dbg[E * 4 + 1] = dbgc[1]; s.dbg[E * 4 + 2] = dbgc[2];
   }
   if (!live) return;
   if (phases & PH_CTRL) {

@@ -42,8 +42,7 @@ template <typename R> DEV void kb_from_solref(const R* solref, R dmax, R timeste
 template <typename R> DEV R row_friction(const R* f3, int k) { return k <= 2 ? f3[0] : (k == 3 ? f3[1] : f3[2]); }
 
 // Builds all constraint rows in the workspace.  Returns nefc (warp-uniform).
-template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn, float* pc = nullptr) {
-#define MTICK(slot)
+template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn) {
   const DModel<R>& m = e.model();
   const WSLayout& L = e.lay();
   int lane = e.lane, nv = m.nv;
@@ -158,7 +157,6 @@ template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn, fl
     }
   }
   __syncwarp();
-  MTICK(7)
   // full contact frames (normal, two tangents) into scratch
   {
     R* fr = e.p(L.scratch);
@@ -197,7 +195,6 @@ template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn, fl
     }
   }
   __syncwarp();
-  MTICK(7)
   // per row: velocity, impedance, regularisation, reference acceleration
   R* ejv = e.p(L.e_jv);  // borrow: holds imp of each row until the cone pass
   B2S_LOOP
@@ -252,7 +249,6 @@ template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn, fl
     ejv[r] = imp;
   }
   __syncwarp();
-  MTICK(8)
   // elliptic cones: friction-row regularisation and cone coefficient mu
   const R* cfric = e.p(L.c_fric);
   B2S_LOOP
@@ -268,11 +264,9 @@ template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn, fl
     efl[adr] = f0 * r_sqrt(R1 / R0);  // cone coefficient mu, kept in the (otherwise unused) frictionloss slot
   }
   __syncwarp();
-  MTICK(9)
   B2S_LOOP
   for (int r = lane; r < nefc; r += 32) eD[r] = R(1) / eR[r];
   __syncwarp();
-  MTICK(10)
   return nefc;
 }
 

@@ -21,9 +21,6 @@ enum {
   PH_NOINTEGRATE = 4,  // forward(): everything of step2 except the Euler update
   PH_EXPORT = 8,     // write derived arrays (xpos, qM, contacts, efc ...) to HBM
   PH_CTRL = 16,      // run the fused controller between step1 and step2
-  PH_POLICY = 32,    // first substep of a control step: consume `action` (set_goal)
-  PH_PROFILE = 128,  // accumulate per-phase clock() cycles per environment into `prof`
-  PH_WORKLIST = 256, // pipeline mode: collision narrow phase runs as global work-list kernels
   PH_CTRL_EXT = 512, // pipeline mode: the controller ran as its own kernel (ctrl_osc_kernel), `ctrl` is already in HBM
   PH_OBS = 64        // write the observation row and the task outputs (after the last substep)
 };
@@ -79,8 +76,6 @@ struct DState {
   R* ctrl_torque;  // exported arm torques before clipping (tests)
   R* jv_state;     // [n_env, 72] JOINT_VELOCITY: goal 8, last_err 8, summed 8, derr ring 5x8, ptr, size, saturated
   R* obs;          // [n_env, obs_dim] sampled after the first substep of a control step (observables.py:230-240)
-  float* prof;     // [n_env, 12] cycles per phase (PH_PROFILE)
-  int* dbg;        // [n_env, 4] analytic candidates, convex candidates, EPA calls, reserved
   R* wsg;          // [n_env, L.total] global workspace rows (pipeline mode)
   // pipeline-mode collision work lists (candidate pairs of ALL environments, compacted with atomics)
   int* cl_cnt;     // per group [8]: number of analytic / convex candidates this substep, overflowed environments (small tail tier),

@@ -25,7 +25,10 @@ struct UnitQ {
   int* ctr;       // [8]: 0 head ticket, 1 tail ticket, 2 finished units, 3 overflow head, 4 overflow tail
   int total, n_large, wpb_large;
   int stride, stride_large;  // words of shared memory per warp: small role / large role
-  unsigned long long* prof;  // B2S_UNIT_PROF: [16] clock64 cycles per stage summed over the blocks' rounds (thread 0 of every block), [15] = rounds
+#ifdef B2S_INSTR
+  unsigned long long* prof;  // array "unit_prof" [16]: clock64 cycles per stage of the small role summed over the blocks' rounds
+                             // (thread 0 of every block), [15] = rounds
+#endif
 };
 
 DEV int ld_acquire_gpu(const int* p) { int v; asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory"); return v; }
@@ -194,8 +197,12 @@ __global__ void __launch_bounds__(UNIT_THREADS, UNIT_BLOCKS) unit_kernel(int pha
   const int wpb = blockDim.x >> 5;
   __shared__ int sh_t0, sh_k;
   R* area = smem + (size_t)warp * q.stride;
-#define UTICK(k) if (q.prof != nullptr && threadIdx.x == 0) { long long tn_ = clock64(); atomicAdd(q.prof + (k), (unsigned long long)(tn_ - tprev)); tprev = tn_; }
+#ifdef B2S_INSTR
+#define UTICK(k) if (threadIdx.x == 0) { long long tn_ = clock64(); atomicAdd(q.prof + (k), (unsigned long long)(tn_ - tprev)); tprev = tn_; }
   long long tprev = clock64();
+#else
+#define UTICK(k)
+#endif
   for (;;) {
     // the block takes up to `wpb` tickets that are ALREADY PRODUCED (head < tail).  The first lockstep version took `wpb` tickets
     // whether they existed or not and waited for the missing ones in front of the first stage barrier: every control step stalled until
@@ -223,7 +230,9 @@ __global__ void __launch_bounds__(UNIT_THREADS, UNIT_BLOCKS) unit_kernel(int pha
     const int t0 = sh_t0;
     if (t0 == 0x7fffffff) break;
     UTICK(0)
-    if (q.prof != nullptr && threadIdx.x == 0) atomicAdd(q.prof + 15, 1ull);
+#ifdef B2S_INSTR
+    if (threadIdx.x == 0) atomicAdd(q.prof + 15, 1ull);
+#endif
     const int t = warp < sh_k ? t0 + warp : q.total;
     bool live = t < q.total;
     int code = 0;

@@ -103,7 +103,6 @@ def lib():
         L.b2s_task_objects.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         L.b2s_task_table.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.b2s_set_export.argtypes = [C.c_void_p, C.c_int]
-        L.b2s_set_profile.argtypes = [C.c_void_p, C.c_int]
         L.b2s_set_mode.argtypes = [C.c_void_p, C.c_int]
         L.b2s_launch_count.argtypes = [C.c_void_p]
         L.b2s_launch_count.restype = C.c_int64
@@ -375,9 +374,6 @@ class BatchedSim:
         """0 = fused single kernel, 1 = pipelined phase kernels, 2 = unit queue (one persistent kernel per control step);
         identical results"""
         self._check(self._L.b2s_set_mode(self._h, int(mode)))
-
-    def set_profile(self, flag):
-        self._check(self._L.b2s_set_profile(self._h, int(bool(flag))))
 
     @property
     def launch_count(self):

@@ -2,7 +2,9 @@
 B2S_LIB=robosuite_b200/variants/libb2s_instr.so).  Answers, from data of the CUDA-graph replay itself:
   * how long each kernel of a group-substep runs and how long the gaps between dependent kernels are (%globaltimer stamps);
   * the Newton-iteration / ncon / nefc histograms and line-search evaluations per solve;
-  * how unevenly the environments of one 14-warp block cost (clock64 per environment-substep): block time = slowest warp.
+  * how unevenly the environments of one block cost (clock64 per environment-substep): block time = slowest warp.  Blocks are
+    taken as 8 consecutive warps, the launch bounds' cap and what phase 0 and the small tail tier of the Lift / Panda f32 layouts
+    get; for models whose blocks hold fewer warps the grouping is approximate.
 usage: python tools/probe_instr.py [task] [robot] [n_env] [controller] -> JSON on stdout"""
 import json
 import os
@@ -96,7 +98,7 @@ out["slow_items"] = [dict(cycles=int(r[0]), types=(int(r[1]), int(r[2])), nvert=
                           hit=int(r[8]), staged=int(r[9]), geoms=(gn[int(r[10])], gn[int(r[11])])) for r in sl if r[0] > 0][:40]
 out["slow_items_total"] = int(st[20])
 cy = sim.cyc.cpu().numpy()[:, :25]  # [n, 25, 2]
-wpb = int(os.environ.get("B2S_WPB5", "8"))
+wpb = 8
 for k, nm in ((0, "P0"), (1, "tail")):
     c = cy[:, :, k]
     ge = n // G
