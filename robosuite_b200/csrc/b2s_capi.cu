@@ -82,8 +82,10 @@ struct b2s_sim {
   int slot = -1;             // constant-memory descriptor slot (per device)
   int mc_small = 0, me_small = 0;  // capacities of the small tail tier (== maxcon / maxefc: no tiering)
   int osc_in_tail = 0;       // layouts built for the in-kernel OSC controller (B2S_CTRL_SPLIT=0)
-  int wpb0 = 8, wpb5s = 8, wpb5l = 4;
-  size_t smem0 = 0, smem5s = 0, smem5l = 0;
+  // phase 0: warps per block; tail: warps per block, words per warp of the small and of the large tier, warps per block that run
+  // the large tier
+  int wpb0 = 8, wpb5 = 8, stride5 = 0, stride5l = 0, nlw5 = 1, tail_wide = 0;
+  size_t smem0 = 0, smem5 = 0;
   DModel<float> mf{};
   DModel<double> md{};
   DState<float> sf{};
@@ -604,7 +606,11 @@ static int fit_wpb(size_t per_warp, int cap) {
 }
 static int choose_blocks(b2s_sim* s) {
   size_t rsz = real_size(s);
-  size_t pw0 = s->lay[LAY_P0].total * rsz, pws = s->lay[LAY_TS].total * rsz, pwl = s->lay[LAY_TL].total * rsz, pwf = s->lay[LAY_FULL].fused_stride * rsz;
+  // the tail's per-warp areas start on 16-byte boundaries
+  auto a4 = [](int x) { return (x + 3) & ~3; };
+  s->stride5 = a4(s->lay[LAY_TS].total);
+  s->stride5l = a4(s->lay[LAY_TL].total);
+  size_t pw0 = s->lay[LAY_P0].total * rsz, pws = s->stride5 * rsz, pwl = s->stride5l * rsz, pwf = s->lay[LAY_FULL].fused_stride * rsz;
   if (std::max(std::max(pw0, pws), std::max(pwl, pwf)) > 226 * 1024) return fail(B2S_ERR_UNSUPPORTED, "model workspace exceeds shared memory");
   // warps per block: as many as the launch bounds allow while the launch bounds' blocks per SM still fit one SM's shared memory
   auto pick = [&](size_t pw, int lb_threads, int lb_blocks) {
@@ -614,15 +620,23 @@ static int choose_blocks(b2s_sim* s) {
     return w;
   };
   s->wpb0 = pick(pw0, P0_THREADS, P0_BLOCKS);
-  s->wpb5s = pick(pws, TAIL_THREADS, TAIL_BLOCKS);
-  s->wpb5l = fit_wpb(pwl, TAIL_THREADS / 32);
-  s->smem0 = pw0 * s->wpb0; s->smem5s = pws * s->wpb5s; s->smem5l = pwl * s->wpb5l;
+  // tail block shape: one 16-warp block per SM when 16 small-tier areas take at most 160 KB, else two blocks per SM.  Measured on an
+  // H100 80GB HBM3 (700 W), env-steps/s two blocks -> one: Lift / Panda f32 (16 areas 146 KB) 310 k -> 325 k; Stack / Sawyer JV f32
+  // (202 KB) 385 k -> 369 k; NutAssemblyRound (52 KB per area: 4 warps in one block) 55.2 k -> 49.9 k
+  s->wpb5 = pick(pws, TAIL_THREADS, TAIL_BLOCKS);
+  const int wide_w = TAIL_WIDE_THREADS / 32;
+  s->tail_wide = pws * wide_w <= 160 * 1024;
+  if (s->tail_wide) s->wpb5 = wide_w;
+  // the large tier reuses the block's small-tier areas: as many full-capacity areas as they hold, at least one
+  s->smem5 = std::max(pws * s->wpb5, pwl);
+  s->nlw5 = std::max(1, std::min(s->wpb5, (int)(s->smem5 / pwl)));
+  s->smem0 = pw0 * s->wpb0;
   int wf = fit_wpb(pwf, 16);
   s->wpb_fused = wf; s->smem_fused = pwf * wf;
   if (getenv("B2S_VERBOSE"))
-    fprintf(stderr, "[b2s] slot %d words/warp: fused %d, P0 %d (%d warps/block), tail small %d [mc %d me %d] (%d warps/block), tail large %d [mc %d me %d] (%d), row %d\n",
-            s->slot, s->lay[LAY_FULL].fused_stride, s->lay[LAY_P0].total, s->wpb0, s->lay[LAY_TS].total, s->mc_small, s->me_small, s->wpb5s,
-            s->lay[LAY_TL].total, s->maxcon, s->maxefc, s->wpb5l, s->lay[LAY_ROW].total);
+    fprintf(stderr, "[b2s] slot %d words/warp: fused %d, P0 %d (%d warps/block), tail small %d [mc %d me %d] (%d warps/block, wide %d), tail large %d [mc %d me %d] (%d), row %d\n",
+            s->slot, s->lay[LAY_FULL].fused_stride, s->lay[LAY_P0].total, s->wpb0, s->lay[LAY_TS].total, s->mc_small, s->me_small, s->wpb5, s->tail_wide,
+            s->lay[LAY_TL].total, s->maxcon, s->maxefc, s->nlw5, s->lay[LAY_ROW].total);
   return B2S_OK;
 }
 
@@ -727,7 +741,8 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
       using R = real_of<decltype(m)>;
       cudaError_t e = optin_max_smem(step_kernel<R>, device);
       if (e == cudaSuccess) e = optin_max_smem(phase0_kernel<R>, device);
-      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_THREADS>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_WIDE_THREADS>, device);
       if (e == cudaSuccess) e = optin_max_smem(phase1_kernel<R>, device);
       return e;
     });
@@ -830,28 +845,27 @@ template <typename R>
 static int enqueue_group(b2s_sim* s, const DModel<R>& m, const DState<R>& st, int phases, int nsub, const R* action, int gi, int G, cudaStream_t q) {
   const int epaw = (EPA_AREA_WORDS(EPA_MAXV, EPA_MAXF) + m.stage_cap) * (int)sizeof(R);
   const int p1smem = std::max(epaw, (int)osc_smem_bytes<R>());  // one block shape for the three roles of phase 1
-  const bool tiered = s->mc_small < s->maxcon || s->me_small < s->maxefc;
   int e0 = (int)((long long)s->n_env * gi / G), e1 = (int)((long long)s->n_env * (gi + 1) / G);
   Grp g{e0, e1 - e0, gi, 0, s->slot};
-  int blocks0 = (g.nenv + s->wpb0 - 1) / s->wpb0, blocks5 = (g.nenv + s->wpb5s - 1) / s->wpb5s;
-  int blocksL = std::min((g.nenv + s->wpb5l - 1) / s->wpb5l, 2 * s->num_sms);  // large tier: warps claim overflowed environments
+  int blocks0 = (g.nenv + s->wpb0 - 1) / s->wpb0, blocks5 = (g.nenv + s->wpb5 - 1) / s->wpb5;
   int nA = g.nenv * st.cl_maxa, nG = g.nenv * st.cl_maxg;
   // convex role: one warp per block, items claimed through a counter.  ~1.6 items per environment are queued per substep (Lift), most of
   // them dismissed in a few microseconds: half a block per environment keeps every slow item on its own warp without flooding the
   // block scheduler with thousands of empty blocks per launch
   const int cvx_blocks = std::max(s->num_sms, g.nenv / 2);
   const bool ctrl_ext = (phases & PH_CTRL_EXT) != 0;
+  // the group's work-list counters for substep 0 (each tail launch zeroes them for the next substep)
+  CUDA_TRY(cudaMemsetAsync(st.cl_cnt + 8 * gi, 0, 8 * sizeof(int), q));
   for (int sub = 0; sub < nsub; sub++) {
     g.sub = sub;
-    CUDA_TRY(cudaMemsetAsync(st.cl_cnt + 8 * gi, 0, 8 * sizeof(int), q));
     phase0_kernel<R><<<blocks0, s->wpb0 * 32, s->smem0, q>>>(phases, g);
     // phase 1: convex narrow phase | controller | analytic narrow phase as block roles of ONE launch (no forks in the graph).
     // Upper bounds of the candidate counts size the grid; warps / threads beyond the device-side counts exit at once.
     P1Cfg c{std::min(nG, cvx_blocks), ctrl_ext ? (g.nenv + OSC_TPB - 1) / OSC_TPB : 0, sub};
     int nAb = (nA + 31) / 32;
     if (c.nG + c.nC + nAb > 0) phase1_kernel<R><<<c.nG + c.nC + nAb, 32, p1smem, q>>>(action, g, c);
-    tail_kernel<R><<<blocks5, s->wpb5s * 32, s->smem5s, q>>>(phases, nsub, action, g, 0);
-    if (tiered) tail_kernel<R><<<blocksL, s->wpb5l * 32, s->smem5l, q>>>(phases, nsub, action, g, 1);
+    if (s->tail_wide) tail_kernel<R, TAIL_WIDE_THREADS><<<blocks5, s->wpb5 * 32, s->smem5, q>>>(phases, nsub, action, g, s->stride5, s->stride5l, s->nlw5);
+    else tail_kernel<R, TAIL_THREADS><<<blocks5, s->wpb5 * 32, s->smem5, q>>>(phases, nsub, action, g, s->stride5, s->stride5l, s->nlw5);
   }
   CUDA_TRY(cudaGetLastError());
   return B2S_OK;
@@ -867,7 +881,6 @@ template <typename R> static int ensure_ws(b2s_sim* s, const DModel<R>& m, DStat
     st.wsg = p;
     size_t ne = (size_t)s->n_env;
     st.cl_cnt = dev_zeros<int>(s, 8 * 64);
-    st.ovf_list = dev_zeros<int>(s, ne);
     // candidate capacity per environment: small models keep small grids (the narrow-phase grids are sized by these bounds)
     st.cl_maxa = s->maxcon <= 32 ? 8 : (s->maxcon <= 48 ? 16 : CL_MAXA);
     st.cl_maxg = s->maxcon <= 32 ? 16 : CL_MAXG;
@@ -894,7 +907,7 @@ template <typename R> static int ensure_ws(b2s_sim* s, const DModel<R>& m, DStat
   return B2S_OK;
 }
 
-// ---- pipeline mode: CUDA-graph replay.  The launch sequence of one environment group (nsub substeps x 3-4 kernels) is captured
+// ---- pipeline mode: CUDA-graph replay.  The launch sequence of one environment group (nsub substeps x 3 kernels) is captured
 // once per (phases, nsub, action given) and replayed on the group's own stream, forked from and joined to the handle's stream: the
 // groups' chains then overlap freely (inside ONE graph, parallel branches were observed to share a limited number of execution
 // lanes).  The action rows are staged into a fixed buffer so kernel arguments never change.
@@ -919,8 +932,7 @@ static int launch_pipeline(b2s_sim* s, int phases, int nsub, const void* action)
       s->gstreams.push_back(st2); s->gevents.push_back(ev);
     }
     if (!s->in_event) CUDA_TRY(cudaEventCreateWithFlags(&s->in_event, cudaEventDisableTiming));
-    const bool tiered = s->mc_small < s->maxcon || s->me_small < s->maxefc;
-    const int launches_per_call = G * nsub * (3 + (tiered ? 1 : 0));  // phase 0, phase 1 (narrow phase + controller), tail, [tail large tier]
+    const int launches_per_call = G * nsub * 3;  // phase 0, phase 1 (narrow phase + controller), tail (both capacity tiers)
     const R* act_in = (const R*)action;
     if (action) {
       int ad = s->ctrl.action_dim > 0 ? s->ctrl.action_dim : 1;

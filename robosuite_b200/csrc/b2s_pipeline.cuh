@@ -4,8 +4,8 @@
 // b2s_collide.cuh), and the stage sequences (phase 0, the tail stages) are defined here once for this pipeline and the unit queue; what
 // changes is scheduling and MEMORY:
 // every kernel has its own compact shared-memory layout (LAY_P0 / LAY_TS / LAY_TL), so 24-28 warps are resident per SM instead of
-// the 14 the one-size-fits-all layout allowed, and the tail kernel runs in two capacity tiers: the small tier holds the contact /
-// row counts almost every environment has, the few that need more are re-run by the large tier (same results, no truncation).
+// the 14 the one-size-fits-all layout allowed, and the tail runs in two capacity tiers: the small tier holds the contact / row counts
+// almost every environment has, the few that need more are re-run by the large tier in the same block (same results, no truncation).
 #pragma once
 #include "b2s_kernel.cuh"
 
@@ -72,7 +72,9 @@ template <typename R> DEV void ws_store(const Eng<R>& e, R* row, const PhaseIO& 
 // A launch covers one group of environments [env0, env0 + nenv); groups run on separate streams so that the tail of one
 // group's kernel (its slowest environment) overlaps with other groups' work.  slot = descriptor slot of the owning handle.
 struct Grp { int env0, nenv, gid, sub, slot; };
-#define CLC(s, g) ((s).cl_cnt + 8 * (g).gid)  // this group's counters: nA, nG, overflowed envs, next convex item, next overflow item
+// this group's counters: nA, nG, (spare), next convex item.  phase0_kernel(s) appends, phase1_kernel(s) consumes, tail_kernel(s) zeroes
+// them at entry for phase0_kernel(s + 1); the memset at the head of the group's graph zeroes them for substep 0
+#define CLC(s, g) ((s).cl_cnt + 8 * (g).gid)
 
 // -DB2S_INSTR: every launch stamps its first / last %globaltimer into st_begin / st_end (device timeline of the CUDA-graph
 // replay, which events cannot subdivide), warps record their clock64 cost per environment-substep.  Empty in product builds.
@@ -367,9 +369,13 @@ DEV void tail_finish(Eng<R>& e, int env, int sub, int nsub, int phases, int ncon
 // thread: with (256, 3) = 80 registers the heavily spilling build mis-executed solve() on 21-dof models (a corrupted workspace
 // pointer, found with compute-sanitizer) - the same family of nvcc 12.9 stack-slot problems as DESIGN.md section 3 records.
 // The kernels are latency bound at 4096 environments (every environment's warp is resident either way), so the lost occupancy
-// costs nothing measurable (256 x 2 was the fastest of the launch-bound variants measured).
+// costs nothing measurable (256 x 2 was the fastest of the launch-bound variants measured for phase 0).
+// The tail has a second block shape, ONE block of 16 warps per SM, (512, 1), also 128 registers: such a block takes the whole register
+// file, so an SM executes one tail block and nothing else until the block is done, instead of two 8-warp blocks (often of different
+// substeps or groups) beside 1-warp phase-1 blocks.  choose_blocks (b2s_capi.cu) says which shape a model gets.
 constexpr int P0_THREADS = 256, P0_BLOCKS = 2;      // phase 0
-constexpr int TAIL_THREADS = 256, TAIL_BLOCKS = 2;  // tail kernel
+constexpr int TAIL_THREADS = 256, TAIL_BLOCKS = 2;  // tail kernel, two blocks per SM
+constexpr int TAIL_WIDE_THREADS = 512;              // tail kernel, one block per SM
 
 // ---- phase 0: kinematics, velocity stage + RNE bias, CRB -> M, broad phase -> global candidate work lists
 template <typename R>
@@ -404,57 +410,59 @@ __global__ void __launch_bounds__(P0_THREADS, P0_BLOCKS) phase0_kernel(int phase
   INSTR_END(s, g, 0)
 }
 
-// ---- tail: gather contacts, constraint rows + Jacobian, (in-kernel controller), actuation, Newton solve, Euler, observations.
-// tier 0: warp per environment of the group, small-capacity layout; an environment whose contacts / rows do not fit is appended to
-// the group's overflow list untouched.  tier 1: warps claim the overflowed environments and run them with the full-capacity layout.
+// ---- tail: gather contacts, constraint rows + Jacobian, (in-kernel controller), actuation, Newton solve, Euler, observations.  One
+// environment with the layout `lid` in the warp's `area`; returns 1 (nothing of the environment's state touched) if it does not fit
+// the layout.  Compiled separately: the kernel calls it for both tiers.
 template <typename R>
-__global__ void __launch_bounds__(TAIL_THREADS, TAIL_BLOCKS) tail_kernel(int phases, int nsub, const R* action, Grp g, int tier) {
+DEVN int tail_env(R* area, int lane, int lid, Grp g, int env, int nsub, int phases, const R* action, unsigned long long* bar, unsigned& parity) {
+  const int sub = g.sub;
+  Eng<R> e(area, lane, g.slot, lid);
+#ifdef B2S_INSTR
   const DState<R>& s = cstate<R>(g.slot);
-  const int lid = tier ? LAY_TL : LAY_TS;
-  const WSLayout& L = c_lay[g.slot][lid];
+  long long instr_t0 = clock64();
+#endif
+  const int pk = tail_rows(e, env, bar, parity);
+  if (TAIL_OVF(pk)) return 1;
+  const int ncon = TAIL_NCON(pk), nefc = TAIL_NEFC(pk);
+  int warn = TAIL_WARN(pk);
+  if ((phases & PH_CTRL) && !(phases & PH_CTRL_EXT)) tail_ctrl(e, env, sub, action);
+  warn |= tail_accel(e);
+  warn |= tail_newton(e, nefc, ncon);
+  tail_finish(e, env, sub, nsub, phases, ncon, warn, bar, parity);
+#ifdef B2S_INSTR
+  if (lane == 0 && s.cyc) s.cyc[((size_t)env * 32 + (sub & 31)) * 2 + 1] = (float)(clock64() - instr_t0);
+  if (lane == 0 && s.stats) { atomicAdd(s.stats + 32 + min(ncon, 128), 1); atomicAdd(s.stats + 176 + min(nefc, 320), 1); if (lid == LAY_TL) atomicAdd(s.stats + 19, 1); }
+#endif
+  return 0;
+}
+
+// Warp per environment of the group with the small-capacity layout (`stride` words per warp); an environment that does not fit is
+// left in the block's overflow list.  After a block barrier the first `nlw` warps re-run the block's overflowed environments with the
+// full-capacity layout (`stride_l` words per warp, over the small tier's dead areas).  An overflowed environment waits for its own
+// block only, not for the whole group.
+template <typename R, int THREADS>
+__global__ void __launch_bounds__(THREADS, THREADS == TAIL_WIDE_THREADS ? 1 : TAIL_BLOCKS) tail_kernel(int phases, int nsub, const R* action, Grp g, int stride, int stride_l, int nlw) {
+  const DState<R>& s = cstate<R>(g.slot);
   extern __shared__ __align__(16) unsigned char smem_raw[];
   R* smem = reinterpret_cast<R*>(smem_raw);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpb = blockDim.x >> 5, sub = g.sub;
-  INSTR_BEGIN(s, g, tier ? 5 : 3)
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
+  INSTR_BEGIN(s, g, 3)
   __shared__ unsigned long long mbar[32];  // one transaction barrier per warp (TMA loads of its workspace regions)
+  __shared__ int ovf[32];                  // per warp: its environment if it did not fit the small tier, else -1
+  if (blockIdx.x == 0 && threadIdx.x == 0) { int* c = CLC(s, g); c[0] = 0; c[1] = 0; c[3] = 0; }  // phase1_kernel is done with them
   if (lane == 0) mbar_init(&mbar[warp]);
   __syncwarp();
   unsigned parity = 0;
-  Eng<R> e(smem + (size_t)warp * L.total, lane, g.slot, lid);
-  int* clc = CLC(s, g);
-  for (int iter = 0;; iter++) {
-    int env;
-    if (tier == 0) {
-      if (iter > 0) break;
-      env = blockIdx.x * wpb + warp;
-      if (env >= g.nenv) break;
-      env += g.env0;
-    } else {
-      int item = 0;
-      if (lane == 0) item = atomicAdd(clc + 4, 1);
-      item = __shfl_sync(B2S_FULL, item, 0);
-      if (item >= clc[2]) break;
-      env = s.ovf_list[g.env0 + item];
-    }
-#ifdef B2S_INSTR
-    long long instr_t0 = clock64();
-#endif
-    const int pk = tail_rows(e, env, &mbar[warp], parity);
-    if (TAIL_OVF(pk)) {  // does not fit this tier: nothing of the environment's state has been touched yet
-      if (lane == 0) s.ovf_list[g.env0 + atomicAdd(clc + 2, 1)] = env;
-      __syncwarp();
-      continue;
-    }
-    const int ncon = TAIL_NCON(pk), nefc = TAIL_NEFC(pk);
-    int warn = TAIL_WARN(pk);
-    if ((phases & PH_CTRL) && !(phases & PH_CTRL_EXT)) tail_ctrl(e, env, sub, action);
-    warn |= tail_accel(e);
-    warn |= tail_newton(e, nefc, ncon);
-    tail_finish(e, env, sub, nsub, phases, ncon, warn, &mbar[warp], parity);
-#ifdef B2S_INSTR
-    if (lane == 0 && s.cyc) s.cyc[((size_t)env * 32 + (sub & 31)) * 2 + 1] = (float)(clock64() - instr_t0);
-    if (lane == 0 && s.stats) { atomicAdd(s.stats + 32 + min(ncon, 128), 1); atomicAdd(s.stats + 176 + min(nefc, 320), 1); if (tier) atomicAdd(s.stats + 19, 1); }
-#endif
-  }
-  INSTR_END(s, g, tier ? 5 : 3)
+  const int env = g.env0 + blockIdx.x * wpb + warp;
+  int o = -1;
+  if (env < g.env0 + g.nenv && tail_env<R>(smem + (size_t)warp * stride, lane, LAY_TS, g, env, nsub, phases, action, &mbar[warp], parity)) o = env;
+  if (lane == 0) ovf[warp] = o;
+  // the small tier's areas are dead from here on (every fitting environment has stored its state, ws_store waited for its bulk
+  // stores); order this thread's generic accesses to them before the large tier's bulk loads into the same shared memory
+  asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+  __syncthreads();
+  if (warp < nlw)
+    for (int k = warp; k < wpb; k += nlw)
+      if (ovf[k] >= 0) tail_env<R>(smem + (size_t)warp * stride_l, lane, LAY_TL, g, ovf[k], nsub, phases, action, &mbar[warp], parity);
+  INSTR_END(s, g, 3)
 }

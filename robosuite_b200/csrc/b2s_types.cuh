@@ -78,9 +78,7 @@ struct DState {
   R* obs;          // [n_env, obs_dim] sampled after the first substep of a control step (observables.py:230-240)
   R* wsg;          // [n_env, L.total] global workspace rows (pipeline mode)
   // pipeline-mode collision work lists (candidate pairs of ALL environments, compacted with atomics)
-  int* cl_cnt;     // per group [8]: number of analytic / convex candidates this substep, overflowed environments (small tail tier),
-                   // next convex work item, next overflow item, (spare x3)
-  int* ovf_list;   // [n_env] environments whose contacts / rows did not fit the small tier (group g's slice starts at its env0)
+  int* cl_cnt;     // per group [8]: number of analytic / convex candidates this substep, (spare), next convex work item, (spare x4)
   int cl_maxa, cl_maxg;  // per-environment candidate capacity of the two work lists
   int* cl_listA;   // [n_env * cl_maxa] env << 12 | pair
   int* cl_listG;   // [n_env * cl_maxg]

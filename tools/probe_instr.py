@@ -3,8 +3,8 @@ B2S_LIB=robosuite_b200/variants/libb2s_instr.so).  Answers, from data of the CUD
   * how long each kernel of a group-substep runs and how long the gaps between dependent kernels are (%globaltimer stamps);
   * the Newton-iteration / ncon / nefc histograms and line-search evaluations per solve;
   * how unevenly the environments of one block cost (clock64 per environment-substep): block time = slowest warp.  Blocks are
-    taken as 8 consecutive warps, the launch bounds' cap and what phase 0 and the small tail tier of the Lift / Panda f32 layouts
-    get; for models whose blocks hold fewer warps the grouping is approximate.
+    taken as 8 (phase 0) and 16 (tail) consecutive warps, the launch bounds' caps and what the Lift / Panda f32 layouts get; for
+    models whose blocks hold fewer warps the grouping is approximate.
 usage: python tools/probe_instr.py [task] [robot] [n_env] [controller] -> JSON on stdout"""
 import json
 import os
@@ -49,7 +49,7 @@ valid = e[:G, :25] > 0
 t0 = b[:G, :25][valid].min()
 B = (b[:G, :25].astype(np.float64) - float(t0)) / 1e3  # us
 E = (e[:G, :25].astype(np.float64) - float(t0)) / 1e3
-names = ["P0", "narrowA", "narrowG", "tail", "ctrl", "tailL"]
+names = ["P0", "narrowA", "narrowG", "tail", "ctrl"]  # the tail launch runs both capacity tiers
 out = {"task": task, "robot": robot, "n_env": n, "controller": ctrl, "groups": G, "step_ms_events": step_ms,
        "span_us": float(E.max()), "kernels": {}, "gaps_us": {}}
 for k, nm in enumerate(names):
@@ -65,6 +65,9 @@ out["gaps_us"]["tail->next P0"] = float((B[:, 1:, 0] - E[:, :-1, 3]).mean())
 if "ctrl" in out["kernels"]:
     out["gaps_us"]["P0->ctrl"] = float((B[:, :, 4] - E[:, :, 0]).mean())
     out["gaps_us"]["ctrl->tail"] = float((B[:, :, 3] - E[:, :, 4]).mean())
+# a group's serial chain per substep: end of its tail launch of substep s -> end of its tail launch of substep s + 1
+ch = E[:, 1:, 3] - E[:, :-1, 3]
+out["chain_us"] = {"mean": float(ch.mean()), "p50": float(np.median(ch)), "max": float(ch.max())}
 per_group_busy = sum((E[:, :, k] - B[:, :, k]).sum(1) for k in range(4))
 out["per_group_kernel_time_us"] = [float(x) for x in per_group_busy]
 out["per_group_span_us"] = [float(E[g].max() - B[g].min()) for g in range(G)]
@@ -98,8 +101,7 @@ out["slow_items"] = [dict(cycles=int(r[0]), types=(int(r[1]), int(r[2])), nvert=
                           hit=int(r[8]), staged=int(r[9]), geoms=(gn[int(r[10])], gn[int(r[11])])) for r in sl if r[0] > 0][:40]
 out["slow_items_total"] = int(st[20])
 cy = sim.cyc.cpu().numpy()[:, :25]  # [n, 25, 2]
-wpb = 8
-for k, nm in ((0, "P0"), (1, "tail")):
+for k, nm, wpb in ((0, "P0", 8), (1, "tail", 16)):
     c = cy[:, :, k]
     ge = n // G
     ratios, lratios = [], []
