@@ -48,7 +48,9 @@ int b2s_step(b2s_sim* sim, int n_substeps);
 /* Named device arrays, leading dimension n_env: qpos qvel qacc qacc_warmstart ctrl time xpos xquat xmat
  * site_xpos site_xmat geom_xpos geom_xmat qM(dense nv x nv) qfrc_bias qfrc_passive qfrc_actuator qfrc_constraint
  * actuator_force ncon contact_geom contact_dist contact_pos contact_frame nefc efc_force warn ...
- * (the attributes the reference touches, SURVEY.md section 8b).  dtype is B2S_F32/F64/I32. */
+ * (the attributes the reference touches, SURVEY.md section 8b).  dtype is B2S_F32/F64/I32.  After the first pipeline-mode step also
+ * tail_key (i32: each environment's tail cost class) and tail_order (i32: per group, the environment each warp position of the last
+ * tail launch ran), the cost order the pipeline's tail hands environments to warps in; written when tail blocks hold 8 warps or more. */
 int b2s_array(b2s_sim* sim, const char* name, void** dev_ptr, int* dtype, int* ndim, int64_t shape[4]);
 
 /* MjSim.get_state().flatten() / set_state_from_flattened (binding_utils.py:1155-1184, MjSimState.flatten :56-70): device buffers

@@ -627,6 +627,12 @@ static int choose_blocks(b2s_sim* s) {
   const int wide_w = TAIL_WIDE_THREADS / 32;
   s->tail_wide = pws * wide_w <= 160 * 1024;
   if (s->tail_wide) s->wpb5 = wide_w;
+  // the tail's cost order (tail_kernel<.., SORTED = true>) for blocks of 8 warps or more: the slack it recovers (a block waits for the
+  // slowest of its warps) grows with the warps per block.  Measured on an H100 80GB HBM3 (700 W), env-steps/s by id -> sorted: Lift /
+  // Panda f32 (16 warps) 323 k -> 335 k, Stack / Sawyer JV f32 (8 warps, two blocks per SM) 383 k -> 397 k; NutAssemblyRound (52 KB
+  // areas, 2 warps per block) 55.2 k -> 54.0 k.  Smaller blocks run the id-order instantiation, which has none of the order's code.
+  const int sorted = s->wpb5 >= 8 ? 1 : 0;
+  with_real(s, [&](auto&, auto& st) { st.tail_sorted = sorted; return 0; });
   // the large tier reuses the block's small-tier areas: as many full-capacity areas as they hold, at least one
   s->smem5 = std::max(pws * s->wpb5, pwl);
   s->nlw5 = std::max(1, std::min(s->wpb5, (int)(s->smem5 / pwl)));
@@ -741,8 +747,9 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
       using R = real_of<decltype(m)>;
       cudaError_t e = optin_max_smem(step_kernel<R>, device);
       if (e == cudaSuccess) e = optin_max_smem(phase0_kernel<R>, device);
-      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_THREADS>, device);
-      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_WIDE_THREADS>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_THREADS, false>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_THREADS, true>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_WIDE_THREADS, true>, device);
       if (e == cudaSuccess) e = optin_max_smem(phase1_kernel<R>, device);
       return e;
     });
@@ -854,8 +861,8 @@ static int enqueue_group(b2s_sim* s, const DModel<R>& m, const DState<R>& st, in
   // block scheduler with thousands of empty blocks per launch
   const int cvx_blocks = std::max(s->num_sms, g.nenv / 2);
   const bool ctrl_ext = (phases & PH_CTRL_EXT) != 0;
-  // the group's work-list counters for substep 0 (each tail launch zeroes them for the next substep)
-  CUDA_TRY(cudaMemsetAsync(st.cl_cnt + 8 * gi, 0, 8 * sizeof(int), q));
+  // the group's work-list counters and both tail class sets for substep 0 (each tail launch zeroes them for the next substep)
+  CUDA_TRY(cudaMemsetAsync(st.cl_cnt + CL_CNT_STRIDE * gi, 0, CL_CNT_STRIDE * sizeof(int), q));
   for (int sub = 0; sub < nsub; sub++) {
     g.sub = sub;
     phase0_kernel<R><<<blocks0, s->wpb0 * 32, s->smem0, q>>>(phases, g);
@@ -864,8 +871,9 @@ static int enqueue_group(b2s_sim* s, const DModel<R>& m, const DState<R>& st, in
     P1Cfg c{std::min(nG, cvx_blocks), ctrl_ext ? (g.nenv + OSC_TPB - 1) / OSC_TPB : 0, sub};
     int nAb = (nA + 31) / 32;
     if (c.nG + c.nC + nAb > 0) phase1_kernel<R><<<c.nG + c.nC + nAb, 32, p1smem, q>>>(action, g, c);
-    if (s->tail_wide) tail_kernel<R, TAIL_WIDE_THREADS><<<blocks5, s->wpb5 * 32, s->smem5, q>>>(phases, nsub, action, g, s->stride5, s->stride5l, s->nlw5);
-    else tail_kernel<R, TAIL_THREADS><<<blocks5, s->wpb5 * 32, s->smem5, q>>>(phases, nsub, action, g, s->stride5, s->stride5l, s->nlw5);
+    if (s->tail_wide) tail_kernel<R, TAIL_WIDE_THREADS, true><<<blocks5, s->wpb5 * 32, s->smem5, q>>>(phases, nsub, action, g, s->stride5, s->stride5l, s->nlw5);
+    else if (st.tail_sorted) tail_kernel<R, TAIL_THREADS, true><<<blocks5, s->wpb5 * 32, s->smem5, q>>>(phases, nsub, action, g, s->stride5, s->stride5l, s->nlw5);
+    else tail_kernel<R, TAIL_THREADS, false><<<blocks5, s->wpb5 * 32, s->smem5, q>>>(phases, nsub, action, g, s->stride5, s->stride5l, s->nlw5);
   }
   CUDA_TRY(cudaGetLastError());
   return B2S_OK;
@@ -880,7 +888,10 @@ template <typename R> static int ensure_ws(b2s_sim* s, const DModel<R>& m, DStat
     s->allocs.push_back(p);
     st.wsg = p;
     size_t ne = (size_t)s->n_env;
-    st.cl_cnt = dev_zeros<int>(s, 8 * 64);
+    st.cl_cnt = dev_zeros<int>(s, CL_CNT_STRIDE * 64);
+    st.tail_key = dev_zeros<int>(s, ne); st.tail_list = dev_zeros<int>(s, ne * TAIL_NKEY); st.tail_order = dev_zeros<int>(s, ne);
+    s->arrays["tail_key"] = ArrayInfo{st.tail_key, B2S_I32, 1, {(int64_t)ne, 0, 0, 0}};
+    s->arrays["tail_order"] = ArrayInfo{st.tail_order, B2S_I32, 1, {(int64_t)ne, 0, 0, 0}};
     // candidate capacity per environment: small models keep small grids (the narrow-phase grids are sized by these bounds)
     st.cl_maxa = s->maxcon <= 32 ? 8 : (s->maxcon <= 48 ? 16 : CL_MAXA);
     st.cl_maxg = s->maxcon <= 32 ? 16 : CL_MAXG;
@@ -891,11 +902,11 @@ template <typename R> static int ensure_ws(b2s_sim* s, const DModel<R>& m, DStat
     s->action_buf = dev_zeros<R>(s, ne * 16);
 #ifdef B2S_INSTR
     st.st_begin = dev_zeros<unsigned long long>(s, 64 * 32 * 8); st.st_end = dev_zeros<unsigned long long>(s, 64 * 32 * 8);
-    st.stats = dev_zeros<int>(s, 512); st.cyc = dev_zeros<float>(s, ne * 64);
+    st.stats = dev_zeros<int>(s, 512); st.cyc = dev_zeros<float>(s, ne * 32 * 8); st.solve_ls = dev_zeros<int>(s, ne);
     s->arrays["st_begin"] = ArrayInfo{st.st_begin, B2S_I64, 1, {64 * 32 * 8, 0, 0, 0}};
     s->arrays["st_end"] = ArrayInfo{st.st_end, B2S_I64, 1, {64 * 32 * 8, 0, 0, 0}};
     s->arrays["stats"] = ArrayInfo{st.stats, B2S_I32, 1, {512, 0, 0, 0}};
-    s->arrays["cyc"] = ArrayInfo{st.cyc, B2S_F32, 3, {(int64_t)ne, 32, 2, 0}};
+    s->arrays["cyc"] = ArrayInfo{st.cyc, B2S_F32, 3, {(int64_t)ne, 32, 8, 0}};
     st.slowlog = dev_zeros<int>(s, 64 * 12);
     s->arrays["slowlog"] = ArrayInfo{st.slowlog, B2S_I32, 2, {64, 12, 0, 0}};
     s->uq_prof = dev_zeros<unsigned long long>(s, 16);

@@ -74,7 +74,17 @@ template <typename R> DEV void ws_store(const Eng<R>& e, R* row, const PhaseIO& 
 struct Grp { int env0, nenv, gid, sub, slot; };
 // this group's counters: nA, nG, (spare), next convex item.  phase0_kernel(s) appends, phase1_kernel(s) consumes, tail_kernel(s) zeroes
 // them at entry for phase0_kernel(s + 1); the memset at the head of the group's graph zeroes them for substep 0
-#define CLC(s, g) ((s).cl_cnt + 8 * (g).gid)
+#define CLC(s, g) ((s).cl_cnt + CL_CNT_STRIDE * (g).gid)
+// then the environments per tail cost class, one set per substep parity: phase0_kernel(s) counts into set s & 1, every block of
+// tail_kernel(s) reads it, tail_kernel(s) zeroes set (s + 1) & 1 for phase0_kernel(s + 1); the head memset zeroes both
+#define CLK(s, g, sub) (CLC(s, g) + 8 + TAIL_NKEY * ((sub) & 1))
+
+// Tail cost class of an environment-substep, 0 .. TAIL_NKEY - 1 (most expensive last), from its deterministic counts: Newton
+// iterations, constraint rows, and whether it needed the full-capacity tier.  Fitted against the INSTR build's recorded tail cycles
+// (tools/probe_tail_order.py, DESIGN.md section 6); the probe repeats this formula.
+DEV int tail_cost_key(int niter, int nefc, bool large) {
+  return large ? TAIL_NKEY - 1 : min(TAIL_NKEY - 2, (niter * (nefc + 24) + 2 * nefc) / 48);
+}
 
 // -DB2S_INSTR: every launch stamps its first / last %globaltimer into st_begin / st_end (device timeline of the CUDA-graph
 // replay, which events cannot subdivide), warps record their clock64 cost per environment-substep.  Empty in product builds.
@@ -333,14 +343,15 @@ template <typename R> DEV void tail_ctrl(Eng<R>& e, int env, int sub, const R* a
 }
 
 // Dynamics, in two parts (the unit queue puts a block barrier between them): actuation + smooth acceleration, then the Newton solve.
-// Both return warn bits.
+// Both return warn bits; the solve also reports its Newton iterations.
 template <typename R> DEV int tail_accel(Eng<R>& e) {
   e.actuation((R*)nullptr);
   return e.acceleration() ? 1 : 0;
 }
-template <typename R> DEV int tail_newton(Eng<R>& e, int nefc, int ncon) {
+template <typename R> DEV int tail_newton(Eng<R>& e, int nefc, int ncon, int* niter = nullptr) {
   int warn = 0;
-  solve(e, nefc, ncon, warn);
+  const int it = solve(e, nefc, ncon, warn);
+  if (niter) *niter = it;
   return warn;
 }
 
@@ -400,22 +411,59 @@ __global__ void __launch_bounds__(P0_THREADS, P0_BLOCKS) phase0_kernel(int phase
   if (lane == 0) {
     if (na) baseA = g.env0 * s.cl_maxa + atomicAdd(CLC(s, g), na);
     if (ng) baseG = g.env0 * s.cl_maxg + atomicAdd(CLC(s, g) + 1, ng);
+    if (s.tail_sorted) {  // the environment's cost class of its last tail files it for this substep's tail (tail_env_at)
+      const int k = s.tail_key[env];
+      s.tail_list[(size_t)g.env0 * TAIL_NKEY + k * g.nenv + atomicAdd(CLK(s, g, g.sub) + k, 1)] = env;
+    }
   }
   baseA = __shfl_sync(B2S_FULL, baseA, 0);
   baseG = __shfl_sync(B2S_FULL, baseG, 0);
   phase0_publish(e, env, na, ng, warn, baseA, baseG, true);
 #ifdef B2S_INSTR
-  if (lane == 0 && s.cyc) s.cyc[((size_t)env * 32 + (g.sub & 31)) * 2] = (float)(clock64() - instr_t0);
+  if (lane == 0 && s.cyc) s.cyc[((size_t)env * 32 + (g.sub & 31)) * 8] = (float)(clock64() - instr_t0);
 #endif
   INSTR_END(s, g, 0)
 }
 
+// The environment at warp position p of the group's tail launch.  The group's environments are ranked by the cost classes phase 0
+// filed them under, most expensive first, in filing order within a class.  Low positions are the blocks the scheduler starts first,
+// so the expensive environments share blocks (a block holds its SM until its slowest warp is done) and start early.  The first
+// TAIL_SOLO blocks are the exception: warp 0 of block b takes rank b and the block's other warps the cheapest ranks, so the launch's
+// most expensive environments run beside warps that are soon done instead of beside other expensive ones (the launch, and with it
+// the group's chain, ends with its slowest environment).
+template <typename R> DEV int tail_env_at(const Grp& g, int p, int lane) {
+  const DState<R>& s = cstate<R>(g.slot);
+  const int wpb = blockDim.x >> 5;
+  if (TAIL_SOLO * wpb <= g.nenv) {  // p -> rank
+    const int b = p / wpb, w = p - b * wpb;
+    if (b >= TAIL_SOLO) p -= TAIL_SOLO * (wpb - 1);
+    else p = w == 0 ? b : g.nenv - 1 - (b * (wpb - 1) + w - 1);
+  }
+  const int cnt = lane < TAIL_NKEY ? CLK(s, g, g.sub)[TAIL_NKEY - 1 - lane] : 0;
+  int incl = cnt;
+#pragma unroll
+  for (int d = 1; d < TAIL_NKEY; d <<= 1) {
+    const int v = __shfl_up_sync(B2S_FULL, incl, d);
+    if (lane >= d) incl += v;
+  }
+  const int c = __ffs(__ballot_sync(B2S_FULL, incl > p)) - 1;  // a lane below TAIL_NKEY: the counts of the group sum to nenv > rank p
+  const int rank = p - __shfl_sync(B2S_FULL, incl - cnt, c);
+  return s.tail_list[(size_t)g.env0 * TAIL_NKEY + (TAIL_NKEY - 1 - c) * g.nenv + rank];
+}
+
 // ---- tail: gather contacts, constraint rows + Jacobian, (in-kernel controller), actuation, Newton solve, Euler, observations.  One
 // environment with the layout `lid` in the warp's `area`; returns 1 (nothing of the environment's state touched) if it does not fit
-// the layout.  Compiled separately: the kernel calls it for both tiers.
-template <typename R>
+// the layout.  Compiled separately: the kernel calls it for both tiers.  SORTED (the cost order): `env` is the environment for the
+// large tier; for the small tier it is the warp's position in the launch, resolved here (tail_env_at, recorded in tail_order) so that
+// the kernel body keeps no loaded value live across the call; the cost class of the environment is written for the next substep.
+template <typename R, bool SORTED>
 DEVN int tail_env(R* area, int lane, int lid, Grp g, int env, int nsub, int phases, const R* action, unsigned long long* bar, unsigned& parity) {
   const int sub = g.sub;
+  if (SORTED && lid == LAY_TS) {
+    const int p = env;
+    env = tail_env_at<R>(g, p, lane);
+    if (lane == 0) cstate<R>(g.slot).tail_order[g.env0 + p] = env;
+  }
   Eng<R> e(area, lane, g.slot, lid);
 #ifdef B2S_INSTR
   const DState<R>& s = cstate<R>(g.slot);
@@ -427,20 +475,27 @@ DEVN int tail_env(R* area, int lane, int lid, Grp g, int env, int nsub, int phas
   int warn = TAIL_WARN(pk);
   if ((phases & PH_CTRL) && !(phases & PH_CTRL_EXT)) tail_ctrl(e, env, sub, action);
   warn |= tail_accel(e);
-  warn |= tail_newton(e, nefc, ncon);
+  int niter;
+  warn |= tail_newton(e, nefc, ncon, &niter);
+  if (SORTED && lane == 0) e.state().tail_key[env] = tail_cost_key(niter, nefc, lid == LAY_TL);
   tail_finish(e, env, sub, nsub, phases, ncon, warn, bar, parity);
 #ifdef B2S_INSTR
-  if (lane == 0 && s.cyc) s.cyc[((size_t)env * 32 + (sub & 31)) * 2 + 1] = (float)(clock64() - instr_t0);
+  if (lane == 0 && s.cyc) {
+    float* c = s.cyc + ((size_t)env * 32 + (sub & 31)) * 8;
+    c[1] = (float)(clock64() - instr_t0);
+    c[2] = (float)niter; c[3] = (float)s.solve_ls[env]; c[4] = (float)nefc; c[5] = (float)ncon;
+    c[6] = lid == LAY_TL ? 1.f : 0.f; c[7] = (float)blockIdx.x;
+  }
   if (lane == 0 && s.stats) { atomicAdd(s.stats + 32 + min(ncon, 128), 1); atomicAdd(s.stats + 176 + min(nefc, 320), 1); if (lid == LAY_TL) atomicAdd(s.stats + 19, 1); }
 #endif
   return 0;
 }
 
-// Warp per environment of the group with the small-capacity layout (`stride` words per warp); an environment that does not fit is
-// left in the block's overflow list.  After a block barrier the first `nlw` warps re-run the block's overflowed environments with the
-// full-capacity layout (`stride_l` words per warp, over the small tier's dead areas).  An overflowed environment waits for its own
-// block only, not for the whole group.
-template <typename R, int THREADS>
+// Warp per environment of the group with the small-capacity layout (`stride` words per warp), in the order of tail_env_at (SORTED)
+// or by id; an environment that does not fit is left in the block's overflow list.  After a block barrier the first `nlw` warps re-run
+// the block's overflowed environments with the full-capacity layout (`stride_l` words per warp, over the small tier's dead areas).
+// An overflowed environment waits for its own block only, not for the whole group.
+template <typename R, int THREADS, bool SORTED>
 __global__ void __launch_bounds__(THREADS, THREADS == TAIL_WIDE_THREADS ? 1 : TAIL_BLOCKS) tail_kernel(int phases, int nsub, const R* action, Grp g, int stride, int stride_l, int nlw) {
   const DState<R>& s = cstate<R>(g.slot);
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -448,14 +503,18 @@ __global__ void __launch_bounds__(THREADS, THREADS == TAIL_WIDE_THREADS ? 1 : TA
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31, wpb = blockDim.x >> 5;
   INSTR_BEGIN(s, g, 3)
   __shared__ unsigned long long mbar[32];  // one transaction barrier per warp (TMA loads of its workspace regions)
-  __shared__ int ovf[32];                  // per warp: its environment if it did not fit the small tier, else -1
-  if (blockIdx.x == 0 && threadIdx.x == 0) { int* c = CLC(s, g); c[0] = 0; c[1] = 0; c[3] = 0; }  // phase1_kernel is done with them
+  __shared__ int ovf[32];                  // per warp: its position if its environment did not fit the small tier, else -1
+  if (blockIdx.x == 0 && warp == 0) {  // phase1_kernel is done with the work-list counters; phase0_kernel(s + 1) files into the other set
+    int* c = CLC(s, g);
+    if (lane == 0) { c[0] = 0; c[1] = 0; c[3] = 0; }
+    if (lane < TAIL_NKEY) CLK(s, g, g.sub + 1)[lane] = 0;
+  }
   if (lane == 0) mbar_init(&mbar[warp]);
   __syncwarp();
   unsigned parity = 0;
-  const int env = g.env0 + blockIdx.x * wpb + warp;
+  const int p = blockIdx.x * wpb + warp;
   int o = -1;
-  if (env < g.env0 + g.nenv && tail_env<R>(smem + (size_t)warp * stride, lane, LAY_TS, g, env, nsub, phases, action, &mbar[warp], parity)) o = env;
+  if (p < g.nenv && tail_env<R, SORTED>(smem + (size_t)warp * stride, lane, LAY_TS, g, SORTED ? p : g.env0 + p, nsub, phases, action, &mbar[warp], parity)) o = p;
   if (lane == 0) ovf[warp] = o;
   // the small tier's areas are dead from here on (every fitting environment has stored its state, ws_store waited for its bulk
   // stores); order this thread's generic accesses to them before the large tier's bulk loads into the same shared memory
@@ -463,6 +522,7 @@ __global__ void __launch_bounds__(THREADS, THREADS == TAIL_WIDE_THREADS ? 1 : TA
   __syncthreads();
   if (warp < nlw)
     for (int k = warp; k < wpb; k += nlw)
-      if (ovf[k] >= 0) tail_env<R>(smem + (size_t)warp * stride_l, lane, LAY_TL, g, ovf[k], nsub, phases, action, &mbar[warp], parity);
+      if (ovf[k] >= 0)
+        tail_env<R, SORTED>(smem + (size_t)warp * stride_l, lane, LAY_TL, g, SORTED ? s.tail_order[g.env0 + ovf[k]] : g.env0 + ovf[k], nsub, phases, action, &mbar[warp], parity);
   INSTR_END(s, g, 3)
 }

@@ -496,7 +496,8 @@ template <typename R> DEVN int solve(Eng<R> e, int nefc, int ncon, int& warn) {
   int niter = 0;
 #ifdef B2S_INSTR
   int instr_ls = 0;
-#define INSTR_SOLVE_DONE { const DState<R>& st_ = e.state(); if (lane == 0 && st_.stats) { atomicAdd(st_.stats + min(niter, 15), 1); atomicAdd(st_.stats + 16, instr_ls); atomicAdd(st_.stats + 17, 1); } }
+#define INSTR_SOLVE_DONE { const DState<R>& st_ = e.state(); if (lane == 0 && st_.stats) { atomicAdd(st_.stats + min(niter, 15), 1); atomicAdd(st_.stats + 16, instr_ls); atomicAdd(st_.stats + 17, 1); } \
+                           if (lane == 0 && st_.solve_ls) st_.solve_ls[e.env] = instr_ls; }
 #else
 #define INSTR_SOLVE_DONE
 #endif

@@ -78,7 +78,8 @@ struct DState {
   R* obs;          // [n_env, obs_dim] sampled after the first substep of a control step (observables.py:230-240)
   R* wsg;          // [n_env, L.total] global workspace rows (pipeline mode)
   // pipeline-mode collision work lists (candidate pairs of ALL environments, compacted with atomics)
-  int* cl_cnt;     // per group [8]: number of analytic / convex candidates this substep, (spare), next convex work item, (spare x4)
+  int* cl_cnt;     // per group [CL_CNT_STRIDE]: number of analytic / convex candidates this substep, (spare), next convex work item,
+                   // (spare x4), then environments per tail cost class for even / odd substeps [2][TAIL_NKEY]
   int cl_maxa, cl_maxg;  // per-environment candidate capacity of the two work lists
   int* cl_listA;   // [n_env * cl_maxa] env << 12 | pair
   int* cl_listG;   // [n_env * cl_maxg]
@@ -86,6 +87,12 @@ struct DState {
   R* cl_outG;      // [n_env * cl_maxg][8]       count + (pos3 normal3 dist)
   R* gjk_cache;    // [n_env][npair][3] last separating direction of each convex pair (GJK warm start)
   int* cl_env;     // [n_env][2 + 2 * (cl_maxa + cl_maxg)] na, ng, then (pair, slot) of each candidate
+  // pipeline-mode tail order: a group's tail launch runs its environments most expensive cost class first when tail_sorted (a block
+  // shape choice, choose_blocks), else by id
+  int tail_sorted;
+  int* tail_key;  // [n_env] cost class of the environment's last tail (tail_cost_key)
+  int* tail_list;  // [n_env * TAIL_NKEY] per group (from env0 * TAIL_NKEY) and class k (at + k * nenv): the environments phase 0 filed
+  int* tail_order; // [n_env] per group: the environment the last tail launch ran at warp position p, at env0 + p
   int* obs_fresh;  // [n_env] 1 = observation cache empty (set at reset, cleared by the first sample)
   // per-environment world poses of bodies welded to the world (the reference writes sampled placements into model.body_pos /
   // body_quat per reset, e.g. the Door: door.py:417-427; model constants are shared by a batch here, so these are DATA): up to 4 bodies
@@ -112,7 +119,9 @@ struct DState {
   unsigned long long* st_end;    //                                     last %globaltimer of the launch
   int* stats;      // [512]: 0..15 Newton-iteration histogram, 16 line-search evaluations, 17 solves, 19 large-tier environments,
                    // 32..160 ncon histogram, 176..496 nefc histogram
-  float* cyc;      // [n_env][32 substeps][2] clock64 cycles of this environment's warp in P0 / the tail kernel
+  float* cyc;      // [n_env][32 substeps][8] per environment-substep: clock64 cycles of its warp in P0, in the tail kernel; then the
+                   // tail's Newton iterations, line-search evaluations, nefc, ncon, capacity tier (1 = large) and tail block index
+  int* solve_ls;   // [n_env] line-search evaluations of the environment's last Newton solve
   int* slowlog;    // [64][12] convex work items above 131 k cycles: cycles, shape types, hull sizes, EPA nV nF, GJK cycles, hit, staged, geoms
 };
 
@@ -149,6 +158,9 @@ enum { PIO_P0 = 0, PIO_TS = 1, PIO_TS_LATE = 2, PIO_TL = 3, PIO_TL_LATE = 4, B2S
 #define CL_MAXG 32  // the run-time caps DState::cl_maxa / cl_maxg are chosen per model (b2s_capi.cu)
 #define CL_RECA 58
 #define CL_ENVW(s) (2 + 2 * ((s).cl_maxa + (s).cl_maxg))
+#define TAIL_NKEY 16                          // tail cost classes (tail_cost_key, b2s_pipeline.cuh)
+#define TAIL_SOLO 2                           // tail blocks whose one expensive environment runs beside cheap ones (tail_env_at)
+#define CL_CNT_STRIDE (8 + 2 * TAIL_NKEY)     // ints per group in DState::cl_cnt
 #define B2S_MAXREG 12
 // load / store lists hold merged 16-byte aligned spans; load_words = sum of the fixed spans, load_dyn = list has the Jacobian
 struct PhaseIO { int nload, nstore, load_words, load_dyn; Region load[B2S_MAXREG], store[B2S_MAXREG]; };

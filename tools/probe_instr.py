@@ -2,9 +2,9 @@
 B2S_LIB=robosuite_b200/variants/libb2s_instr.so).  Answers, from data of the CUDA-graph replay itself:
   * how long each kernel of a group-substep runs and how long the gaps between dependent kernels are (%globaltimer stamps);
   * the Newton-iteration / ncon / nefc histograms and line-search evaluations per solve;
-  * how unevenly the environments of one block cost (clock64 per environment-substep): block time = slowest warp.  Blocks are
-    taken as 8 (phase 0) and 16 (tail) consecutive warps, the launch bounds' caps and what the Lift / Panda f32 layouts get; for
-    models whose blocks hold fewer warps the grouping is approximate.
+  * how unevenly the environments of one block cost (clock64 per environment-substep): block time = slowest warp.  Tail blocks are
+    the ones the environments were recorded running in; phase-0 blocks are taken as 8 consecutive warps, the launch bounds' cap and
+    what the Lift / Panda f32 layout gets (for models whose phase-0 blocks hold fewer warps that grouping is approximate).
 usage: python tools/probe_instr.py [task] [robot] [n_env] [controller] -> JSON on stdout"""
 import json
 import os
@@ -100,16 +100,21 @@ gn = env.model.names["geom"]
 out["slow_items"] = [dict(cycles=int(r[0]), types=(int(r[1]), int(r[2])), nvert=(int(r[3]), int(r[4])), epa_nV=int(r[5]), epa_nF=int(r[6]), gjk_cycles=int(r[7]),
                           hit=int(r[8]), staged=int(r[9]), geoms=(gn[int(r[10])], gn[int(r[11])])) for r in sl if r[0] > 0][:40]
 out["slow_items_total"] = int(st[20])
-cy = sim.cyc.cpu().numpy()[:, :25]  # [n, 25, 2]
-for k, nm, wpb in ((0, "P0", 8), (1, "tail", 16)):
+cy = sim.cyc.cpu().numpy()[:, :25]  # [n, 25, 8]: P0 cycles, tail cycles, ..., tail block index
+for k, nm in ((0, "P0"), (1, "tail")):
     c = cy[:, :, k]
-    ge = n // G
     ratios, lratios = [], []
     for g in range(G):
-        cg = c[g * ge:(g + 1) * ge]
-        nb = ge // wpb
-        blk = cg[:nb * wpb].reshape(nb, wpb, 25)
-        ratios.append(float((blk.max(1) / np.maximum(blk.mean(1), 1)).mean()))   # block time / mean warp time
+        e0, e1 = n * g // G, n * (g + 1) // G
+        cg = c[e0:e1]
+        # phase 0: environment env0 + 8 b + w runs in block b; the tail records the block each environment-substep ran in
+        bg = cy[e0:e1, :, 7].astype(np.int64) if k == 1 else np.repeat((np.arange(e1 - e0) // 8)[:, None], 25, 1)
+        for s in range(25):
+            cnt = np.bincount(bg[:, s])
+            mx = np.zeros(len(cnt))
+            np.maximum.at(mx, bg[:, s], cg[:, s])
+            ok = cnt > 0
+            ratios.append(float((mx[ok] / np.maximum(np.bincount(bg[:, s], cg[:, s])[ok] / cnt[ok], 1)).mean()))  # block time / mean warp time
         lratios.append(float((cg.max(0) / np.maximum(cg.mean(0), 1)).mean()))    # launch time / mean warp time
     out["cycles_" + nm] = {"mean": float(c.mean()), "p50": float(np.median(c)), "p90": float(np.percentile(c, 90)),
                            "p99": float(np.percentile(c, 99)), "max": float(c.max()),
