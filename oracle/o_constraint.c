@@ -52,7 +52,8 @@ void o_make_constraint(const OModel* m, OData* d) {
       d->efc_J[(size_t)r * nv + i] = 1;
       d->nf++;
     }
-  /* --- joint limits (slide / hinge); active only when violated because margin = 0 */
+  /* --- joint limits (slide / hinge): a side is active within the joint's margin (both sides when the range is narrower than
+   * twice the margin) */
   for (int j = 0; j < m->njnt; j++) {
     if (!m->jnt_limited[j]) continue;
     int t = m->jnt_type[j];

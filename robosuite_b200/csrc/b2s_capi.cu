@@ -328,6 +328,7 @@ template <typename R> static void build_model(b2s_sim* s, const Blob& b, DModel<
   m.jnt_type = up_i(s, b, "jnt_type"); m.jnt_qposadr = up_i(s, b, "jnt_qposadr"); m.jnt_dofadr = up_i(s, b, "jnt_dofadr");
   m.jnt_bodyid = up_i(s, b, "jnt_bodyid"); m.jnt_limited = up_i(s, b, "jnt_limited");
   m.jnt_pos = up_f<R>(s, b, "jnt_pos"); m.jnt_axis = up_f<R>(s, b, "jnt_axis"); m.jnt_range = up_f<R>(s, b, "jnt_range");
+  m.jnt_margin = up_f<R>(s, b, "jnt_margin");
   m.jnt_solref = up_f<R>(s, b, "jnt_solref"); m.jnt_solimp = up_f<R>(s, b, "jnt_solimp"); m.qpos0 = up_f<R>(s, b, "qpos0");
   m.dof_bodyid = up_i(s, b, "dof_bodyid"); m.dof_jntid = up_i(s, b, "dof_jntid"); m.dof_parentid = up_i(s, b, "dof_parentid");
   m.dof_kind = dev_upload(s, dkind); m.dof_cddstart = dev_upload(s, cddstart); m.fl_dof = dev_upload(s, fl_dof);

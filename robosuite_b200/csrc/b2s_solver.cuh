@@ -85,17 +85,19 @@ template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn) {
       nefc += __popc(mask);
     }
   }
-  // --- joint limits
+  // --- joint limits: candidate k is side k & 1 (lower first) of limited joint k >> 1.  A side is active within its joint's margin,
+  // so a range narrower than twice the margin has both rows.  The row's pos is dist - margin: impedance and aref take it as is.
   B2S_LOOP
-  for (int base = 0; base < m.nlim; base += 32) {
-    int k = base + lane, act = 0, j = 0, side = 0;
+  for (int base = 0; base < 2 * m.nlim; base += 32) {
+    int k = base + lane, act = 0, j = 0, upper = 0;
     R dist = 0;
-    if (k < m.nlim) {
-      j = m.lim_jnt[k];
-      R value = qpos[m.jnt_qposadr[j]];
-      R dlo = value - m.jnt_range[2 * j], dhi = m.jnt_range[2 * j + 1] - value;
-      if (dlo < 0) { act = 1; side = -1; dist = dlo; }
-      else if (dhi < 0) { act = 1; side = 1; dist = dhi; }
+    if (k < 2 * m.nlim) {
+      j = m.lim_jnt[k >> 1];
+      upper = k & 1;
+      R value = qpos[m.jnt_qposadr[j]], margin = m.jnt_margin[j];
+      dist = upper ? m.jnt_range[2 * j + 1] - value : value - m.jnt_range[2 * j];
+      act = dist < margin;
+      dist -= margin;
     }
     unsigned mask = __ballot_sync(B2S_FULL, act);
     if (act) {
@@ -103,7 +105,7 @@ template <typename R> DEVN int make_constraint(Eng<R> e, int ncon, int& warn) {
       if (r < L.me) {
         int dof = m.jnt_dofadr[j];
         B2S_LOOP
-        for (int i = 0; i < nv; i++) J[r * nv + i] = i == dof ? R(-side) : R(0);
+        for (int i = 0; i < nv; i++) J[r * nv + i] = i == dof ? R(upper ? -1 : 1) : R(0);
         eint[r] = C_LIMIT | (j << 8);
         epos[r] = dist;
         efl[r] = 0;
@@ -459,6 +461,11 @@ template <typename R> DEVN int solve(Eng<R> e, int nefc, int ncon, int& warn) {
     int t1 = m.body_treeid[m.geom_bodyid[cint[5 * c]]], t2 = m.body_treeid[m.geom_bodyid[cint[5 * c + 1]]];
     if (t1 >= 0 && t2 >= 0 && t1 != t2) cross_tree = true;
   }
+  // both limit rows of one joint (a range narrower than twice its margin) follow each other and hit one dof
+  bool two_sided = false;
+  B2S_LOOP
+  for (int r = lane + 1; r < first_contact_row; r += 32) two_sided |= (eint[r] & 255) == C_LIMIT && eint[r - 1] == eint[r];
+  two_sided = __any_sync(B2S_FULL, two_sided);
 
   // --- warm start: previous qacc unless the unconstrained acceleration is cheaper
   R cost_ws = 0, cost_sm = 0;
@@ -552,15 +559,17 @@ template <typename R> DEVN int solve(Eng<R> e, int nefc, int ncon, int& warn) {
     B2S_LOOP
     for (int k = lane; k < nv * nv; k += 32) H[k] = M[k];
     __syncwarp();
-    // a dof can carry a friction-loss row AND a joint-limit row: two passes of plain adds (rows of one kind hit distinct dofs) keep the
-    // summation order fixed - a float atomicAdd left it to the hardware, and two handles stepping side by side then drifted apart
+    // a dof can carry a friction-loss row AND the lower and upper limit rows of its joint: one pass of plain adds per kind (rows of
+    // one kind hit distinct dofs) keeps the summation order fixed - a float atomicAdd left it to the hardware, and two handles
+    // stepping side by side then drifted apart.  Pass 0: friction loss, pass 1: limits, pass 2: the upper side of a two-sided joint
     B2S_LOOP
-    for (int pass = 0; pass < 2; pass++) {
+    for (int pass = 0; pass < (two_sided ? 3 : 2); pass++) {
       B2S_LOOP
       for (int r = lane; r < first_contact_row; r += 32) {
         int ty = eint[r] & 255, id = eint[r] >> 8;
         R d = act[r];
-        if ((ty == C_FRICTION) == (pass == 0) && d != 0) {
+        int p = ty == C_FRICTION ? 0 : (two_sided && r > 0 && eint[r - 1] == eint[r] ? 2 : 1);
+        if (p == pass && d != 0) {
           int dof = ty == C_FRICTION ? id : m.jnt_dofadr[id];
           H[dof * nv + dof] += d;
         }

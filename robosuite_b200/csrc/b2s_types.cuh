@@ -38,7 +38,7 @@ struct DModel {
   const R *body_xpos0, *body_xquat0;  // world pose of bodies welded to the world (constant)
   // joints
   const int *jnt_type, *jnt_qposadr, *jnt_dofadr, *jnt_bodyid, *jnt_limited;
-  const R *jnt_pos, *jnt_axis, *jnt_range, *jnt_solref, *jnt_solimp, *qpos0;
+  const R *jnt_pos, *jnt_axis, *jnt_range, *jnt_margin, *jnt_solref, *jnt_solimp, *qpos0;
   // dofs
   const int *dof_bodyid, *dof_jntid, *dof_parentid, *dof_kind, *dof_cddstart, *fl_dof, *lim_jnt, *dof_treebase, *dof_treesize, *body_treeid;
   const unsigned long long* body_dofmask;  // bit i set: dof i is on the chain of this body
