@@ -252,6 +252,28 @@ def test_controller_config_surface():
         cc.resolve(model, bad, CtrlCfg)
 
 
+def test_switches_set_the_library_variables_and_restore_them():
+    """tests/schedules.py's switches(): the requested values inside; on exit, also through an exception, an absent variable is absent
+    again and a pre-existing value (here a user's B2S_GROUPS=4, itself set by an outer switches()) is back"""
+    from tests.schedules import switches
+
+    def now():
+        return [os.environ.get(k) for k in ("B2S_NO_GJK_CACHE", "B2S_CTRL_SPLIT", "B2S_GROUPS")]
+
+    outside = now()
+    with switches(groups=4):
+        assert now() == [None, None, "4"]
+        with switches(gjk_cache=False, ctrl_split=False, groups=1):
+            assert now() == ["1", "0", "1"]
+        assert now() == [None, None, "4"]
+        with pytest.raises(RuntimeError):
+            with switches(gjk_cache=False, ctrl_split=False):
+                assert now() == ["1", "0", None]
+                raise RuntimeError("inside")
+        assert now() == [None, None, "4"]
+    assert now() == outside
+
+
 # ------------------------------------------------------------------------------------------------ multi-process
 _WORKER = r"""
 import os, sys, torch, numpy as np

@@ -10,6 +10,7 @@ import os
 import numpy as np
 import pytest
 
+from tests.schedules import switches
 from tests.util import ROOT, lift_states, load
 
 pytestmark = pytest.mark.gpu
@@ -177,8 +178,7 @@ def test_two_handles_step_concurrently_and_bit_exactly():
             assert L.b2s_forward(h) == 0 and L.b2s_ctrl_reset(h, None) == 0
         return h
 
-    os.environ["B2S_NO_GJK_CACHE"] = "1"
-    try:
+    with switches(gjk_cache=False):
         sa, sb = torch.cuda.Stream(), torch.cuda.Stream()
         ha, hb = setup(sa), setup(sb)
         torch.cuda.synchronize()
@@ -202,8 +202,6 @@ def test_two_handles_step_concurrently_and_bit_exactly():
         torch.cuda.synchronize()
         qc, vc = _arr(L, hc, "qpos").clone(), _arr(L, hc, "qvel").clone()
         L.b2s_destroy(hc)
-    finally:
-        os.environ.pop("B2S_NO_GJK_CACHE", None)
     assert torch.isfinite(qa).all()
 
     def where(x, y):

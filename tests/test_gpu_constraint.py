@@ -28,6 +28,7 @@ import numpy as np
 import pytest
 
 from tests import constraint_ref as cr
+from tests.schedules import switches
 from tests.test_cpu_constraint import CASE_NAMES, case_named, oracle_forward, rel_err
 
 pytestmark = pytest.mark.gpu
@@ -261,34 +262,31 @@ _SCHEDULE_CASES = ["joints", "sphere_condim1", "capsule_condim6_impratio100", "t
 
 
 def _steps(case, mode, prec, tier_small, n=20):
-    import os
-
     import torch
 
     from robosuite_b200.engine import BatchedSim
 
-    os.environ["B2S_NO_GJK_CACHE"] = "1"  # the fused kernel has no GJK warm start
     maxcon, me = CAPACITY.get(case.name, (None, None))
-    sim = BatchedSim(case.model, case.n, precision=prec, maxcon=maxcon, maxefc=me, tier_small=tier_small)
-    try:
-        dt = sim.dtype
-        t = lambda a: torch.as_tensor(np.asarray(a), dtype=dt)
-        if case.specs:
-            for f in ("geom_friction", "geom_solref", "geom_solimp"):
-                for g in case.specs[0][f]:
-                    sim.model_override(f, g).copy_(t([s[f][g] for s in case.specs]))
-            sim.model_override("dof_frictionloss").copy_(t([s["dof_frictionloss"] for s in case.specs]))
-            sim.set_const()
-        sim.set_mode(mode)
-        sim.qpos.copy_(t(case.Q))
-        sim.qvel.copy_(t(case.V))
-        sim.step(n)
-        torch.cuda.synchronize()
-        assert int(sim.warn.abs().max()) == 0
-        return sim.qpos.cpu().numpy().copy(), sim.qvel.cpu().numpy().copy()
-    finally:
-        sim.close()
-        os.environ.pop("B2S_NO_GJK_CACHE", None)
+    with switches(gjk_cache=False):  # the fused kernel has no GJK warm start
+        sim = BatchedSim(case.model, case.n, precision=prec, maxcon=maxcon, maxefc=me, tier_small=tier_small)
+        try:
+            dt = sim.dtype
+            t = lambda a: torch.as_tensor(np.asarray(a), dtype=dt)
+            if case.specs:
+                for f in ("geom_friction", "geom_solref", "geom_solimp"):
+                    for g in case.specs[0][f]:
+                        sim.model_override(f, g).copy_(t([s[f][g] for s in case.specs]))
+                sim.model_override("dof_frictionloss").copy_(t([s["dof_frictionloss"] for s in case.specs]))
+                sim.set_const()
+            sim.set_mode(mode)
+            sim.qpos.copy_(t(case.Q))
+            sim.qvel.copy_(t(case.V))
+            sim.step(n)
+            torch.cuda.synchronize()
+            assert int(sim.warn.abs().max()) == 0
+            return sim.qpos.cpu().numpy().copy(), sim.qvel.cpu().numpy().copy()
+        finally:
+            sim.close()
 
 
 @pytest.mark.parametrize("prec", ["f64", "f32"])

@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from tests.dynamics_override_host import dynamics_override_model, perturb_values
+from tests.schedules import make_env, random_actions, run
 from tests.util import ROOT, load
 
 torch = pytest.importorskip("torch")
@@ -158,28 +159,6 @@ def test_per_environment_dynamics_follow_their_own_oracles(task, prec):
     sim.close()
 
 
-def _lift_env(n, mode, seed=9, **kw):
-    import robosuite_b200 as suite
-
-    env = suite.make("Lift", robots="Panda", num_envs=n, seed=seed, kernel_mode="fused" if mode == 0 else "pipeline", **kw)
-    if mode == 2:
-        env.sim.set_mode(2)
-    return env
-
-
-def _acts(env, k, seed=0):
-    gen = torch.Generator(device=env.device)
-    gen.manual_seed(seed)
-    return torch.rand((k, env.num_envs, env.action_dim), generator=gen, device=env.device, dtype=env.dtype) * 2 - 1
-
-
-def _run(stepper, env, acts):
-    for a in acts:
-        stepper.step(a)
-    torch.cuda.synchronize()
-    return env.sim.qpos.clone(), env.sim.qvel.clone(), env.sim.obs.clone()
-
-
 @pytest.mark.parametrize("tier", [None, (4, 16)])
 def test_schedules_agree_with_randomized_dynamics(tier):
     """fused, pipeline and unit queue are bit-identical with every field randomised per environment; (4, 16) forces environments
@@ -189,15 +168,15 @@ def test_schedules_agree_with_randomized_dynamics(tier):
     n = 64
     res = []
     for mode in (0, 1, 2):
-        env = _lift_env(n, mode, **({"tier_small": tier} if tier else {}))
+        env = make_env("Lift", n, mode, 9, **({"tier_small": tier} if tier else {}))
         w = BatchedDomainRandomizationWrapper(env, seed=5, randomize_every_n_steps=3)
         w.reset()
-        acts = _acts(env, 8)
-        r = _run(w, env, acts)
+        acts = random_actions(env, 8)
+        r = run(w, acts)
         mask = torch.zeros(n, dtype=torch.bool, device=env.device)
         mask[::5] = True
         w.reset(mask=mask)
-        res.append(r + _run(w, env, acts[:4]) + (env.sim.model_override("dof_frictionloss").clone(),))
+        res.append(r + run(w, acts[:4]) + (env.sim.model_override("dof_frictionloss").clone(),))
         env.close()
     for r in res[1:]:
         for a, b in zip(res[0], r):
@@ -207,15 +186,15 @@ def test_schedules_agree_with_randomized_dynamics(tier):
 @pytest.mark.parametrize("mode", [0, 1, 2])
 def test_declaring_dynamics_overrides_changes_no_bit(mode):
     n = 32
-    a, b = _lift_env(n, mode), _lift_env(n, mode)
+    a, b = make_env("Lift", n, mode, 9), make_env("Lift", n, mode, 9)
     m = a.model
     for f in DOF:
         b.sim.model_override(f)
     for g in (m.names["geom"].index("cube_g0"), m.names["geom"].index("table_collision")):
         b.sim.model_override("geom_solref", g)
         b.sim.model_override("geom_solimp", g)
-    acts = _acts(a, 10)
-    ra, rb = _run(a, a, acts), _run(b, b, acts)
+    acts = random_actions(a, 10)
+    ra, rb = run(a, acts), run(b, acts)
     for x, y in zip(ra, rb):
         assert torch.equal(x, y)
     a.close()
@@ -226,11 +205,11 @@ def test_masked_perturbation_and_reset_leave_the_others_alone():
     from robosuite_b200.wrappers import BatchedDomainRandomizationWrapper
 
     n = 64
-    a, b = _lift_env(n, 1, seed=5), _lift_env(n, 1, seed=5)
+    a, b = make_env("Lift", n, 1, 5), make_env("Lift", n, 1, 5)
     wa = BatchedDomainRandomizationWrapper(a, seed=1, randomize_every_n_steps=0)
     wb = BatchedDomainRandomizationWrapper(b, seed=1, randomize_every_n_steps=0)
-    acts = _acts(a, 10)
-    _run(wa, a, acts[:5]); _run(wb, b, acts[:5])
+    acts = random_actions(a, 10)
+    run(wa, acts[:5]); run(wb, acts[:5])
     mask = torch.zeros(n, dtype=torch.bool, device=a.device)
     mask[3::7] = True
     damp = a.sim.model_override("dof_damping")
@@ -241,7 +220,7 @@ def test_masked_perturbation_and_reset_leave_the_others_alone():
     assert torch.equal(damp[~mask], d0[~mask]) and not torch.equal(damp[mask], d0[mask])
     for k, v in before.items():
         assert torch.equal(getattr(a.sim, k)[~mask], v[~mask]), k
-    ra, rb = _run(wa, a, acts[5:]), _run(wb, b, acts[5:])
+    ra, rb = run(wa, acts[5:]), run(wb, acts[5:])
     for x, y in zip(ra, rb):
         assert torch.equal(x[~mask], y[~mask])
     assert int(a.sim.warn.abs().max()) == 0

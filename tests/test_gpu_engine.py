@@ -2,6 +2,7 @@
 import numpy as np
 import pytest
 
+from tests.schedules import assert_same, lift_rollout
 from tests.util import lift_states, load
 
 pytestmark = pytest.mark.gpu
@@ -220,63 +221,18 @@ def test_env_step_f32_100_control_steps():
     assert eq < 5e-3 and ev < 1e-2
 
 
-def _scripted_rollout(mode, steps, no_cache, ctrl_split=False, tier_small=None, n=16, groups=None):
-    """groups: B2S_GROUPS for the pipeline (None: the library's default)"""
-    import os
-    import torch
-    from robosuite_b200 import controller_config as cc
-    from robosuite_b200.engine import BatchedSim, CtrlCfg
-
-    model = load("Lift_Panda")
-    q, v = lift_states(model, n, seed=21)
-    rng = np.random.default_rng(3)
-    actions = rng.uniform(-1, 1, size=(steps, n, 7))
-    actions[:, :, 6] = 1.0  # keep closing the gripper: sliding / sticking finger contacts exercise the friction cones
-    actions[8:, : (n + 1) // 2, :3] = [0.0, 0.0, -1.0]  # half of the arms (at least one) push down onto the table / cube
-    if no_cache:
-        os.environ["B2S_NO_GJK_CACHE"] = "1"
-    else:
-        os.environ.pop("B2S_NO_GJK_CACHE", None)
-    # the thread-per-environment controller kernel orders its fp64 sums differently from the in-kernel controller (last-bit
-    # differences in the torques): bit-exactness of the two SCHEDULES is tested with the controller inside the tail kernel
-    os.environ["B2S_CTRL_SPLIT"] = "1" if ctrl_split else "0"
-    sim = BatchedSim(model, n, precision="f32", tier_small=tier_small)
-    sim.ctrl_config(cc.resolve(model, cc.default_composite_config(), CtrlCfg))
-    sim.set_export(False)
-    if groups is not None:
-        os.environ["B2S_GROUPS"] = str(groups)
-    sim.set_mode(mode)  # reads B2S_GROUPS
-    if groups is not None:
-        os.environ.pop("B2S_GROUPS")
-    sim.qpos.copy_(torch.as_tensor(q, dtype=torch.float32))
-    sim.forward()
-    sim.ctrl_reset()
-    for t in range(steps):
-        sim.env_step(torch.as_tensor(actions[t], dtype=torch.float32, device=sim.torch_device).contiguous(), 25)
-    torch.cuda.synchronize()
-    assert int(sim.warn.abs().max()) == 0
-    out = (sim.qpos.cpu().numpy().copy(), sim.qvel.cpu().numpy().copy())
-    sim.close()
-    os.environ.pop("B2S_NO_GJK_CACHE", None)
-    os.environ.pop("B2S_CTRL_SPLIT", None)
-    return out
-
-
 def test_pipeline_mode_matches_fused_bit_exact():
     """phase kernels + collision work lists run the same device functions as the fused kernel: without the GJK warm
     start the two schedules are bit-identical over a contact-rich 1000-substep rollout"""
-    a = _scripted_rollout(0, 40, True)
-    b = _scripted_rollout(1, 40, True)
-    assert np.isfinite(b[0]).all()
-    assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
+    assert_same(lift_rollout(0, 40, clean=True), lift_rollout(1, 40, clean=True))
 
 
 def test_pipeline_gjk_warm_start_changes_paths_not_results():
     """the remembered separating direction only shortens GJK: over 300 substeps results stay within fp32 noise of the
     fused kernel (beyond that, arms pressing on the table are chaotic and any rounding difference is amplified)"""
-    a = _scripted_rollout(0, 12, False)
-    b = _scripted_rollout(1, 12, False)
-    dq = np.abs(a[0] - b[0]).max()
+    a = lift_rollout(0, 12, gjk_cache=True, clean=True)
+    b = lift_rollout(1, 12, gjk_cache=True, clean=True)
+    dq = np.abs(a.qpos - b.qpos).max()
     print("pipeline(warm start) vs fused after 300 substeps: max |dqpos| %.3g" % dq)
     assert dq < 1e-4
 
@@ -286,19 +242,13 @@ def test_unit_queue_mode_matches_pipeline_bit_exact(no_cache):
     """mode 2 (one persistent kernel per control step, environment-substep units on a ticket ring, b2s_unit.cuh) runs the same
     device functions on the same per-environment data as the phase pipeline: bit-identical over a contact-rich 1000-substep
     rollout, with and without the GJK warm start (the cache is per environment and pair: scheduling cannot change it)"""
-    a = _scripted_rollout(1, 40, no_cache)
-    b = _scripted_rollout(2, 40, no_cache)
-    assert np.isfinite(b[0]).all()
-    assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
+    assert_same(lift_rollout(1, 40, gjk_cache=not no_cache, clean=True), lift_rollout(2, 40, gjk_cache=not no_cache, clean=True))
 
 
 @pytest.mark.parametrize("tier", [(4, 24), (12, 44)])
 def test_unit_queue_mode_tiers_are_exact(tier):
     """small-tier units + large-role warps (overflow ring) vs every unit at full capacity: bit-identical"""
-    a = _scripted_rollout(2, 24, True)
-    b = _scripted_rollout(2, 24, True, tier_small=tier)
-    assert np.isfinite(b[0]).all()
-    assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
+    assert_same(lift_rollout(2, 24, clean=True), lift_rollout(2, 24, tier_small=tier, clean=True))
 
 
 @pytest.mark.parametrize("tier", [(4, 24), (8, 32)])
@@ -306,21 +256,18 @@ def test_small_tail_tier_is_exact(tier):
     """the tail kernel's small capacity tier + large-tier re-run of the environments that do not fit must be BIT-IDENTICAL to running
     every environment with the full capacities: the arithmetic is the same, only the shared-memory layout differs.  (4, 24) is
     small enough that most environments of this contact-rich rollout overflow; (8, 32) is Lift's production setting."""
-    a = _scripted_rollout(1, 24, True, ctrl_split=True)
-    b = _scripted_rollout(1, 24, True, ctrl_split=True, tier_small=tier)
-    assert np.isfinite(b[0]).all()
-    assert np.array_equal(a[0], b[0]) and np.array_equal(a[1], b[1])
+    assert_same(lift_rollout(1, 24, ctrl_split=True, clean=True), lift_rollout(1, 24, ctrl_split=True, tier_small=tier, clean=True))
 
 
 def test_split_controller_kernel_matches_in_kernel_controller():
     """the OSC controller as its own thread-per-environment kernel (ctrl_osc_kernel, default in pipeline mode) vs the same
     controller evaluated inside the tail kernel: same inputs, fp64 algebra in both, different summation order -> torques agree to
     fp32 rounding; over 100 substeps of free-space motion the states stay within 1e-6"""
-    a = _scripted_rollout(1, 4, True, ctrl_split=False)
-    b = _scripted_rollout(1, 4, True, ctrl_split=True)
-    dq = np.abs(a[0] - b[0]).max()
+    a = lift_rollout(1, 4, clean=True)
+    b = lift_rollout(1, 4, ctrl_split=True, clean=True)
+    dq = np.abs(a.qpos - b.qpos).max()
     print("split controller kernel vs in-kernel controller after 100 substeps: max |dqpos| %.3g" % dq)
-    assert np.isfinite(b[0]).all() and dq < 1e-5
+    assert np.isfinite(b.qpos).all() and dq < 1e-5
 
 
 def _task_states(name, n=2):

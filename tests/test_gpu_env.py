@@ -4,6 +4,7 @@ import pytest
 
 import os
 
+from tests.schedules import make_env
 from tests.util import ROOT, load
 
 pytestmark = pytest.mark.gpu
@@ -318,7 +319,6 @@ def test_unit_queue_mode_matches_pipeline_on_task_envs(task, robot, ctrl):
     controller kernel of the pipeline orders its fp64 sums differently)"""
     import torch
 
-    import robosuite_b200 as suite
     from robosuite_b200 import controller_config as cc
 
     n, steps = 24, 5
@@ -326,22 +326,17 @@ def test_unit_queue_mode_matches_pipeline_on_task_envs(task, robot, ctrl):
     if ctrl != "OSC_POSE":
         kw["controller_configs"] = cc.refactor_composite_controller_config(cc.load_part_controller_config(ctrl), robot, ["right"])
     out = []
-    os.environ["B2S_CTRL_SPLIT"] = "0"
-    try:
-        for mode in (1, 2):
-            env = suite.make(task, robots=robot, num_envs=n, seed=5, horizon=10 ** 6, **kw)
-            env.sim.set_mode(mode)
-            gen = torch.Generator(device=env.device)
-            gen.manual_seed(9)
-            for t in range(steps):
-                act = torch.rand((n, env.action_dim), generator=gen, device=env.device, dtype=env.dtype) * 2 - 1
-                act[: n // 2, 2] = -1.0  # half of the arms push down: contacts, EPA, large-tier environments
-                env.step(act)
-            torch.cuda.synchronize()
-            assert int(env.sim.warn.abs().max()) == 0
-            out.append((env.sim.qpos.clone(), env.sim.qvel.clone(), env.flat_obs().clone()))
-            env.close()
-    finally:
-        os.environ.pop("B2S_CTRL_SPLIT", None)
+    for mode in (1, 2):
+        env = make_env(task, n, mode, 5, ctrl_split=False, robots=robot, horizon=10 ** 6, **kw)
+        gen = torch.Generator(device=env.device)
+        gen.manual_seed(9)
+        for t in range(steps):
+            act = torch.rand((n, env.action_dim), generator=gen, device=env.device, dtype=env.dtype) * 2 - 1
+            act[: n // 2, 2] = -1.0  # half of the arms push down: contacts, EPA, large-tier environments
+            env.step(act)
+        torch.cuda.synchronize()
+        assert int(env.sim.warn.abs().max()) == 0
+        out.append((env.sim.qpos.clone(), env.sim.qvel.clone(), env.flat_obs().clone()))
+        env.close()
     for a, b in zip(out[0], out[1]):
         assert torch.isfinite(b).all() and torch.equal(a, b)

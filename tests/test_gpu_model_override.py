@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from tests.model_override_host import override_model
+from tests.schedules import make_env, random_actions, run
 from tests.util import ROOT, lift_states, load
 
 torch = pytest.importorskip("torch")
@@ -15,6 +16,7 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 PACKAGED = sorted(glob.glob(os.path.join(ROOT, "robosuite_b200", "assets", "models", "*.npz")))
+QPOS_OBS = ("qpos", "obs")  # what the schedule and masking comparisons here hold bit-identical
 
 
 def _free_bodies(m):
@@ -199,28 +201,6 @@ def test_enlarged_cube_rests_on_the_table(prec):
     sim.close()
 
 
-def _lift_env(n, mode, seed=9, **kw):
-    import robosuite_b200 as suite
-
-    env = suite.make("Lift", robots="Panda", num_envs=n, seed=seed, kernel_mode="fused" if mode == 0 else "pipeline", **kw)
-    if mode == 2:
-        env.sim.set_mode(2)
-    return env
-
-
-def _run(env, acts):
-    for a in acts:
-        env.step(a)
-    torch.cuda.synchronize()
-    return env.sim.qpos.clone(), env.sim.obs.clone()
-
-
-def _acts(env, k, seed=0):
-    gen = torch.Generator(device=env.device)
-    gen.manual_seed(seed)
-    return torch.rand((k, env.num_envs, env.action_dim), generator=gen, device=env.device, dtype=env.dtype) * 2 - 1
-
-
 @pytest.mark.parametrize("tier", [None, (4, 16)])
 def test_schedules_agree_with_overrides(tier):
     """fused, pipeline and unit queue are bit-identical with per-environment cubes; (4, 16) forces environments into the large tier"""
@@ -228,13 +208,13 @@ def test_schedules_agree_with_overrides(tier):
     res = []
     for mode in (0, 1, 2):
         kw = {"tier_small": tier} if tier else {}
-        env = _lift_env(n, mode, per_env_cube_size=True, hard_reset=True, **kw)
-        acts = _acts(env, 8)
-        res.append(_run(env, acts))
+        env = make_env("Lift", n, mode, 9, per_env_cube_size=True, hard_reset=True, **kw)
+        acts = random_actions(env, 8)
+        res.append(run(env, acts, QPOS_OBS))
         mask = torch.zeros(n, dtype=torch.bool, device=env.device)
         mask[::5] = True
         env.reset(mask=mask)  # new cubes for the masked environments
-        res[-1] = res[-1] + _run(env, acts[:4])
+        res[-1] = res[-1] + run(env, acts[:4], QPOS_OBS)
         env.close()
     for r in res[1:]:
         for a, b in zip(res[0], r):
@@ -244,7 +224,7 @@ def test_schedules_agree_with_overrides(tier):
 @pytest.mark.parametrize("mode", [0, 1, 2])
 def test_declaring_overrides_changes_no_bit(mode):
     n = 32
-    a, b = _lift_env(n, mode), _lift_env(n, mode)
+    a, b = make_env("Lift", n, mode, 9), make_env("Lift", n, mode, 9)
     m = a.model
     g, body = _cube(m)
     for gg in (g, m.names["geom"].index("table_collision")):
@@ -252,8 +232,8 @@ def test_declaring_overrides_changes_no_bit(mode):
         b.sim.model_override("geom_friction", gg)
     b.sim.model_override("body_mass", body)
     b.sim.model_override("body_inertia", body)
-    acts = _acts(a, 10)
-    ra, rb = _run(a, acts), _run(b, acts)
+    acts = random_actions(a, 10)
+    ra, rb = run(a, acts, QPOS_OBS), run(b, acts, QPOS_OBS)
     for x, y in zip(ra, rb):
         assert torch.equal(x, y)
     a.close()
@@ -262,10 +242,10 @@ def test_declaring_overrides_changes_no_bit(mode):
 
 def test_masked_reset_with_new_cubes_leaves_the_others_alone():
     n = 64
-    a = _lift_env(n, 1, seed=5, per_env_cube_size=True, hard_reset=True)
-    b = _lift_env(n, 1, seed=5, per_env_cube_size=True, hard_reset=True)
-    acts = _acts(a, 10)
-    _run(a, acts[:5]); _run(b, acts[:5])
+    a = make_env("Lift", n, 1, 5, per_env_cube_size=True, hard_reset=True)
+    b = make_env("Lift", n, 1, 5, per_env_cube_size=True, hard_reset=True)
+    acts = random_actions(a, 10)
+    run(a, acts[:5]); run(b, acts[:5])
     mask = torch.zeros(n, dtype=torch.bool, device=a.device)
     mask[3::7] = True
     size = a._cube_ov[0]
@@ -275,7 +255,7 @@ def test_masked_reset_with_new_cubes_leaves_the_others_alone():
     assert torch.equal(size[~mask], s0[~mask]) and not torch.equal(size[mask], s0[mask])
     for k, v in before.items():
         assert torch.equal(getattr(a.sim, k)[~mask], v[~mask]), k
-    ra, rb = _run(a, acts[5:]), _run(b, acts[5:])
+    ra, rb = run(a, acts[5:], QPOS_OBS), run(b, acts[5:], QPOS_OBS)
     for x, y in zip(ra, rb):
         assert torch.equal(x[~mask], y[~mask])
     assert int(a.sim.warn.abs().max()) == 0
@@ -283,7 +263,7 @@ def test_masked_reset_with_new_cubes_leaves_the_others_alone():
 
 def test_lift_per_env_cube_size():
     n = 64
-    env = _lift_env(n, 1, seed=2, per_env_cube_size=True, hard_reset=True)
+    env = make_env("Lift", n, 1, 2, per_env_cube_size=True, hard_reset=True)
     m = env.model
     g, b = _cube(m)
     size, mass, inertia = (t.double().cpu().numpy() for t in env._cube_ov)
@@ -305,7 +285,7 @@ def test_lift_per_env_cube_size():
     assert torch.equal(s1[~mask], s0[~mask]) and bool((s1[mask] != s0[mask]).all())
     assert int(env.sim.warn.abs().max()) == 0
     # without hard_reset the cubes are drawn once
-    env2 = _lift_env(8, 1, seed=2, per_env_cube_size=True)
+    env2 = make_env("Lift", 8, 1, 2, per_env_cube_size=True)
     s0 = env2._cube_ov[0].clone()
     env2.reset()
     assert torch.equal(env2._cube_ov[0], s0)

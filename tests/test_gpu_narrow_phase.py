@@ -24,12 +24,11 @@ order, dist, pos and frame.
   bit-identical qpos and qvel.  The pipeline's and the unit queue's thread-per-pair analytic role runs sphere, capsule and cylinder
   pairs here, which no packaged model puts in contact.
 """
-import os
-
 import numpy as np
 import pytest
 
 from tests import narrow_phase_ref as npr
+from tests.schedules import switches
 from tests.test_cpu_narrow_phase import CURVED, scene, tolerances
 
 pytestmark = pytest.mark.gpu
@@ -224,9 +223,7 @@ def _schedule_run(model, q, mode, steps=2):
     from robosuite_b200 import controller_config as cc
     from robosuite_b200.engine import BatchedSim, CtrlCfg
 
-    os.environ["B2S_NO_GJK_CACHE"] = "1"
-    os.environ["B2S_CTRL_SPLIT"] = "0"
-    try:
+    with switches(gjk_cache=False, ctrl_split=False):
         sim = BatchedSim(model, len(q), precision="f32", maxcon=64, maxefc=256)  # 21 resting contacts, ~20 analytic candidates
         cfg = {"type": "BASIC", "body_parts": {"arms": {"right": cc.load_part_controller_config("JOINT_TORQUE")}}}
         sim.ctrl_config(cc.resolve(model, cfg, CtrlCfg))
@@ -243,9 +240,6 @@ def _schedule_run(model, q, mode, steps=2):
         out = sim.qpos.cpu().numpy().copy(), sim.qvel.cpu().numpy().copy()
         sim.close()
         return out
-    finally:
-        os.environ.pop("B2S_NO_GJK_CACHE", None)
-        os.environ.pop("B2S_CTRL_SPLIT", None)
 
 
 def test_schedules_bit_exact_on_primitive_contacts():

@@ -1,35 +1,13 @@
 """Whole-environment snapshots (b2s_snapshot / b2s_restore, BatchedSim.snapshot / restore / clone_envs, the environment layer's
 get_env_state / set_env_state / clone_envs): a restored environment continues bit-identically to its source under the same actions,
-whatever the batch around it.  The rollouts are contact-rich scripted Lift rollouts in the style of test_gpu_engine._scripted_rollout
-(random arm actions, gripper closing, half of the arms pushing down onto the table / cube), fp32 with the GJK warm start on unless noted."""
-import os
-
+whatever the batch around it.  The rollouts are contact-rich scripted Lift rollouts (tests/schedules.py, lift_actions: random arm
+actions, gripper closing, half of the arms pushing down onto the table / cube), fp32 with the GJK warm start on unless noted."""
 import numpy as np
 import pytest
 
+from tests.schedules import lift_actions, make_env
+
 pytestmark = pytest.mark.gpu
-
-
-def _actions(steps, n, dim=7, seed=3):
-    rng = np.random.default_rng(seed)
-    a = rng.uniform(-1, 1, size=(steps, n, dim))
-    a[:, :, dim - 1] = 1.0
-    a[8:, : (n + 1) // 2, :3] = [0.0, 0.0, -1.0]
-    return a
-
-
-def _make(task="Lift", n=16, mode=1, precision="f32", groups=None, **kw):
-    import robosuite_b200 as suite
-
-    os.environ.pop("B2S_NO_GJK_CACHE", None)
-    if groups is not None:
-        os.environ["B2S_GROUPS"] = str(groups)
-    try:
-        env = suite.make(task, robots="Panda", num_envs=n, seed=11, horizon=10 ** 6, precision=precision, **kw)
-        env.sim.set_mode(mode)
-    finally:
-        os.environ.pop("B2S_GROUPS", None)
-    return env
 
 
 def _run(env, acts):
@@ -58,7 +36,7 @@ def _differing(env, a, b):
 
 
 def _warm(env, steps=10, seed=5):
-    _run(env, _actions(steps, env.num_envs, env.action_dim, seed=seed))
+    _run(env, lift_actions(steps, env.num_envs, seed=seed, dim=env.action_dim))
 
 
 # the task draws the cube's mass and moments itself (per_env_cube_size); the wrapper randomises everything else
@@ -73,9 +51,9 @@ LIVE = ("qpos", "qvel", "qacc", "qacc_warmstart", "obs", "task_out", "ctrl", "ct
 def test_round_trip_bit_exact(mode, precision):
     """snapshot, 20 control steps, restore, the same 20 steps again: every state array, the observation and task rows, the controller
     state, the warn bits and the whole snapshot row (GJK cache included) are bit-identical to the first run"""
-    env = _make(mode=mode, precision=precision)
+    env = make_env("Lift", 16, mode, 11, horizon=10 ** 6, precision=precision)
     _warm(env)
-    acts = _actions(20, env.num_envs)
+    acts = lift_actions(20, env.num_envs)
     snap = env.sim.snapshot()
     _run(env, acts)
     first = {k: env.sim.array(k).cpu().numpy().copy() for k in LIVE}
@@ -94,7 +72,7 @@ def _clone_checks(env, steps=20):
     """from one saved batch state S: a plain run (per-environment actions), then runs from S with clones; every cloned environment
     ends with exactly its source's row of the plain run"""
     n = env.num_envs
-    acts = _actions(steps, n, env.action_dim)
+    acts = lift_actions(steps, n, dim=env.action_dim)
     S = env.sim.snapshot()
     _run(env, acts)
     base = _rows(env)
@@ -116,7 +94,7 @@ def _clone_checks(env, steps=20):
 def test_clone_bit_exact():
     """env 3 cloned into all 16 environments stays identical to itself and to env 3's own run; a reversed permutation gives the
     reversed trajectories; environments with src = -1 are bit-identical to a run without any restore"""
-    env = _make()
+    env = make_env("Lift", 16, 1, 11, horizon=10 ** 6)
     _warm(env)
     _clone_checks(env)
     env.close()
@@ -128,12 +106,12 @@ def test_cross_handle_bit_exact(mode):
     with 8 groups and no small tail tier, continues bit-identically for 40 control steps"""
     import torch
 
-    src = _make(n=16, mode=mode)
+    src = make_env("Lift", 16, mode, 11, horizon=10 ** 6)
     _warm(src)
     snap = src.sim.snapshot([5])
-    acts = _actions(40, 16)
-    one = _make(n=1, mode=mode)
-    many = _make(n=13, mode=mode, groups=8, tier_small=(48, 128))
+    acts = lift_actions(40, 16)
+    one = make_env("Lift", 1, mode, 11, horizon=10 ** 6)
+    many = make_env("Lift", 13, mode, 11, groups=8, horizon=10 ** 6, tier_small=(48, 128))
     one.sim.restore(snap, torch.zeros(1, dtype=torch.int32, device=one.device))
     many.sim.restore(snap, np.zeros(13, dtype=np.int32))
     for t in range(40):
@@ -154,11 +132,9 @@ def test_overrides_are_carried():
     the dof vectors and the derived constants, and continue bit-identically"""
     import torch
 
-    from robosuite_b200.envs.lift import BatchedLift
     from robosuite_b200.wrappers import BatchedDomainRandomizationWrapper
 
-    os.environ.pop("B2S_NO_GJK_CACHE", None)
-    w = BatchedDomainRandomizationWrapper(BatchedLift(robots="Panda", num_envs=16, seed=4, horizon=10 ** 6, per_env_cube_size=True),
+    w = BatchedDomainRandomizationWrapper(make_env("Lift", 16, 1, 4, horizon=10 ** 6, per_env_cube_size=True),
                                           seed=2, randomize_every_n_steps=0, dynamics_randomization_args=_TASK_DRAWS_CUBE)
     w.reset()
     env = w.env
@@ -188,7 +164,7 @@ def test_overrides_are_carried():
 def test_door_pose_overrides_are_carried():
     import torch
 
-    env = _make("Door", n=8)
+    env = make_env("Door", 8, 1, 11, horizon=10 ** 6)
     _warm(env)
     names = [n for n, *_ in env.sim.snapshot_layout()[2]]
     assert any(n.startswith("body_xpos_ov:") for n in names) and any(n.startswith("body_xquat_ov:") for n in names)
@@ -205,10 +181,10 @@ def test_pick_place_env_state_clone():
     """PickPlace: clones reproduce their source's rewards, `done`, episode clock and objects_in_bins step by step"""
     import torch
 
-    env = _make("PickPlace", n=8, reward_shaping=True)
+    env = make_env("PickPlace", 8, 1, 11, horizon=10 ** 6, reward_shaping=True)
     env.horizon = 22  # the 10 warm-up steps and 12 more reach it
     _warm(env)
-    acts = _actions(12, 8)
+    acts = lift_actions(12, 8)
     st = env.get_env_state()
     ref = _run(env, acts)
     ref_bins = env.objects_in_bins.clone()
@@ -231,7 +207,7 @@ def test_gym_wrapper_resets_clones_on_source_schedule(device_src):
 
     from robosuite_b200.wrappers import BatchedGymWrapper
 
-    env = _make(n=8)
+    env = make_env("Lift", 8, 1, 11, horizon=10 ** 6)
     env.horizon = 10
     g = BatchedGymWrapper(env)
     g.reset()
@@ -257,9 +233,9 @@ def test_signature_mismatch_raises():
     from robosuite_b200.envs.lift import BatchedLift
     from tests.util import load
 
-    a = _make(n=4)
+    a = make_env("Lift", 4, 1, 11, horizon=10 ** 6)
     snap = a.sim.snapshot()
-    for other in (_make("Stack", n=4), _make(n=4, precision="f64"),
+    for other in (make_env("Stack", 4, 1, 11, horizon=10 ** 6), make_env("Lift", 4, 1, 11, horizon=10 ** 6, precision="f64"),
                   BatchedLift(robots="Panda", num_envs=4, seed=1, per_env_cube_size=True)):
         with pytest.raises(ValueError, match="signature"):
             other.sim.restore(snap)
@@ -280,7 +256,7 @@ def test_bad_indices():
 
     from robosuite_b200.engine import B2SError
 
-    env = _make(n=8)
+    env = make_env("Lift", 8, 1, 11, horizon=10 ** 6)
     _warm(env)
     with pytest.raises(B2SError):
         env.sim.snapshot([0, 8])
@@ -311,7 +287,7 @@ def test_field_decode_and_layout():
     w = BatchedDomainRandomizationWrapper(BatchedLift(robots="Panda", num_envs=6, seed=3, per_env_cube_size=True), seed=1,
                                           randomize_every_n_steps=2, dynamics_randomization_args=_TASK_DRAWS_CUBE)
     w.reset()
-    _run(w, _actions(5, 6))
+    _run(w, lift_actions(5, 6))
     snap = w.env.sim.snapshot()
     torch.cuda.synchronize()
     checked = 0

@@ -3,12 +3,10 @@ phase 0 files each environment under the cost class the tail wrote for it the su
 the tail launch takes an environment by its rank, most expensive class first (b2s_pipeline.cuh, tail_env_at).  Which warp runs an
 environment never changes its arithmetic: every case here is bit-identical to the fused kernel over the contact-rich scripted Lift
 rollout, with many tail blocks per group."""
-import os
-
 import numpy as np
 import pytest
 
-from tests.test_gpu_pipeline_tail import _rollout, _same
+from tests.schedules import assert_same, lift_rollout, switches
 from tests.util import lift_states, load
 
 pytestmark = pytest.mark.gpu
@@ -21,16 +19,17 @@ pytestmark = pytest.mark.gpu
     (256, 1, 25, (4, 24)),    # the first blocks get more overflowed environments than they have full-capacity warps
 ])
 def test_ordered_tail_matches_fused(n, groups, nsub, tier_small):
-    a = _rollout(0, nsub, n=n)
-    b = _rollout(1, nsub, n=n, groups=groups, tier_small=tier_small)
-    _same(a, b)
+    calls = 300 // nsub
+    a = lift_rollout(0, calls, nsub, n=n, push_from=calls // 4)
+    b = lift_rollout(1, calls, nsub, n=n, groups=groups, tier_small=tier_small, push_from=calls // 4)
+    assert_same(a, b)
 
 
 def test_ordered_tail_f64_matches_fused():
     """f64 Lift tail blocks hold fewer than 8 warps, below the sorting threshold of choose_blocks: the id-order tail kernel"""
-    a = _rollout(0, 25, substeps=150, n=256, precision="f64")
-    b = _rollout(1, 25, substeps=150, n=256, groups=1, precision="f64")
-    _same(a, b)
+    a = lift_rollout(0, 6, n=256, precision="f64", push_from=1)
+    b = lift_rollout(1, 6, n=256, groups=1, precision="f64", push_from=1)
+    assert_same(a, b)
 
 
 def test_order_is_a_permutation_sorted_by_the_previous_keys():
@@ -44,14 +43,11 @@ def test_order_is_a_permutation_sorted_by_the_previous_keys():
     model = load("Lift_Panda")
     q, _ = lift_states(model, n, seed=21)
     rng = np.random.default_rng(3)
-    os.environ["B2S_GROUPS"] = str(G)
-    try:
+    with switches(groups=G):
         sim = BatchedSim(model, n, precision="f32")
         sim.ctrl_config(cc.resolve(model, cc.default_composite_config(), CtrlCfg))
         sim.set_export(False)  # env_step runs the pipeline only without the derived-array export
         sim.set_mode(1)  # reads B2S_GROUPS
-    finally:
-        os.environ.pop("B2S_GROUPS", None)
     sim.qpos.copy_(torch.as_tensor(q, dtype=sim.dtype))
     sim.forward()
     sim.ctrl_reset()
