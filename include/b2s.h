@@ -168,11 +168,33 @@ int b2s_perturb_model(b2s_sim* sim, const uint8_t* env_mask, uint64_t seed, uint
 /* Observation program = MujocoEnv._get_observations flattened (environments/base.py:429-465): one (op, a, b) entry
  * per output scalar (ops: enum OB_* in csrc/b2s_types.cuh; OB_REL_*_LAG entries read the previous sample, as the reference's
  * sensor ordering does: manipulation_env.py:268-329).  Creates the device arrays "obs" [n_env, obs_dim] and "obs_fresh" [n_env]
- * (1 = observation cache empty; set it when an environment is reset).  "obs" is written by b2s_env_step after the LAST
- * substep - reset()'s forced update advances the observables' period timer by one model step, so every later sample falls on
- * the last substep of a control step (utils/observables.py:214-259, environments/base.py:418-427) - and by b2s_forward for
- * environments whose obs_fresh flag is set. obs_dim <= 128. */
+ * (1 = observation cache empty; set it when an environment is reset).  "obs" is written by b2s_env_step when an observable samples
+ * and by b2s_forward for environments whose obs_fresh flag is set.  Without b2s_obs_modifiers every observable samples after the
+ * LAST substep of a control step: reset()'s forced update advances the observables' period timer by one model step, so at the
+ * control rate every later sample falls on the last substep (utils/observables.py:214-259, environments/base.py:418-427).
+ * obs_dim <= 128. */
 int b2s_obs_config(b2s_sim* sim, int obs_dim, const int* op_host, const int* a_host, const int* b_host);
+/* Sampling rates and corruptors of the observables (Observable.sampling_rate / corruptor, utils/observables.py, with delay 0).
+ * row_obs_host[obs_dim] maps each observation row to its observable (0 .. nobs - 1); mods_host[nobs] gives each observable's period
+ * T = 1 / sampling_rate in seconds and its corruptor: B2S_CORRUPT_GAUSSIAN (p0 = mean, p1 = std) adds mean + std * z,
+ * B2S_CORRUPT_UNIFORM (p0 = min_noise, p1 = max_noise) adds min + (max - min) * u, both then clip to [low, high];
+ * B2S_CORRUPT_NONE leaves the value as it is.  Per environment and observable a timer t (fp64), a flag `sampled` and a sample count
+ * follow Observable.update after every substep (dt = the model's timestep in fp64):
+ *   t += dt;  if not sampled and t <= T: sample, sampled = 1;  if t >= T: sample if not sampled, sampled = 0, t = fmod(t, T)
+ * and reset (b2s_forward of an environment whose obs_fresh flag is set) restarts it with t = 0, sampled = 0 and a forced sample.
+ * A sample forms the observable's rows as above (poses of this substep's step1, qpos / qvel after its step2) and corrupts them;
+ * the rows are the observation cache the lagged entries read.  Noise: Philox4x32-10 with key = seed and counter = (env, the
+ * observable's sample count, row, 0), u1 / u2 = 53 bits of output words (0, 1) / (2, 3) as b2s_perturb_model forms u, z by
+ * Box-Muller sqrt(-2 log(1 - u1)) cos(2 pi u2), arithmetic in fp64, rounded to the handle's precision last.  Sample counts are never
+ * rewound, so episodes do not repeat their noise.  The first call creates "obs_timer" [n_env, nobs] f64, "obs_sampled" [n_env] i32
+ * (bit o = observable o) and "obs_nsample" [n_env, nobs] i32; a call on a handle without modifiers (re)starts the timers in the
+ * state the default rule has at a control-step boundary (t = dt, sampled).  While configured, the three arrays are snapshot
+ * sections.  nobs = 0 clears the configuration (the handle runs exactly as before the first call).  B2S_ERR_ARG: observations not
+ * configured, nobs > 32, a non-positive or non-finite period, an unknown corruptor, a non-finite noise parameter, std < 0,
+ * max_noise < min_noise, low > high, or a row mapped out of range. */
+enum { B2S_CORRUPT_NONE = 0, B2S_CORRUPT_GAUSSIAN = 1, B2S_CORRUPT_UNIFORM = 2 };
+typedef struct { double period; int corruptor; double p0, p1, low, high; } b2s_obs_mod;
+int b2s_obs_modifiers(b2s_sim* sim, int nobs, const int* row_obs_host, const b2s_obs_mod* mods_host, uint64_t seed);
 /* Task outputs "task_out" [n_env,8] = (target body height, |site - body|, grasp flag, horizontal |body - body2|,
  * obj-obj2 contact flag, 0, 0, 0) from the poses/contacts of the
  * last step1 (what the reference's reward()/_check_grasp read: manipulation/lift.py:224-273, manipulation_env.py:331-376).
@@ -198,12 +220,13 @@ int b2s_task_table(b2s_sim* sim, int n, const int* op, const int* a, const int* 
  *                    ctrl_jv_state ctrl_torque, gjk_cache (npair x 3; written as zeros and ignored on restore while the handle has no
  *                    cache: fused mode before the pipeline's first use, or B2S_NO_GJK_CACHE)
  *   b2s_obs_config   obs, obs_fresh (i32), task_out
+ *   b2s_obs_modifiers  obs_timer (f64), obs_sampled (i32), obs_nsample (i32), while configured
  *   b2s_task_table   task_vec
  *   overrides        body_xpos_ov:<id> body_xquat_ov:<id> per pose override; geom_{size,friction,rbound,aabb,solref,solimp}:<id> per geom
  *                    slot; body_mass:<id> body_inertia:<id> per body slot; the declared dof vectors; dof_invweight0 body_invweight0
  *                    meaninertia (copied, not recomputed: a snapshot taken while they were stale restores them stale)
  * Not in a row: the exported derived arrays (xpos, contacts, efc_*, ...), ncon / nefc / solver_niter, pipeline workspaces,
- * and handle configuration (controller gains, obs / task tables, perturbation tables).
+ * and handle configuration (controller gains, obs / task tables, perturbation tables, observable rates and corruptors).
  * The SIGNATURE is a 64-bit FNV-1a hash of the section table (names, counts, dtypes), the precision, the controller kind, the obs and
  * task op tables and the model blob without its capacity records (opt_maxcon, opt_maxefc and the small-tier pair): rows restore only
  * into a handle with the same signature (the Python layer checks it; the C layer does not).

@@ -136,6 +136,11 @@ struct b2s_sim {
   uint64_t snap_sig = 0, blob_hash = 0;  // blob_hash: the model blob without its capacity records
   SnapSec* snap_dev = nullptr;           // device copy of the section table (capacity SNAP_MAXSEC)
   std::vector<int> obs_tab_h, task_tab_h;  // host copies of the observation / task op tables (signature)
+  // b2s_obs_modifiers: the device table (allocated at the first call), observables of the per-environment arrays (0: none yet),
+  // whether a configuration is active, the model's timestep in fp64
+  ObsModDev* obs_mod_dev = nullptr;
+  int obs_arr_n = 0, obs_mod_on = 0;
+  double timestep_h = 0;
 };
 
 // Every entry point picks the handle's precision once: f(DModel<R>&, DState<R>&) runs with R = float or double, and
@@ -194,7 +199,8 @@ template <typename R> static void build_model(b2s_sim* s, const Blob& b, DModel<
   m.nq = b.scalar_i("nq"); m.nv = b.scalar_i("nv"); m.nu = b.scalar_i("nu"); m.nbody = b.scalar_i("nbody");
   m.njnt = b.scalar_i("njnt"); m.ngeom = b.scalar_i("ngeom"); m.nsite = b.scalar_i("nsite"); m.npair = b.scalar_i("npair");
   m.nmocap = b.scalar_i("nmocap");
-  m.timestep = (R)b.scalar_f("opt_timestep"); m.impratio = (R)b.scalar_f("opt_impratio");
+  s->timestep_h = b.scalar_f("opt_timestep");
+  m.timestep = (R)s->timestep_h; m.impratio = (R)b.scalar_f("opt_impratio");
   m.density = (R)b.scalar_f("opt_density"); m.viscosity = (R)b.scalar_f("opt_viscosity");
   m.tolerance = (R)b.scalar_f("opt_tolerance"); m.meaninertia = (R)b.scalar_f("stat_meaninertia");
   m.iterations = b.scalar_i("opt_iterations"); m.ls_iterations = b.scalar_i("opt_ls_iterations");
@@ -1506,9 +1512,72 @@ int b2s_obs_config(b2s_sim* s, int obs_dim, const int* op, const int* a, const i
       st.obs = state_arr<R>(s, "obs", obs_dim); st.task_out = state_arr<R>(s, "task_out", 8); st.obs_fresh = fresh;
     });
   } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
+  with_real(s, [](auto&, auto& st) { st.obs_mod = nullptr; });  // the rows of a previous table no longer exist
+  if (s->obs_mod_on) s->obs_mod_on = 0;
   s->has_obs = 1;
   s->dirty = 1;
   s->layout_version++;
+  return B2S_OK;
+}
+
+int b2s_obs_modifiers(b2s_sim* s, int nobs, const int* row_obs, const b2s_obs_mod* mods, uint64_t seed) {
+  if (!s) return fail(B2S_ERR_ARG, "null handle");
+  if (!s->has_obs) return fail(B2S_ERR_ARG, "b2s_obs_modifiers: observations are not configured (b2s_obs_config)");
+  if (nobs < 0 || nobs > B2S_MAXOBS) return fail(B2S_ERR_ARG, "b2s_obs_modifiers: nobs must be in [0, 32]");
+  if (nobs > 0 && (!row_obs || !mods)) return fail(B2S_ERR_ARG, "b2s_obs_modifiers: bad argument");
+  const int od = s->ctrl.obs_dim;
+  ObsModDev h{};
+  h.nobs = nobs; h.seed = seed; h.dt = s->timestep_h;
+  for (int o = 0; o < nobs; o++) {
+    const b2s_obs_mod& q = mods[o];
+    const std::string at = "b2s_obs_modifiers: observable " + std::to_string(o) + ": ";
+    if (!(q.period > 0) || !std::isfinite(q.period)) return fail(B2S_ERR_ARG, at + "the period must be finite and > 0");
+    if (q.corruptor != B2S_CORRUPT_NONE && q.corruptor != B2S_CORRUPT_GAUSSIAN && q.corruptor != B2S_CORRUPT_UNIFORM)
+      return fail(B2S_ERR_ARG, at + "unknown corruptor");
+    if (q.corruptor != B2S_CORRUPT_NONE) {
+      if (!std::isfinite(q.p0) || !std::isfinite(q.p1)) return fail(B2S_ERR_ARG, at + "noise parameters must be finite");
+      if (q.corruptor == B2S_CORRUPT_GAUSSIAN && q.p1 < 0) return fail(B2S_ERR_ARG, at + "std < 0");
+      if (q.corruptor == B2S_CORRUPT_UNIFORM && q.p1 < q.p0) return fail(B2S_ERR_ARG, at + "max_noise < min_noise");
+      if (!(q.low <= q.high)) return fail(B2S_ERR_ARG, at + "low > high");
+    }
+    h.period[o] = q.period; h.kind[o] = q.corruptor; h.p0[o] = q.p0; h.p1[o] = q.p1; h.lo[o] = q.low; h.hi[o] = q.high;
+  }
+  for (int k = 0; k < od && nobs > 0; k++) {
+    if (row_obs[k] < 0 || row_obs[k] >= nobs)
+      return fail(B2S_ERR_ARG, "b2s_obs_modifiers: row " + std::to_string(k) + " is mapped to observable " + std::to_string(row_obs[k]) + ", out of range");
+    h.row_obs[k] = row_obs[k];
+  }
+  CUDA_TRY(cudaSetDevice(s->device));
+  const ObsModDev* dev = nullptr;
+  if (nobs > 0) {
+    try {
+      if (!s->obs_mod_dev) s->obs_mod_dev = dev_zeros<ObsModDev>(s, 1);
+      if (s->obs_arr_n != nobs) {  // replaced arrays stay allocated until the handle is destroyed
+        s->arrays.erase("obs_timer"); s->arrays.erase("obs_sampled"); s->arrays.erase("obs_nsample");
+        state_arr<double>(s, "obs_timer", nobs);
+        state_arr_i(s, "obs_sampled", 0);
+        state_arr_i(s, "obs_nsample", nobs);
+        s->obs_arr_n = nobs;
+        s->obs_mod_on = 0;
+      }
+    } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
+    h.timer = (double*)s->arrays["obs_timer"].ptr; h.sampled = (int*)s->arrays["obs_sampled"].ptr; h.nsample = (int*)s->arrays["obs_nsample"].ptr;
+    if (!s->obs_mod_on) {  // the state of the default rule at a control-step boundary; the sample counts are kept
+      std::vector<double> t((size_t)s->n_env * nobs, s->timestep_h);
+      std::vector<int> f(s->n_env, (int)(nobs == 32 ? 0xffffffffu : (1u << nobs) - 1u));
+      CUDA_TRY(cudaMemcpyAsync(h.timer, t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice, s->stream));
+      CUDA_TRY(cudaMemcpyAsync(h.sampled, f.data(), f.size() * sizeof(int), cudaMemcpyHostToDevice, s->stream));
+      CUDA_TRY(cudaStreamSynchronize(s->stream));  // pageable sources
+    }
+    // stream-ordered behind the kernels that read the previous table
+    CUDA_TRY(cudaMemcpyAsync(s->obs_mod_dev, &h, sizeof(h), cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaStreamSynchronize(s->stream));
+    dev = s->obs_mod_dev;
+  }
+  with_real(s, [&](auto&, auto& st) { st.obs_mod = dev; });
+  if ((nobs > 0) != (s->obs_mod_on != 0)) s->layout_version++;  // the snapshot sections change
+  s->obs_mod_on = nobs > 0;
+  s->dirty = 1;
   return B2S_OK;
 }
 
@@ -1595,6 +1664,10 @@ static int ensure_snap(b2s_sim* s) {
     add("ctrl_grip_state", st.grip_state, 4, R); add("ctrl_jv_state", st.jv_state, 72, R); add("ctrl_torque", st.ctrl_torque, 8, R);
     add("gjk_cache", st.gjk_cache, (int64_t)m.npair * 3, R);  // null until the pipeline's first use, or with B2S_NO_GJK_CACHE
     if (s->has_obs) { add("obs", st.obs, s->ctrl.obs_dim, R); add("obs_fresh", st.obs_fresh, 1, B2S_I32); add("task_out", st.task_out, 8, R); }
+    if (s->obs_mod_on) {
+      add("obs_timer", s->arrays["obs_timer"].ptr, s->obs_arr_n, B2S_F64); add("obs_sampled", s->arrays["obs_sampled"].ptr, 1, B2S_I32);
+      add("obs_nsample", s->arrays["obs_nsample"].ptr, s->obs_arr_n, B2S_I32);
+    }
     if (st.task_vec) add("task_vec", st.task_vec, s->ctrl.task_dim, R);
     for (int k = 0; k < st.n_ov; k++) {
       const std::string id = std::to_string(st.ov_body[k]);

@@ -447,6 +447,13 @@ template <typename R> DEV R table_value(const Eng<R>& e, int op, int a, int b, c
         v = r[comp];
       } else {
         R rel[9], q[4];
+        if (e.state().obs_mod != nullptr) {
+          // with observable modifiers the cache may be corrupted, so not unit-length: normalise it as the reference's quat2mat does
+          // (transform_utils.py: q *= sqrt(2 / n), the identity when n < 4 eps); a unit cache needs no such step
+          const R n = qo[0] * qo[0] + qo[1] * qo[1] + qo[2] * qo[2] + qo[3] * qo[3];
+          if (n < R(8.881784197001252e-16)) { qo[0] = 1; qo[1] = 0; qo[2] = 0; qo[3] = 0; }
+          else { const R sc = R(1) / r_sqrt(n); for (int k = 0; k < 4; k++) qo[k] *= sc; }
+        }
         q2mat(Ro, qo);
         for (int i = 0; i < 3; i++)
           for (int j = 0; j < 3; j++) rel[3 * i + j] = Re[i] * Ro[j] + Re[3 + i] * Ro[3 + j] + Re[6 + i] * Ro[6 + j];
@@ -460,26 +467,87 @@ template <typename R> DEV R table_value(const Eng<R>& e, int op, int a, int b, c
   return v;
 }
 
+// Observable timers: Observable.update with delay 0 (utils/observables.py:214-259), called after every substep's step2
+// (environments/base.py:494-505), one lane per observable, in fp64 in both precisions so the sample instants follow Python's floats:
+//   t += dt;  if (force or (not sampled and t <= T)): sample, sampled = 1;  if (t >= T): (sample if not sampled), sampled = 0, t = fmod(t, T)
+// Returns the mask of the observables that sample now.  `only_fresh` (forward()): only an environment whose observation cache is empty
+// (just reset) samples, with reset()'s forced update (environments/base.py:418-427): t = 0, sampled = 0, then the update with force.
+// Without modifiers (DState::obs_mod null) every observable samples on the last substep, which is where this rule puts the samples of
+// the default rate.  The timers live out of line: inlined, their fp64 code (fmod) cost the tail's default path spill slots.
+template <typename R> DEVN unsigned obs_timers(const Eng<R> e, int env, bool only_fresh) {
+  const ObsModDev* om = e.state().obs_mod;
+  if (only_fresh && !e.state().obs_fresh[env]) return 0u;
+  const int n = om->nobs, lane = e.lane;
+  const size_t i = (size_t)env * n + lane;
+  bool sampled = !only_fresh && ((om->sampled[env] >> lane) & 1), due = false;
+  if (lane < n) {
+    const double T = om->period[lane];
+    double t = __dadd_rn(only_fresh ? 0.0 : om->timer[i], om->dt);
+    if (only_fresh || (!sampled && t <= T)) { due = true; sampled = true; }
+    if (t >= T) {
+      if (!sampled) due = true;
+      sampled = false;
+      t = fmod(t, T);
+    }
+    om->timer[i] = t;
+  }
+  const unsigned dm = __ballot_sync(B2S_FULL, due), sm = __ballot_sync(B2S_FULL, sampled && lane < n);
+  if (lane == 0) om->sampled[env] = (int)sm;
+  return dm;
+}
+template <typename R> DEV unsigned obs_due(const Eng<R>& e, int env, bool last, bool only_fresh) {
+  return e.state().obs_mod == nullptr ? (last ? ~0u : 0u) : obs_timers(e, env, only_fresh);
+}
+
+// Corruptor of observation row k of a sample (create_gaussian_noise_corrupter / create_uniform_noise_corrupter, utils/observables.py):
+// Philox4x32-10 keyed by the seed, counter (env, the observable's sample count, row, 0), so an environment's noise depends on neither the
+// batch nor the mask.  u1, u2 = 53 bits of output words (0, 1) and (2, 3) as in perturb_kernel.
+//   Gaussian  v + (mean + std * z),  z = sqrt(-2 log(1 - u1)) cos(2 pi u2)      Uniform  v + (min + (max - min) u1)
+// then clipped to [low, high], in fp64 without contraction, rounded to the handle's precision last.
+template <typename R> DEV R obs_corrupt(const ObsModDev* om, int env, int k, R v) {
+  const int o = om->row_obs[k], kind = om->kind[o];
+  if (kind == OBS_CORRUPT_NONE) return v;
+  const unsigned cnt = (unsigned)om->nsample[(size_t)env * om->nobs + o];
+  const uint4 x = philox4x32_10(make_uint4((unsigned)env, cnt, (unsigned)k, 0u), (unsigned)om->seed, (unsigned)(om->seed >> 32));
+  const double u1 = (double)(((unsigned long long)(x.x >> 5) << 26) | (x.y >> 6)) * 0x1p-53;
+  double d;
+  if (kind == OBS_CORRUPT_GAUSSIAN) {
+    const double u2 = (double)(((unsigned long long)(x.z >> 5) << 26) | (x.w >> 6)) * 0x1p-53;
+    const double z = __dmul_rn(sqrt(__dmul_rn(-2.0, log(__dsub_rn(1.0, u1)))), cos(__dmul_rn(6.283185307179586, u2)));
+    d = __dadd_rn(om->p0[o], __dmul_rn(om->p1[o], z));
+  } else {
+    d = __dadd_rn(om->p0[o], __dmul_rn(__dsub_rn(om->p1[o], om->p0[o]), u1));
+  }
+  return (R)fmin(fmax(__dadd_rn((double)v, d), om->lo[o]), om->hi[o]);
+}
+
+// The observation rows of the observables in `due` (bit o: observable o = obs_mod->row_obs[row]; without modifiers every row).
 // `only_fresh`: called from forward() - sample only environments whose observation cache is empty (just reset)
-template <typename R> DEVN void write_obs(const Eng<R> e, int env, bool only_fresh = false) {
+template <typename R> DEVN void write_obs(const Eng<R> e, int env, bool only_fresh, unsigned due) {
   const DState<R>& s = e.state();
   const CtrlCfgDev& cc = e.ccfg();
+  const ObsModDev* om = s.obs_mod;
   R* out = s.obs + (size_t)env * cc.obs_dim;
   int fresh = s.obs_fresh[env];
   if (only_fresh && !fresh) return;
   R val[4];  // obs_dim <= 128: all values are formed before any is written (lagged entries read the previous sample)
+  unsigned on = 0;
 #pragma unroll 1
-  for (int it = 0; it < 4; it++) {  // rolled: table_value is large and runs once per control step
+  for (int it = 0; it < 4; it++) {  // rolled: table_value is large and runs once per sample
     int k = e.lane + 32 * it;
-    val[it] = k < cc.obs_dim ? table_value(e, cc.obs_op[k], cc.obs_a[k], cc.obs_b[k], out, fresh) : R(0);
+    const bool take = k < cc.obs_dim && (om == nullptr || ((due >> om->row_obs[k]) & 1));
+    val[it] = take ? table_value(e, cc.obs_op[k], cc.obs_a[k], cc.obs_b[k], out, fresh) : R(0);
+    if (take && om) val[it] = obs_corrupt(om, env, k, val[it]);
+    on |= (unsigned)take << it;
   }
   __syncwarp();
 #pragma unroll 1
   for (int it = 0; it < 4; it++) {
     int k = e.lane + 32 * it;
-    if (k < cc.obs_dim) out[k] = val[it];
+    if ((on >> it) & 1) out[k] = val[it];
   }
   if (e.lane == 0 && fresh) s.obs_fresh[env] = 0;
+  if (om && e.lane < om->nobs && ((due >> e.lane) & 1)) om->nsample[(size_t)env * om->nobs + e.lane]++;
 }
 
 // Task outputs after the last substep (poses / contacts of the last step1, as the reference's reward() sees them:

@@ -168,10 +168,13 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
       }
     }
     if (live && (phases & PH_OBS) && c_cc[slot].obs_dim > 0) {
-      // The reference's observables sample on the LAST substep of a control step: reset()'s forced update already
-      // advances their period timer by one model timestep (utils/observables.py:214-259, environments/base.py:418-427),
-      // so the period closes after substep 24 and the next update - substep 25 - takes the sample.
-      if (sub == nsub - 1) { write_obs(e, env, (phases & PH_NOINTEGRATE) != 0); write_task(e, env, ncon); }
+      // The reference's observables sample on the LAST substep of a control step at the default rate: reset()'s forced update
+      // already advances their period timer by one model timestep (utils/observables.py:214-259, environments/base.py:418-427),
+      // so the period closes after substep 24 and the next update - substep 25 - takes the sample.  Other rates: obs_due.
+      const bool last = sub == nsub - 1, only_fresh = (phases & PH_NOINTEGRATE) != 0;
+      const unsigned due = obs_due(e, env, last, only_fresh);
+      if (due) write_obs(e, env, only_fresh, due);
+      if (last) write_task(e, env, ncon);
     }
     __syncwarp();
   }
@@ -325,17 +328,6 @@ __global__ void __launch_bounds__(512, 1) set_const_kernel(const uint8_t* mask, 
 // with explicit roundings (no contraction), so a host restatement reproduces every bit; the result is rounded to the handle's precision.
 struct PerturbEntry { void* dst; int stride, mode, one_draw; double amp; };  // value of (env, component c) at dst[env * stride + c]
 struct PerturbItem { int entry, comp; double model; };                     // one per (entry, component), in entry order
-
-DEV uint4 philox4x32_10(uint4 c, unsigned k0, unsigned k1) {
-#pragma unroll
-  for (int r = 0; r < 10; r++) {
-    if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
-    const unsigned lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
-    const unsigned lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
-    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
-  }
-  return c;
-}
 
 template <typename R>
 __global__ void perturb_kernel(const PerturbEntry* ent, const PerturbItem* item, int nitems, int n_env, const uint8_t* mask,

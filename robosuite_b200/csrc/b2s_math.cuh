@@ -143,3 +143,15 @@ template <typename R> DEV void warp_argmax(R& v, int& idx) {
     if (ov > v || (ov == v && oi < idx)) { v = ov; idx = oi; }
   }
 }
+
+// Philox4x32-10 (Salmon et al., SC'11): the counter-based generator of the device draws (perturb_kernel, the observation corruptors)
+DEV uint4 philox4x32_10(uint4 c, unsigned k0, unsigned k1) {
+#pragma unroll
+  for (int r = 0; r < 10; r++) {
+    if (r) { k0 += 0x9E3779B9u; k1 += 0xBB67AE85u; }
+    const unsigned lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+    const unsigned lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+    c = make_uint4(hi1 ^ c.y ^ k0, lo1, hi0 ^ c.w ^ k1, lo0);
+  }
+  return c;
+}

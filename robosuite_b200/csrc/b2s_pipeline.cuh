@@ -355,7 +355,8 @@ template <typename R> DEV int tail_newton(Eng<R>& e, int nefc, int ncon, int* ni
   return warn;
 }
 
-// Finish: Euler, on the last substep of a control step the observation and task rows, state write-back.
+// Finish: Euler, the rows of the observables that sample on this substep (obs_due: all of them on the last substep without
+// modifiers), on the last substep of a control step the task rows, state write-back.
 template <typename R>
 DEV void tail_finish(Eng<R>& e, int env, int sub, int nsub, int phases, int ncon, int warn, unsigned long long* bar, unsigned& parity) {
   const DState<R>& s = e.state();
@@ -364,14 +365,17 @@ DEV void tail_finish(Eng<R>& e, int env, int sub, int nsub, int phases, int ncon
   if (!(phases & PH_NOINTEGRATE)) {
     { int eb = e.euler(&time); if (eb & 32) warn |= 32; else if (eb) warn |= 2; }
   }
-  if ((phases & PH_OBS) && e.ccfg().obs_dim > 0 && sub == nsub - 1) {
-    // The reference's observables sample on the LAST substep of a control step: reset()'s forced update already
-    // advances their period timer by one model timestep (utils/observables.py:214-259, environments/base.py:418-427),
-    // so the period closes after substep 24 and the next update - substep 25 - takes the sample.
-    // Body / site poses of this substep's step1 arrive now, over the (dead) constraint Jacobian.
-    ws_load(e, s.wsg + (size_t)env * c_lay[e.slot][LAY_ROW].total, c_pio[e.slot][e.lid == LAY_TL ? PIO_TL_LATE : PIO_TS_LATE], bar, parity);
-    write_obs(e, env, (phases & PH_NOINTEGRATE) != 0);
-    write_task(e, env, ncon);
+  if ((phases & PH_OBS) && e.ccfg().obs_dim > 0) {
+    // The reference's observables sample on the LAST substep of a control step at the default rate: reset()'s forced update
+    // already advances their period timer by one model timestep (utils/observables.py:214-259, environments/base.py:418-427),
+    // so the period closes after substep 24 and the next update - substep 25 - takes the sample.  Other rates: obs_due.
+    const bool last = sub == nsub - 1, only_fresh = (phases & PH_NOINTEGRATE) != 0;
+    const unsigned due = obs_due(e, env, last, only_fresh);
+    // Body / site poses of this substep's step1 arrive now, over the (dead) constraint Jacobian (`due` is warp-uniform).
+    if (due || last)
+      ws_load(e, s.wsg + (size_t)env * c_lay[e.slot][LAY_ROW].total, c_pio[e.slot][e.lid == LAY_TL ? PIO_TL_LATE : PIO_TS_LATE], bar, parity);
+    if (due) write_obs(e, env, only_fresh, due);
+    if (last) write_task(e, env, ncon);
   }
   store_state(e, env, time, warn);
 }

@@ -123,6 +123,7 @@ struct DState {
                    // tail's Newton iterations, line-search evaluations, nefc, ncon, capacity tier (1 = large) and tail block index
   int* solve_ls;   // [n_env] line-search evaluations of the environment's last Newton solve
   int* slowlog;    // [64][12] convex work items above 131 k cycles: cycles, shape types, hull sizes, EPA nV nF, GJK cycles, hit, staged, geoms
+  const struct ObsModDev* obs_mod;  // sampling rates and corruptors (b2s_obs_modifiers); null: every observable on the last substep, no noise
 };
 
 // offsets (in units of R) of the per-warp shared-memory workspace
@@ -172,6 +173,24 @@ enum { OB_QPOS = 0, OB_COS_QPOS, OB_SIN_QPOS, OB_QVEL, OB_QACC, OB_SITE_POS, OB_
        // `{obj}_to_eef_pos/quat` before `{obj}_pos/quat` in the same pass: manipulation_env.py:268-329) and the current
        // hand pose; zeros on the first sample after a reset.  a = pos_slot | quat_slot << 12, b = k | site << 8 | body << 16
        OB_REL_POS_LAG, OB_REL_QUAT_LAG };
+
+// Observable sampling rates and corruptors (b2s_obs_modifiers), kept in device memory (the constant bank is nearly full).  Per
+// observable o: period T = 1 / sampling_rate and the corruptor (kind: B2S_CORRUPT_* of include/b2s.h; p0, p1 = mean, std or
+// min_noise, max_noise; clip range [lo, hi]).  Per environment: the time since the last period boundary, the flags of the
+// observables sampled in the current period, and the samples each observable took (the noise counter, never rewound).
+#define B2S_MAXOBS 32
+struct ObsModDev {
+  int nobs;
+  unsigned long long seed;
+  double dt;  // the model's timestep in fp64 in both precisions: the reference's timers are Python floats
+  double period[B2S_MAXOBS], p0[B2S_MAXOBS], p1[B2S_MAXOBS], lo[B2S_MAXOBS], hi[B2S_MAXOBS];
+  int kind[B2S_MAXOBS];
+  int row_obs[128];  // the observable of each observation row
+  double* timer;     // [n_env, nobs]
+  int* sampled;      // [n_env] bit o: observable o has sampled in its current period
+  int* nsample;      // [n_env, nobs]
+};
+enum { OBS_CORRUPT_NONE = 0, OBS_CORRUPT_GAUSSIAN = 1, OBS_CORRUPT_UNIFORM = 2 };  // = B2S_CORRUPT_* (include/b2s.h)
 
 struct CtrlCfgDev {
   int kind, action_dim, n_arm, eef_site, base_site, n_grip, uncouple;

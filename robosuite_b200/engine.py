@@ -43,6 +43,15 @@ GEOM_CONTACT_FIELDS = ("geom_solref", "geom_solimp")
 PERTURB_SCALE, PERTURB_SHIFT = 0, 1
 
 
+CORRUPT_NONE, CORRUPT_GAUSSIAN, CORRUPT_UNIFORM = 0, 1, 2
+
+
+class ObsMod(C.Structure):
+    """b2s_obs_mod: period (s) and corruptor of one observable (b2s_obs_modifiers)"""
+    _fields_ = [("period", C.c_double), ("corruptor", C.c_int), ("p0", C.c_double), ("p1", C.c_double), ("low", C.c_double),
+                ("high", C.c_double)]
+
+
 class PerturbSpec(C.Structure):
     """b2s_perturb: one (field, id) entry of b2s_perturb_config"""
     _fields_ = [("field", C.c_char_p), ("id", C.c_int), ("mode", C.c_int), ("amplitude", C.c_double), ("one_draw", C.c_int)]
@@ -98,6 +107,7 @@ def lib():
         L.b2s_perturb_config.argtypes = [C.c_void_p, C.POINTER(PerturbSpec), C.c_int]
         L.b2s_perturb_model.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64]
         L.b2s_obs_config.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
+        L.b2s_obs_modifiers.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(ObsMod), C.c_uint64]
         L.b2s_task_config.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.b2s_task_config2.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.b2s_task_objects.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
@@ -344,6 +354,21 @@ class BatchedSim:
     def obs_config(self, ops, a, b):
         ops, a, b = (np.ascontiguousarray(x, dtype=np.int32) for x in (ops, a, b))
         self._check(self._L.b2s_obs_config(self._h, len(ops), ops.ctypes.data, a.ctypes.data, b.ctypes.data))
+
+    def obs_modifiers(self, row_obs, mods, seed=0):
+        """sampling rates and corruptors of the observables (b2s_obs_modifiers): row_obs [obs_dim] = the observable of each observation
+        row, mods = one (period_s, corruptor, p0, p1, low, high) per observable (corruptor CORRUPT_NONE / GAUSSIAN (p0 mean, p1 std) /
+        UNIFORM (p0 min_noise, p1 max_noise)), noise keyed by `seed`.  Empty `mods` clears the configuration.  The per-environment
+        timers, flags and sample counts are the arrays "obs_timer", "obs_sampled" and "obs_nsample"."""
+        mods = list(mods)
+        rows = np.ascontiguousarray(row_obs, dtype=np.int32)
+        arr = (ObsMod * max(len(mods), 1))()
+        for k, (T, kind, p0, p1, lo, hi) in enumerate(mods):
+            arr[k] = ObsMod(float(T), int(kind), float(p0), float(p1), float(lo), float(hi))
+        self._check(self._L.b2s_obs_modifiers(self._h, len(mods), rows.ctypes.data if len(mods) else None, arr,
+                                              int(seed) & (2 ** 64 - 1)))
+        for name in ("obs_timer", "obs_sampled", "obs_nsample"):  # arrays may have been (re)created
+            self._cache.pop(name, None)
 
     def task_config(self, body, site, left, right, obj):
         left, right, obj = (np.ascontiguousarray(x, dtype=np.int32) for x in (left, right, obj))

@@ -157,6 +157,8 @@ class BatchedMujocoEnv:
         ob = ObsBuilder()
         self._setup_observables(ob)
         op, a, b, self._obs_slices, self._modality_slices = ob.tables()
+        self._obs_op = op
+        self._obs_mods = {}  # observable name -> {"sampling_rate": Hz, "corruptor": spec or None} (modify_observable)
         self.obs_dim = len(op)
         self.sim.obs_config(op, a, b)
         self._setup_task()
@@ -395,6 +397,78 @@ class BatchedMujocoEnv:
         # per-environment engine flags since the last reset, as a device tensor (no host sync here; see SIM_WARN_BITS): a non-zero entry means
         # the episode is no longer a faithful MuJoCo rollout (capacity overflow, singular mass matrix / Hessian, diverged state)
         return self._get_observations(), reward, self.done, {"sim_warn": self.sim.warn}
+
+    # ---- observable modifiers (utils/observables.py Observable.set_sampling_rate / set_corrupter, MujocoEnv.modify_observable)
+    _UNSUPPORTED_OBS_ATTRS = {
+        "delayer": "observation delays are not implemented",
+        "filter": "observation filters are not implemented",
+        "sensor": "sensors are fixed observation-table programs on the device",
+        "enabled": "enabling or disabling an observable changes obs_dim",
+        "active": "activating or deactivating an observable changes obs_dim",
+    }
+
+    def modify_observable(self, observable_name, attribute, modifier):
+        """Change one observable of every environment (environments/base.py modify_observable): attribute "corruptor" (or the
+        reference's spelling "corrupter") takes a spec from robosuite_b200.observables (create_gaussian_noise_corruptor /
+        create_uniform_noise_corruptor) or None (no noise); "sampling_rate" takes a rate in Hz > 0.  Sampling and noise run on the
+        device after every substep, as the reference's Observable.update does (delay 0).  The noise key is derived from
+        make(seed=...) (a seed drawn once when seed is None) under a tag of its own, so the same seed given to
+        BatchedDomainRandomizationWrapper draws an independent stream.  Nothing changes if the call raises.  A handle whose
+        observables all keep the control rate and no corruptor runs the unmodified path."""
+        import math
+
+        from ..observables import GaussianNoiseCorruptor, UniformNoiseCorruptor
+
+        if observable_name not in self._obs_slices:
+            raise ValueError("No valid observable with name {} found. Options are: {}".format(observable_name, list(self._obs_slices)))
+        if attribute in self._UNSUPPORTED_OBS_ATTRS:
+            raise NotImplementedError("modify_observable: attribute {!r}: {}".format(attribute, self._UNSUPPORTED_OBS_ATTRS[attribute]))
+        cur = dict(self._obs_mods.get(observable_name, {"sampling_rate": float(self.control_freq), "corruptor": None}))
+        if attribute in ("corruptor", "corrupter"):
+            if modifier is not None and not isinstance(modifier, (GaussianNoiseCorruptor, UniformNoiseCorruptor)):
+                raise NotImplementedError("modify_observable: attribute {!r}: arbitrary callables cannot run on the device; "
+                                          "use robosuite_b200.observables.create_gaussian_noise_corruptor / "
+                                          "create_uniform_noise_corruptor".format(attribute))
+            cur["corruptor"] = modifier
+        elif attribute == "sampling_rate":
+            a, b = self._obs_slices[observable_name]
+            if any(int(op) in (OB_REL_POS_LAG, OB_REL_QUAT_LAG) for op in self._obs_op[a:b]):
+                raise NotImplementedError("modify_observable: attribute 'sampling_rate' of {}: the reference computes it from a hidden "
+                                          "gripper-pose observable that keeps the control rate".format(observable_name))
+            rate = float(modifier)
+            if not (math.isfinite(rate) and rate > 0):
+                raise ValueError("sampling_rate must be a finite rate in Hz > 0, got {}".format(modifier))
+            cur["sampling_rate"] = rate
+        else:
+            raise ValueError("Invalid observable attribute specified. Requested: {}, valid options are {}".format(
+                attribute, ["sensor", "corrupter", "filter", "delayer", "sampling_rate", "enabled", "active"]))
+        mods = dict(self._obs_mods)
+        mods[observable_name] = cur
+        self._upload_obs_modifiers(mods)  # raises before anything is changed on the device
+        self._obs_mods = mods
+
+    def _upload_obs_modifiers(self, obs_mods):
+        """the device tables of `obs_mods` (name -> rate / corruptor), one observable per slice of _obs_slices in observation order"""
+        from ..engine import CORRUPT_NONE
+
+        names = list(self._obs_slices)
+        mods = [obs_mods.get(n, {"sampling_rate": float(self.control_freq), "corruptor": None}) for n in names]
+        if all(m["corruptor"] is None and m["sampling_rate"] == float(self.control_freq) for m in mods):
+            self.sim.obs_modifiers([], [])  # the default rule: every sample on the last substep, no noise
+            return
+        if len(names) > 32:
+            raise NotImplementedError("observable modifiers support at most 32 observables ({} has {})".format(type(self).__name__, len(names)))
+        row_obs = np.zeros(self.obs_dim, dtype=np.int32)
+        for o, n in enumerate(names):
+            a, b = self._obs_slices[n]
+            row_obs[a:b] = o
+        spec = [(1.0 / m["sampling_rate"],) + (m["corruptor"].spec() if m["corruptor"] is not None else (CORRUPT_NONE, 0.0, 0.0, -np.inf, np.inf))
+                for m in mods]
+        if "_obs_noise_seed" not in self.__dict__:
+            base = int(self.seed) if self.seed is not None else int(np.random.SeedSequence().generate_state(1, np.uint64)[0])
+            # "OBSN": the observation-noise stream of this seed (Philox keys of the dynamics perturbation take the seed itself)
+            self._obs_noise_seed = int(np.random.SeedSequence([base & (2 ** 64 - 1), 0x4F42534E]).generate_state(1, np.uint64)[0])
+        self.sim.obs_modifiers(row_obs, spec, self._obs_noise_seed)
 
     def check_sim_warnings(self):
         """Host-side check of the engine flags (one device sync): raises SimulationError naming the flags and how many

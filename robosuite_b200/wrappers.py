@@ -73,6 +73,11 @@ class BatchedGymWrapper:
          self.action_space) = _make_spaces(self.obs_dim, self.action_low, self.action_high, self.num_envs)
         self.metadata, self.render_mode, self.spec = {"autoreset_mode": "same_step"}, None, None
 
+    def __getattr__(self, name):  # the environment's own API (modify_observable, get_env_state, ...), as robosuite's Wrapper delegates
+        if name == "env":
+            raise AttributeError(name)
+        return getattr(self.env, name)
+
     def _flatten_obs(self, obs_dict):
         import torch
 
