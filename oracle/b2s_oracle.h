@@ -47,7 +47,7 @@ typedef struct {
   const double *jnt_pos, *jnt_axis, *jnt_range, *jnt_margin, *jnt_solref, *jnt_solimp, *jnt_stiffness;
   const int *dof_bodyid, *dof_jntid, *dof_parentid, *dof_Madr;
   const double *dof_armature, *dof_damping, *dof_frictionloss, *dof_solref, *dof_solimp, *dof_invweight0, *dof_M0;
-  const double* qpos0;
+  const double *qpos0, *qpos_spring;
   /* geoms */
   const int *geom_type, *geom_contype, *geom_conaffinity, *geom_condim, *geom_bodyid, *geom_dataid, *geom_priority;
   const double *geom_size, *geom_pos, *geom_quat, *geom_friction, *geom_solmix, *geom_solref, *geom_solimp,

@@ -64,7 +64,7 @@ OModel* o_model_load(const void* blob_in, size_t nbytes) {
   PF(jnt_pos); PF(jnt_axis); PF(jnt_range); PF(jnt_margin); PF(jnt_solref); PF(jnt_solimp); PF(jnt_stiffness);
   PI(dof_bodyid); PI(dof_jntid); PI(dof_parentid); PI(dof_Madr);
   PF(dof_armature); PF(dof_damping); PF(dof_frictionloss); PF(dof_solref); PF(dof_solimp); PF(dof_invweight0);
-  PF(dof_M0); PF(qpos0);
+  PF(dof_M0); PF(qpos0); PF(qpos_spring);
   PI(geom_type); PI(geom_contype); PI(geom_conaffinity); PI(geom_condim); PI(geom_bodyid); PI(geom_dataid);
   PI(geom_priority);
   PF(geom_size); PF(geom_pos); PF(geom_quat); PF(geom_friction); PF(geom_solmix); PF(geom_solref); PF(geom_solimp);
@@ -447,10 +447,10 @@ void o_rne_bias(const OModel* m, OData* d) {
 void o_passive(const OModel* m, OData* d) {
   int nv = m->nv;
   for (int i = 0; i < nv; i++) d->qfrc_passive[i] = -m->dof_damping[i] * d->qvel[i];
-  /* joint springs (stiffness) - none of the in-scope models use them, kept for completeness on slide/hinge */
+  /* joint springs on slide and hinge joints, about the spring reference (springref), not the joint's zero (ref) */
   for (int j = 0; j < m->njnt; j++)
     if (m->jnt_stiffness[j] != 0 && (m->jnt_type[j] == O_JNT_SLIDE || m->jnt_type[j] == O_JNT_HINGE))
-      d->qfrc_passive[m->jnt_dofadr[j]] -= m->jnt_stiffness[j] * (d->qpos[m->jnt_qposadr[j]] - m->qpos0[m->jnt_qposadr[j]]);
+      d->qfrc_passive[m->jnt_dofadr[j]] -= m->jnt_stiffness[j] * (d->qpos[m->jnt_qposadr[j]] - m->qpos_spring[m->jnt_qposadr[j]]);
   if (m->density <= 0 && m->viscosity <= 0) return;
   /* fluid forces, inertia-box model (option density / viscosity are non-zero in models/assets/base.xml:3-5) */
   double* jp = (double*)malloc(sizeof(double) * 3 * nv);

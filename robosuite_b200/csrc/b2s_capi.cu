@@ -206,6 +206,8 @@ template <typename R> static void build_model(b2s_sim* s, const Blob& b, DModel<
   m.iterations = b.scalar_i("opt_iterations"); m.ls_iterations = b.scalar_i("opt_ls_iterations");
   const double* grav = b.f64("opt_gravity");
   for (int k = 0; k < 3; k++) m.gravity[k] = (R)grav[k];
+  const double* wind = b.f64("opt_wind");
+  for (int k = 0; k < 3; k++) m.wind[k] = (R)wind[k];
   if (b.scalar_i("opt_cone") != 1) throw std::string("only elliptic friction cones are implemented (reference models set cone=elliptic)");
   if (m.nv > 64) throw std::string("nv > 64 not supported");
   int nb = m.nbody, nv = m.nv, nj = m.njnt, ng = m.ngeom;
@@ -266,7 +268,14 @@ template <typename R> static void build_model(b2s_sim* s, const Blob& b, DModel<
   const int* jlim = b.i32("jnt_limited");
   for (int j = 0; j < nj; j++)
     if (jlim[j] && (jtype[j] == JNT_SLIDE || jtype[j] == JNT_HINGE)) lim_jnt.push_back(j);
-  m.nfl = (int)fl_dof.size(); m.nlim = (int)lim_jnt.size();
+  std::vector<int> spr_jnt;
+  const double* stiff = b.f64("jnt_stiffness");
+  for (int j = 0; j < nj; j++) {
+    if (stiff[j] == 0) continue;
+    if (jtype[j] == JNT_FREE) throw std::string("stiffness on a free joint is not supported");
+    spr_jnt.push_back(j);
+  }
+  m.nfl = (int)fl_dof.size(); m.nlim = (int)lim_jnt.size(); m.nspr = (int)spr_jnt.size();
   std::vector<unsigned long long> dofmask(nb, 0ull);
   for (int i = 1; i < nb; i++) {
     dofmask[i] = dofmask[parent[i]];
@@ -339,6 +348,7 @@ template <typename R> static void build_model(b2s_sim* s, const Blob& b, DModel<
   m.dof_bodyid = up_i(s, b, "dof_bodyid"); m.dof_jntid = up_i(s, b, "dof_jntid"); m.dof_parentid = up_i(s, b, "dof_parentid");
   m.dof_kind = dev_upload(s, dkind); m.dof_cddstart = dev_upload(s, cddstart); m.fl_dof = dev_upload(s, fl_dof);
   m.lim_jnt = dev_upload(s, lim_jnt); m.body_dofmask = dev_upload(s, dofmask);
+  m.spr_jnt = dev_upload(s, spr_jnt); m.jnt_stiffness = up_f<R>(s, b, "jnt_stiffness"); m.qpos_spring = up_f<R>(s, b, "qpos_spring");
   m.dof_armature = up_f<R>(s, b, "dof_armature"); m.dof_damping = up_f<R>(s, b, "dof_damping");
   m.dof_frictionloss = up_f<R>(s, b, "dof_frictionloss"); m.dof_solref = up_f<R>(s, b, "dof_solref");
   m.dof_solimp = up_f<R>(s, b, "dof_solimp"); m.dof_invweight0 = up_f<R>(s, b, "dof_invweight0");

@@ -374,7 +374,7 @@ struct Eng {
   }
 
   // ------------------------------------------------------------------------------------------- velocity stage
-  // cvel, cdof_dot, RNE bias forces, passive (damping + fluid) forces
+  // cvel, cdof_dot, RNE bias forces, passive (damping + fluid + joint spring) forces
   DEVN void velocity() {
     const DModel<R>& m = model(); const WSLayout& L = lay();
     const R* cdof = p(L.cdof); const R* qvel = p(L.qvel);
@@ -440,6 +440,7 @@ struct Eng {
         R lin[3], t[3], lv[6], lf[6] = {0, 0, 0, 0, 0, 0};
         v3cross(t, cv, c);
         v3add(lin, cv + 3, t);
+        lin[0] -= m.wind[0]; lin[1] -= m.wind[1]; lin[2] -= m.wind[2];  // relative to the medium (exact without wind)
         m3mulTv(lv, Ri, cv);
         m3mulTv(lv + 3, Ri, lin);
         if (m.viscosity > 0) {
@@ -484,6 +485,15 @@ struct Eng {
       passive[i] = -damping[i] * qvel[i] + dot6(cdof + 6 * i, g);
     }
     __syncwarp();
+    // joint springs: one uniform count test for a model without them
+    if (m.nspr > 0) {
+      const R* qpos = p(L.qpos);
+      for (int k = lane; k < m.nspr; k += 32) {
+        int j = m.spr_jnt[k], qa = m.jnt_qposadr[j];
+        passive[m.jnt_dofadr[j]] -= m.jnt_stiffness[j] * (qpos[qa] - m.qpos_spring[qa]);
+      }
+      __syncwarp();
+    }
   }
 
   // ------------------------------------------------------------------------------------------- CRB -> dense M

@@ -27,11 +27,11 @@ enum {
 
 template <typename R>
 struct DModel {
-  int nq, nv, nu, nbody, njnt, ngeom, nsite, npair, ncg, nment, maxdepth, maxcon, maxefc, nmocap, nfl, nlim, hc_stride, max_treesize;
+  int nq, nv, nu, nbody, njnt, ngeom, nsite, npair, ncg, nment, maxdepth, maxcon, maxefc, nmocap, nfl, nlim, nspr, hc_stride, max_treesize;
   int stage_cap;  // reals of shared memory the convex narrow-phase kernel has for staging the hull vertices of a pair
   R timestep, impratio, density, viscosity, tolerance, meaninertia;
   int iterations, ls_iterations;
-  R gravity[3];
+  R gravity[3], wind[3];
   // bodies
   const int *body_parentid, *body_jntid, *body_dofnum, *body_dofadr, *body_weldid, *body_subtree_end, *body_depth;
   const R *body_pos, *body_quat, *body_ipos, *body_iquat, *body_mass, *body_inertia, *body_invweight0;
@@ -39,6 +39,8 @@ struct DModel {
   // joints
   const int *jnt_type, *jnt_qposadr, *jnt_dofadr, *jnt_bodyid, *jnt_limited;
   const R *jnt_pos, *jnt_axis, *jnt_range, *jnt_margin, *jnt_solref, *jnt_solimp, *qpos0;
+  const int* spr_jnt;                       // the nspr hinge and slide joints with nonzero stiffness
+  const R *jnt_stiffness, *qpos_spring;     // spring force -stiffness (qpos - qpos_spring) on the listed joints
   // dofs
   const int *dof_bodyid, *dof_jntid, *dof_parentid, *dof_kind, *dof_cddstart, *fl_dof, *lim_jnt, *dof_treebase, *dof_treesize, *body_treeid;
   const unsigned long long* body_dofmask;  // bit i set: dof i is on the chain of this body

@@ -279,6 +279,8 @@ def compile_mjcf(xml_string: str, mesh_root: str = None) -> Model:
         B["quat"].append(_orientation(el, use_degree, eulerseq) if bid else np.array([1.0, 0, 0, 0]))
         B["mocap"].append(el.get("mocap", "false") == "true")
         B["inertial"].append(el.find("inertial"))
+        if float(el.get("gravcomp", 0)) != 0:
+            raise NotImplementedError("body gravcomp is not implemented")
         for ch in el:
             if ch.tag in ("joint", "freejoint"):
                 J.append((bid, ch))
@@ -335,6 +337,7 @@ def compile_mjcf(xml_string: str, mesh_root: str = None) -> Model:
     jnt_solimp = np.tile([0.9, 0.95, 0.001, 0.5, 2.0], (njnt, 1))
     dof = dict(body=[], jnt=[], armature=[], damping=[], frictionloss=[], solref=[], solimp=[])
     qpos0 = []
+    qpos_spring = []  # spring reference: springref for hinge and slide joints, qpos0 for free and ball joints
     jnames = []
     nq = nv = 0
     for j, (bid, el) in enumerate(J):
@@ -358,6 +361,10 @@ def compile_mjcf(xml_string: str, mesh_root: str = None) -> Model:
         jnt_limited[j] = 1 if lim == "true" else 0 if lim == "false" else int(autolimits and rng is not None)
         jnt_margin[j] = float(el.get("margin", 0))
         jnt_stiffness[j] = float(el.get("stiffness", 0))
+        if jt == JNT_FREE and jnt_stiffness[j] != 0:
+            raise NotImplementedError("stiffness on a free joint is not implemented")
+        if el.get("springdamper") is not None and np.any(_vec(el.get("springdamper"), 2) != 0):
+            raise NotImplementedError("joint springdamper is not implemented")
         if el.get("solreflimit"):
             jnt_solref[j] = _vec(el.get("solreflimit"), 2)
         if el.get("solimplimit"):
@@ -367,11 +374,15 @@ def compile_mjcf(xml_string: str, mesh_root: str = None) -> Model:
         if jt == JNT_FREE:
             # free joint: only allowed on children of world; qpos0 = body frame
             qpos0 += list(B["pos"][bid]) + list(B["quat"][bid])
+            qpos_spring += qpos0[-7:]
             jnt_pos[j] = 0
         elif jt == JNT_BALL:
             qpos0 += [1.0, 0, 0, 0]
+            qpos_spring += [1.0, 0, 0, 0]
         else:
-            qpos0.append(float(el.get("ref", 0)))
+            deg = math.pi / 180 if use_degree and jt == JNT_HINGE else 1.0  # a hinge's ref and springref are angles
+            qpos0.append(float(el.get("ref", 0)) * deg)
+            qpos_spring.append(float(el.get("springref", 0)) * deg)
         for _ in range(nd):
             dof["body"].append(bid)
             dof["jnt"].append(j)
@@ -388,6 +399,7 @@ def compile_mjcf(xml_string: str, mesh_root: str = None) -> Model:
     m.jnt_margin, m.jnt_stiffness, m.jnt_solref, m.jnt_solimp = jnt_margin, jnt_stiffness, jnt_solref, jnt_solimp
     m.names["joint"] = jnames
     m.qpos0 = np.array(qpos0, dtype=np.float64)
+    m.qpos_spring = np.array(qpos_spring, dtype=np.float64)
     m.dof_bodyid = np.array(dof["body"], dtype=np.int32)
     m.dof_jntid = np.array(dof["jnt"], dtype=np.int32)
     m.dof_armature = np.array(dof["armature"], dtype=np.float64)
@@ -625,6 +637,9 @@ def compile_mjcf(xml_string: str, mesh_root: str = None) -> Model:
     for i, e in enumerate(A):
         anames.append(e.get("name"))
         jn = e.get("joint")
+        for attr, ok in (("dyntype", ("none",)), ("gaintype", ("fixed",)), ("biastype", ("none", "affine"))):
+            if e.get(attr, ok[0]) not in ok:
+                raise NotImplementedError("actuator %s=%s is not implemented" % (attr, e.get(attr)))
         if jn is None:
             raise NotImplementedError("only joint transmissions are implemented")
         m.actuator_trnid[i] = jnames.index(jn)
@@ -906,4 +921,8 @@ def load_model(path: str) -> Model:
             m.names = json.loads(bytes(z[k]).decode())
         else:
             setattr(m, k, z[k])
+    if not hasattr(m, "qpos_spring"):
+        # written before the compiler recorded springref: those compilers sprang every joint back to qpos0, and the packaged
+        # models (robosuite_b200/assets/models) have springref = ref = 0 on every joint
+        m.qpos_spring = np.array(m.qpos0, dtype=np.float64)
     return m

@@ -137,7 +137,7 @@ class BatchedGymWrapper:
 
 # the reference's DEFAULT_DYNAMICS_ARGS (wrappers/domain_randomization_wrapper.py) under the same names.  The knobs the batched engine
 # cannot honour default to False here and raise NotImplementedError when set: local body poses (randomize_position /
-# randomize_quaternion), joint stiffness (the engine has no joint-spring term yet), and the global density / viscosity.
+# randomize_quaternion), joint stiffness (shared by the batch: the engine's springs are not per environment), and the global density / viscosity.
 DEFAULT_DYNAMICS_ARGS = {
     "randomize_density": False, "randomize_viscosity": False,
     "density_perturbation_ratio": 0.1, "viscosity_perturbation_ratio": 0.1,

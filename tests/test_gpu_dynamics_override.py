@@ -97,8 +97,6 @@ def _task_model_and_states(task, n, seed=3):
     env = suite.make(task, robots="Panda", num_envs=n, seed=seed, **({"door_placement": (0.08, 0.0, -np.pi / 2 - 0.125)} if task == "Door" else {}))
     m, q = env.model, env._reset_qpos.double().cpu().numpy().copy()
     env.close()
-    # the engine has no joint-spring term yet (Door's latch has stiffness 1 in the model): the oracles run the same physics without it
-    m.jnt_stiffness = np.zeros_like(m.jnt_stiffness)
     # every free object starts 0.5 mm above the table top instead of the task's 10 mm: a short landing, not a tumble whose corner
     # contacts come and go on last-bit differences
     geoms = _object_geoms(m)
