@@ -195,6 +195,16 @@ int b2s_obs_config(b2s_sim* sim, int obs_dim, const int* op_host, const int* a_h
 enum { B2S_CORRUPT_NONE = 0, B2S_CORRUPT_GAUSSIAN = 1, B2S_CORRUPT_UNIFORM = 2 };
 typedef struct { double period; int corruptor; double p0, p1, low, high; } b2s_obs_mod;
 int b2s_obs_modifiers(b2s_sim* sim, int nobs, const int* row_obs_host, const b2s_obs_mod* mods_host, uint64_t seed);
+/* Per-environment object selection (single_object_mode 1 of PickPlace / NutAssembly: pick_place.py, nut_assembly.py draw one object
+ * at every reset and switch the observables of the others off).  body_ids_host[n] lists 1 to 4 bodies with a free joint; the call
+ * creates "obj_sel" [n_env] i32, zeros at its creation (kept by later calls), which the caller writes (e.g. at a reset).  Observation
+ * and task ops OB_SEL_BODY_POS / OB_SEL_BODY_QUAT_XYZW (b = component, quaternion as x, y, z, w) read body body_ids[obj_sel[env]],
+ * OB_SEL_INDEX reads obj_sel[env] as a real; every path that writes observations evaluates them (b2s_env_step in all three modes,
+ * b2s_forward, b2s_reset_envs).  An environment whose selection is outside [0, n) gets 0 in those rows and warn bit 512; nothing is
+ * read through it.  While a list is configured "obj_sel" is a snapshot section and the list is part of the signature.  n = 0 clears
+ * the list.  B2S_ERR_ARG: n outside [0, 4], a body without a free joint, or n = 0 while the observation or task table uses a
+ * selection op (b2s_obs_config / b2s_task_table in turn refuse such ops while no list is configured). */
+int b2s_obs_objects(b2s_sim* sim, int n, const int* body_ids_host);
 /* Task outputs "task_out" [n_env,8] = (target body height, |site - body|, grasp flag, horizontal |body - body2|,
  * obj-obj2 contact flag, 0, 0, 0) from the poses/contacts of the
  * last step1 (what the reference's reward()/_check_grasp read: manipulation/lift.py:224-273, manipulation_env.py:331-376).
@@ -222,6 +232,7 @@ int b2s_task_table(b2s_sim* sim, int n, const int* op, const int* a, const int* 
  *   b2s_obs_config   obs, obs_fresh (i32), task_out
  *   b2s_obs_modifiers  obs_timer (f64), obs_sampled (i32), obs_nsample (i32), while configured
  *   b2s_task_table   task_vec
+ *   b2s_obs_objects  obj_sel (i32), while a list is configured
  *   overrides        body_xpos_ov:<id> body_xquat_ov:<id> per pose override; geom_{size,friction,rbound,aabb,solref,solimp}:<id> per geom
  *                    slot; body_mass:<id> body_inertia:<id> per body slot; the declared dof vectors; dof_invweight0 body_invweight0
  *                    meaninertia (copied, not recomputed: a snapshot taken while they were stale restores them stale)

@@ -141,6 +141,7 @@ struct b2s_sim {
   ObsModDev* obs_mod_dev = nullptr;
   int obs_arr_n = 0, obs_mod_on = 0;
   double timestep_h = 0;
+  std::vector<char> body_free_h;  // body b has a free joint (b2s_obs_objects takes only such bodies)
 };
 
 // Every entry point picks the handle's precision once: f(DModel<R>&, DState<R>&) runs with R = float or double, and
@@ -725,6 +726,12 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
     s->qpos0.assign(q0, q0 + s->nq);
     const int* sb = b.i32("site_bodyid");
     s->site_bodyid.assign(sb, sb + s->nsite);
+    {
+      int64_t nj = 0;
+      const int* jt = b.i32("jnt_type", &nj); const int* jb = b.i32("jnt_bodyid");
+      s->body_free_h.assign(s->nbody, 0);
+      for (int64_t j = 0; j < nj; j++) if (jt[j] == JNT_FREE && jb[j] >= 0 && jb[j] < s->nbody) s->body_free_h[jb[j]] = 1;
+    }
     for (const char* ty : {"body", "joint", "geom", "site", "actuator", "mesh", "camera", "light"}) {
       std::string key = std::string("names_") + ty;
       if (!b.has(key.c_str())) continue;
@@ -1502,8 +1509,19 @@ int b2s_env_step(b2s_sim* s, const void* action, int nsub) {
   return launch(s, PH_STEP1 | PH_STEP2 | PH_CTRL | (s->has_obs ? PH_OBS : 0) | (s->export_env_step ? PH_EXPORT : 0), nsub, action);
 }
 
+}  // extern "C"
+// whether an op table reads the per-environment object selection (OB_SEL_*)
+static bool uses_selection(const int* op, int n) {
+  for (int k = 0; k < n; k++) if (op[k] == OB_SEL_BODY_POS || op[k] == OB_SEL_BODY_QUAT_XYZW || op[k] == OB_SEL_INDEX) return true;
+  return false;
+}
+static int n_selection(b2s_sim* s) { return s->ctrl.n_sel; }
+extern "C" {
+
 int b2s_obs_config(b2s_sim* s, int obs_dim, const int* op, const int* a, const int* b) {
   if (!s || obs_dim <= 0 || !op || !a || !b) return fail(B2S_ERR_ARG, "b2s_obs_config: bad argument");
+  if (n_selection(s) == 0 && uses_selection(op, obs_dim))
+    return fail(B2S_ERR_ARG, "b2s_obs_config: the table reads the object selection, but no object list is configured (b2s_obs_objects)");
   CUDA_TRY(cudaSetDevice(s->device));
   try {
     std::vector<int> vo(op, op + obs_dim), va(a, a + obs_dim), vb(b, b + obs_dim);
@@ -1591,6 +1609,31 @@ int b2s_obs_modifiers(b2s_sim* s, int nobs, const int* row_obs, const b2s_obs_mo
   return B2S_OK;
 }
 
+int b2s_obs_objects(b2s_sim* s, int n, const int* body_ids) {
+  if (!s) return fail(B2S_ERR_ARG, "null handle");
+  if (n < 0 || n > 4 || (n > 0 && !body_ids)) return fail(B2S_ERR_ARG, "b2s_obs_objects: n must be in [0, 4]");
+  for (int k = 0; k < n; k++)
+    if (body_ids[k] <= 0 || body_ids[k] >= s->nbody || !s->body_free_h[body_ids[k]])
+      return fail(B2S_ERR_ARG, "b2s_obs_objects: body " + std::to_string(body_ids[k]) + " is not a body with a free joint");
+  if (n == 0 && (uses_selection(s->obs_tab_h.data(), s->has_obs ? s->ctrl.obs_dim : 0) ||
+                 uses_selection(s->task_tab_h.data(), s->task_tab_h.empty() ? 0 : s->ctrl.task_dim)))
+    return fail(B2S_ERR_ARG, "b2s_obs_objects: the observation or task table reads the object selection; it cannot be cleared");
+  CUDA_TRY(cudaSetDevice(s->device));
+  int* sel = nullptr;
+  if (n > 0) {
+    try {
+      if (!s->arrays.count("obj_sel")) state_arr_i(s, "obj_sel", 0);  // zeros: every environment starts on the first object
+    } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
+    sel = (int*)s->arrays["obj_sel"].ptr;
+  }
+  s->ctrl.n_sel = n;
+  for (int k = 0; k < 4; k++) s->ctrl.sel_body[k] = k < n ? body_ids[k] : 0;
+  s->ctrl.obj_sel = sel;
+  s->dirty = 1;
+  s->layout_version++;  // the snapshot sections and signature follow the list
+  return B2S_OK;
+}
+
 int b2s_task_config2(b2s_sim* s, int body2, const int* obj2, int no2) {
   if (!s || body2 >= s->nbody) return fail(B2S_ERR_ARG, "b2s_task_config2: bad argument");
   unsigned long long mk = 0;
@@ -1605,6 +1648,8 @@ int b2s_task_config2(b2s_sim* s, int body2, const int* obj2, int no2) {
 
 int b2s_task_table(b2s_sim* s, int n, const int* op, const int* a, const int* b) {
   if (!s || n <= 0 || n > 64 || !op || !a || !b) return fail(B2S_ERR_ARG, "b2s_task_table: bad argument");
+  if (n_selection(s) == 0 && uses_selection(op, n))
+    return fail(B2S_ERR_ARG, "b2s_task_table: the table reads the object selection, but no object list is configured (b2s_obs_objects)");
   CUDA_TRY(cudaSetDevice(s->device));
   try {
     std::vector<int> vo(op, op + n), va(a, a + n), vb(b, b + n);
@@ -1679,6 +1724,7 @@ static int ensure_snap(b2s_sim* s) {
       add("obs_nsample", s->arrays["obs_nsample"].ptr, s->obs_arr_n, B2S_I32);
     }
     if (st.task_vec) add("task_vec", st.task_vec, s->ctrl.task_dim, R);
+    if (s->ctrl.n_sel > 0) add("obj_sel", s->ctrl.obj_sel, 1, B2S_I32);
     for (int k = 0; k < st.n_ov; k++) {
       const std::string id = std::to_string(st.ov_body[k]);
       add("body_xpos_ov:" + id, st.ov_pos[k], 3, R); add("body_xquat_ov:" + id, st.ov_quat[k], 4, R);
@@ -1720,6 +1766,9 @@ static int ensure_snap(b2s_sim* s) {
   h = fnv1a(h, &no, sizeof(int)); h = fnv1a(h, s->obs_tab_h.data(), sizeof(int) * no);
   h = fnv1a(h, &nt, sizeof(int)); h = fnv1a(h, s->task_tab_h.data(), sizeof(int) * nt);
   h = fnv1a(h, &s->blob_hash, sizeof(uint64_t));
+  if (s->ctrl.n_sel > 0) {  // the object list (a handle without one hashes what it always did)
+    h = fnv1a(h, &s->ctrl.n_sel, sizeof(int)); h = fnv1a(h, s->ctrl.sel_body, sizeof(int) * s->ctrl.n_sel);
+  }
   CUDA_TRY(cudaSetDevice(s->device));
   if (!s->snap_dev) {
     try { s->snap_dev = dev_zeros<SnapSec>(s, SNAP_MAXSEC); } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }

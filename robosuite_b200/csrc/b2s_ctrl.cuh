@@ -421,6 +421,14 @@ template <typename R> DEV void mat2quat_wpos(const R* M, R* q) {
 // one scalar of the observation / task tables; `prev` = this environment's previous observation row (lagged entries)
 template <typename R> DEV R table_value(const Eng<R>& e, int op, int a, int b, const R* prev, int fresh) {
   const WSLayout& L = e.lay();
+  if (op >= OB_SEL_BODY_POS) {  // the environment's selected object (b2s_obs_objects): the body's plain op
+    const CtrlCfgDev& cc = e.ccfg();
+    const int k = cc.obj_sel[e.env];
+    if (k < 0 || k >= cc.n_sel) { atomicOr(e.state().warn + e.env, 512); return R(0); }  // nothing is read through a bad selection
+    if (op == OB_SEL_INDEX) return R(k);
+    a = cc.sel_body[k];
+    op = op == OB_SEL_BODY_POS ? OB_BODY_POS : OB_BODY_QUAT_XYZW;
+  }
   R v = 0;
   switch (op) {
     case OB_QPOS: v = e.p(L.qpos)[a]; break;
@@ -586,6 +594,7 @@ template <typename R> DEVN void write_task(const Eng<R> e, int env, int ncon) {
   // task table: poses the task's reward / success checks read after the step (same scalar ops as the observation table)
   for (int k = e.lane; k < cc.task_dim; k += 32)
     s.task_vec[(size_t)env * cc.task_dim + k] = table_value(e, cc.task_op[k], cc.task_a[k], cc.task_b[k], (const R*)nullptr, 0);
+  __syncwarp();  // orders warn bit 512 of a selection op (any lane) before store_state's read-modify-write (lane 0)
 }
 
 // controller.reset_goal + initial joints (osc.py:520-544, controller.py:126-132): goal <- current eef pose (world),

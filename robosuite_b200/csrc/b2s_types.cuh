@@ -174,7 +174,10 @@ enum { OB_QPOS = 0, OB_COS_QPOS, OB_SIN_QPOS, OB_QVEL, OB_QACC, OB_SITE_POS, OB_
        // object pose in the gripper frame from the object pose of the PREVIOUS observation sample (the reference evaluates
        // `{obj}_to_eef_pos/quat` before `{obj}_pos/quat` in the same pass: manipulation_env.py:268-329) and the current
        // hand pose; zeros on the first sample after a reset.  a = pos_slot | quat_slot << 12, b = k | site << 8 | body << 16
-       OB_REL_POS_LAG, OB_REL_QUAT_LAG };
+       OB_REL_POS_LAG, OB_REL_QUAT_LAG,
+       // the environment's selected object (b2s_obs_objects): xpos / xquat (x, y, z, w) component b of body sel_body[obj_sel[env]],
+       // and the selection itself as a real.  A selection outside [0, n_sel) gives 0 and sets warn bit 512
+       OB_SEL_BODY_POS, OB_SEL_BODY_QUAT_XYZW, OB_SEL_INDEX };
 
 // Observable sampling rates and corruptors (b2s_obs_modifiers), kept in device memory (the constant bank is nearly full).  Per
 // observable o: period T = 1 / sampling_rate and the corruptor (kind: B2S_CORRUPT_* of include/b2s.h; p0, p1 = mean, std or
@@ -201,6 +204,8 @@ struct CtrlCfgDev {
   int task_body2; unsigned long long mask_obj2;  // second object (Stack: cubeB), -1 / 0 when unused
   int n_objs; unsigned long long mask_objs[4];   // per-object grasp flags (multi-object tasks)
   int task_dim; const int* task_op; const int* task_a; const int* task_b;  // task table (device arrays)
+  // per-environment object selection (b2s_obs_objects): the OB_SEL_* ops read body sel_body[obj_sel[env]].  n_sel == 0: no list
+  int n_sel, sel_body[4]; int* obj_sel;  // obj_sel: [n_env], in [0, n_sel)
   // JOINT_VELOCITY part controller (controllers/parts/generic/joint_vel.py)
   double jv_kp[8], jv_ki[8], jv_kd[8], jv_in_max[8], jv_in_min[8], jv_out_max[8], jv_out_min[8], jv_vel_lo, jv_vel_hi;
   int jv_use_vel_limits, jv_torque_comp;

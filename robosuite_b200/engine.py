@@ -108,6 +108,7 @@ def lib():
         L.b2s_perturb_model.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64]
         L.b2s_obs_config.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.b2s_obs_modifiers.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(ObsMod), C.c_uint64]
+        L.b2s_obs_objects.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
         L.b2s_task_config.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.b2s_task_config2.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_int]
         L.b2s_task_objects.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
@@ -369,6 +370,14 @@ class BatchedSim:
                                               int(seed) & (2 ** 64 - 1)))
         for name in ("obs_timer", "obs_sampled", "obs_nsample"):  # arrays may have been (re)created
             self._cache.pop(name, None)
+
+    def obs_objects(self, body_ids):
+        """per-environment object selection (b2s_obs_objects): 1 to 4 bodies with a free joint.  Returns the "obj_sel" tensor [n_env]
+        int32 (zeros when first created): the observation / task ops OB_SEL_* of environment e read body body_ids[obj_sel[e]].  An
+        empty list clears the selection (B2SError while a table still reads it) and returns None."""
+        ids = np.ascontiguousarray(body_ids, dtype=np.int32).reshape(-1)
+        self._check(self._L.b2s_obs_objects(self._h, len(ids), ids.ctypes.data if len(ids) else None))
+        return self.array("obj_sel") if len(ids) else None
 
     def task_config(self, body, site, left, right, obj):
         left, right, obj = (np.ascontiguousarray(x, dtype=np.int32) for x in (left, right, obj))

@@ -25,7 +25,7 @@ _ASSETS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "assets
 # observation scalar ops (must match enum OB_* in csrc/b2s_types.cuh)
 OB_QPOS, OB_COS_QPOS, OB_SIN_QPOS, OB_QVEL, OB_QACC, OB_SITE_POS, OB_BODY_POS, OB_BODY_QUAT_XYZW, OB_SITE_QUAT_XYZW, \
     OB_BODY_MINUS_SITE, OB_SITE_MINUS_SITE, OB_BODY_QUAT_REL_SITE_XYZW, OB_ZERO, OB_BODY_MINUS_BODY, OB_REL_POS_LAG, \
-    OB_REL_QUAT_LAG = range(16)
+    OB_REL_QUAT_LAG, OB_SEL_BODY_POS, OB_SEL_BODY_QUAT_XYZW, OB_SEL_INDEX = range(19)
 
 
 def register_env(cls):
@@ -100,7 +100,8 @@ SIM_WARN_BITS = {1: "singular mass matrix", 2: "non-finite state in the integrat
                  128: "invalid model override (non-finite or non-positive size, friction, mass or moment, moments violating the "
                       "triangle inequality, non-finite or negative damping, armature or friction loss, or a non-finite solref / "
                       "solimp component)",
-                 256: "restore source row out of range (b2s_restore): the environment was left untouched"}
+                 256: "restore source row out of range (b2s_restore): the environment was left untouched",
+                 512: "object selection out of range (obj_sel, b2s_obs_objects): the selected-object observation rows were written as 0"}
 
 
 class BatchedMujocoEnv:
@@ -261,7 +262,9 @@ class BatchedMujocoEnv:
         raise NotImplementedError
 
     def _randomize_model(self, mask):
-        """per-reset placements the reference writes into MODEL constants (Door: door.py:417-427); mask: bool [N] on the device or None"""
+        """per-reset draws that live outside qpos, applied to the masked environments before the engine's reset: placements the
+        reference writes into MODEL constants (Door: door.py:417-427) and the drawn object of single_object_mode 1 (PickPlace,
+        NutAssembly); mask: bool [N] on the device or None"""
 
     def reward(self, action=None):
         raise NotImplementedError
@@ -303,6 +306,8 @@ class BatchedMujocoEnv:
         host_mask: the same mask as a numpy bool array when the caller has it (keeps the host mirror of the episode clocks exact)."""
         import torch
 
+        # the two hooks run in this order, both over all num_envs rows: _randomize_model applies to the masked environments what
+        # _sample_reset_state drew besides qpos (single_object_mode 1 hands its object draw over in `_sel_draw`, envs/single_object.py)
         q = self._sample_reset_state(self.num_envs).to(self.dtype).contiguous()
         self._randomize_model(None if mask is None else mask.to(device=self.device).bool())
         if mask is None:

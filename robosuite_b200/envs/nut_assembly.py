@@ -4,23 +4,31 @@ import math
 import numpy as np
 
 from .base import (OB_BODY_POS, OB_BODY_QUAT_XYZW, OB_SITE_POS, BatchedMujocoEnv, load_task_model, register_env)
+from .single_object import SingleObjectMixin, parse_mode, reject_fixed
 
 # models/assets/objects/{square,round}-nut.xml: bottom_site z, horizontal_radius_site (x, y)
 NUT_META = {"SquareNut": dict(bottom=-0.05, hradius=math.hypot(0.11, 0.06)), "RoundNut": dict(bottom=-0.05, hradius=math.hypot(0.11, 0.05))}
 
 
-class _BatchedNutAssembly(BatchedMujocoEnv):
-    """Both nuts are in the model (as in the reference).  single_object_mode 2 (NutAssemblySquare / NutAssemblyRound):
-    the unused nut is moved out of the scene at reset (environments/base.py:591-602 clear_objects -> (10, 10, 10)),
-    where it drops onto the floor plane and rests."""
+class _BatchedNutAssembly(SingleObjectMixin, BatchedMujocoEnv):
+    """Both nuts are in the model (as in the reference).  single_object_mode 2 (NutAssemblySquare / NutAssemblyRound, or
+    nut_type="square" / "round"): the unused nut is moved out of the scene at reset (environments/base.py:591-602 clear_objects ->
+    (10, 10, 10)), where it drops onto the floor plane and rests.  single_object_mode 1 (NutAssemblySingle): one nut per environment,
+    drawn at every reset (envs/single_object.py)."""
 
     table_offset = (0.0, 0.0, 0.82)  # nut_assembly.py:166
     maxcon, maxefc = 96, 288
     nut_names = ("SquareNut", "RoundNut")
     nut_to_id = {"square": 0, "round": 1}
-    single_object_mode = 0
     nut_id = 0
-    _task_state = ("objects_on_pegs",)  # carried by get_env_state / set_env_state
+    _task_state = ("objects_on_pegs",)  # carried by get_env_state / set_env_state (mode 1's selection: by the engine's snapshot)
+
+    def __init__(self, *args, single_object_mode=0, nut_type=None, **kwargs):
+        self.single_object_mode, self._fixed_object = parse_mode(single_object_mode, nut_type, self.nut_to_id, "nut_type")
+        if self._fixed_object is not None:
+            self.nut_id = self._fixed_object
+        self._object_names = self.nut_names
+        super().__init__(*args, **kwargs)
 
     def _load_model(self, xml):
         return load_task_model("NutAssemblyRound", self.robot_name, xml)  # same composed model for all variants
@@ -34,12 +42,15 @@ class _BatchedNutAssembly(BatchedMujocoEnv):
         self.obj_qadr = {n: int(m.jnt_qposadr[jn.index(n + "_joint0")]) for n in self.nut_names}
         self.obj_geom_id = {n: [i for i, g in enumerate(gn) if g and g.startswith(n + "_g") and m.geom_contype[i]] for n in self.nut_names}
         self.object_site_ids = [sn.index(n + "_handle_site") for n in self.nut_names]
-        self.active = [i for i in range(2) if self.single_object_mode == 0 or i == self.nut_id]
+        self.active = [i for i in range(2) if self.single_object_mode != 2 or i == self.nut_id]
         self.objects_on_pegs = None
+        self._setup_selection()
 
     def _setup_observables(self, ob):
         super()._setup_observables(ob)
-        if self.use_object_obs:  # nut_assembly.py:478-580; inactive nuts' sensors are disabled, world_pose_in_gripper is inactive
+        if self.use_object_obs and self.single_object_mode == 1:
+            self._add_selected_object_obs(ob, "nut", "nut_id")
+        elif self.use_object_obs:  # nut_assembly.py:478-580; inactive nuts' sensors are disabled, world_pose_in_gripper is inactive
             for i in self.active:
                 n = self.nut_names[i]
                 b = self.obj_body_id[n]
@@ -73,10 +84,7 @@ class _BatchedNutAssembly(BatchedMujocoEnv):
             y = self.table_offset[1] + (yr[0] + u[:, 1] * (yr[1] - yr[0]))
             z = torch.full((n,), self.table_offset[2] + 0.02 - NUT_META[name]["bottom"], device=dev, dtype=torch.float64)
             self._place_free_body(q, self.obj_qadr[name], x, y, z, u[:, 2] * 2 * math.pi)
-            if i not in self.active:  # clear_objects
-                a = self.obj_qadr[name]
-                q[:, a] = 10.0; q[:, a + 1] = 10.0; q[:, a + 2] = 10.0
-                q[:, a + 3] = 1.0; q[:, a + 4:a + 7] = 0.0
+        self._park_objects(q)  # clear_objects
         return q
 
     def reset(self, mask=None, host_mask=None):
@@ -162,11 +170,25 @@ class BatchedNutAssembly(_BatchedNutAssembly):
     single_object_mode = 0
 
 
-@register_env
-class BatchedNutAssemblySquare(_BatchedNutAssembly):
-    single_object_mode, nut_id = 2, 0
+class _FixedNutAssembly(_BatchedNutAssembly):
+    _mode = _type = None
+
+    def __init__(self, *args, **kwargs):
+        reject_fixed(kwargs, "single_object_mode", "nut_type")
+        super().__init__(*args, single_object_mode=self._mode, nut_type=self._type, **kwargs)
 
 
 @register_env
-class BatchedNutAssemblyRound(_BatchedNutAssembly):
-    single_object_mode, nut_id = 2, 1
+class BatchedNutAssemblySquare(_FixedNutAssembly):
+    _mode, _type = 2, "square"
+
+
+@register_env
+class BatchedNutAssemblyRound(_FixedNutAssembly):
+    _mode, _type = 2, "round"
+
+
+@register_env
+class BatchedNutAssemblySingle(_FixedNutAssembly):
+    """NutAssembly with single_object_mode 1: one nut per environment, drawn at every reset"""
+    _mode = 1

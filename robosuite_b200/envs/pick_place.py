@@ -4,6 +4,7 @@ import math
 import numpy as np
 
 from .base import OB_BODY_POS, OB_BODY_QUAT_XYZW, OB_SITE_POS, BatchedMujocoEnv, load_task_model, register_env
+from .single_object import SingleObjectMixin, parse_mode, reject_fixed
 
 # models/assets/objects/{milk,bread,cereal,can}.xml: bottom_site z, top_site z, horizontal_radius_site (x, y)
 OBJ_META = {
@@ -15,17 +16,30 @@ OBJ_META = {
 
 
 @register_env
-class BatchedPickPlace(BatchedMujocoEnv):
-    """suite.make("PickPlace", robots="Panda", num_envs=N): four objects in bin 1, one target quadrant each in bin 2
-    (single_object_mode 0).  The visual target objects have no physics and are not modelled."""
+class BatchedPickPlace(SingleObjectMixin, BatchedMujocoEnv):
+    """suite.make("PickPlace", robots="Panda", num_envs=N, single_object_mode=0, object_type=None): four objects in bin 1, one
+    target quadrant each in bin 2.  single_object_mode 1 (one object drawn per environment at every reset) and 2 (the object
+    `object_type`: "milk", "bread", "cereal" or "can"): see envs/single_object.py.  The visual target objects have no physics and are
+    not modelled."""
 
     obj_names = ("Milk", "Bread", "Cereal", "Can")
+    object_to_id = {"milk": 0, "bread": 1, "cereal": 2, "can": 3}
     maxcon, maxefc = 64, 224
     tier_small = (12, 56)  # small tail tier: see BatchedMujocoEnv.tier_small
-    _task_state = ("objects_in_bins",)  # carried by get_env_state / set_env_state
+    _task_state = ("objects_in_bins",)  # carried by get_env_state / set_env_state (mode 1's selection: by the engine's snapshot)
+
     bin1_pos = np.array([0.1, -0.25, 0.8])   # pick_place.py:186-187
     bin2_pos = np.array([0.1, 0.28, 0.8])
     bin_size = np.array([0.39, 0.49, 0.82])  # BinsArena table_full_size (pick_place.py:184)
+
+    def __init__(self, *args, single_object_mode=0, object_type=None, **kwargs):
+        self.single_object_mode, self._fixed_object = parse_mode(single_object_mode, object_type, self.object_to_id, "object_type")
+        self._object_names = self.obj_names
+        if self.single_object_mode:
+            # the parked objects resting on the floor add contacts: 13 on average at 4096 environments under random actions, 16 - 17 at
+            # the 99.9th percentile (tools/probe_instr.py on an H100), where (12, 56) left 99.9 % of the environment-substeps to the large tier
+            self.tier_small = (18, 80)
+        super().__init__(*args, **kwargs)
 
     def _load_model(self, xml):
         return load_task_model("PickPlace", self.robot_name, xml)
@@ -48,11 +62,16 @@ class BatchedPickPlace(BatchedMujocoEnv):
             tb[i] = [x + self.bin_size[0] / 4.0, y + self.bin_size[1] / 4.0, self.bin2_pos[2]]
         self.target_bin_placements = tb
         self.objects_in_bins = None
+        self._setup_selection()
 
     def _setup_observables(self, ob):
         super()._setup_observables(ob)
-        if self.use_object_obs:  # pick_place.py:585-685
-            for n in self.obj_names:
+        if self.use_object_obs and self.single_object_mode == 1:
+            self._add_selected_object_obs(ob, "obj", "obj_id")
+        elif self.use_object_obs:  # pick_place.py:585-685; mode 2: the fixed object's observables only
+            for i, n in enumerate(self.obj_names):
+                if self.single_object_mode == 2 and i != self._fixed_object:
+                    continue
                 b = self.obj_body_id[n]
                 ob.add_rel_pose(n, self.eef_site_id, self.eef_body_id, "object")
                 ob.add(n + "_pos", "object", [(OB_BODY_POS, b, k) for k in range(3)])
@@ -98,6 +117,7 @@ class BatchedPickPlace(BatchedMujocoEnv):
             yaw = torch.rand((n,), generator=self.rng, device=dev, dtype=torch.float64) * 2 * math.pi
             self._place_free_body(q, self.obj_qadr[name], x, y, torch.full((n,), z, device=dev, dtype=torch.float64), yaw)
             placed.append((x, y, z, meta))
+        self._park_objects(q)
         return q
 
     def reset(self, mask=None, host_mask=None):
@@ -137,7 +157,8 @@ class BatchedPickPlace(BatchedMujocoEnv):
 
     def _check_success(self):
         self._update_in_bins()
-        return self.objects_in_bins.sum(dim=1) == 4
+        n = self.objects_in_bins.sum(dim=1)
+        return n > 0 if self.single_object_mode > 0 else n == 4
 
     def staged_rewards(self):
         import torch
@@ -177,5 +198,40 @@ class BatchedPickPlace(BatchedMujocoEnv):
         if self.reward_shaping:
             r = r + torch.stack(self.staged_rewards(), dim=1).max(dim=1).values.to(self.dtype)
         if self.reward_scale is not None:
-            r = r * self.reward_scale / 4.0
+            r = r * self.reward_scale / 4.0 if self.single_object_mode == 0 else r * self.reward_scale
         return r
+
+
+class _FixedPickPlace(BatchedPickPlace):
+    _mode = _type = None
+
+    def __init__(self, *args, **kwargs):
+        reject_fixed(kwargs, "single_object_mode", "object_type")
+        super().__init__(*args, single_object_mode=self._mode, object_type=self._type, **kwargs)
+
+
+@register_env
+class BatchedPickPlaceSingle(_FixedPickPlace):
+    """PickPlace with single_object_mode 1: one object per environment, drawn at every reset"""
+    _mode = 1
+
+
+@register_env
+class BatchedPickPlaceMilk(_FixedPickPlace):
+    _mode, _type = 2, "milk"
+
+
+@register_env
+class BatchedPickPlaceBread(_FixedPickPlace):
+    _mode, _type = 2, "bread"
+
+
+@register_env
+class BatchedPickPlaceCereal(_FixedPickPlace):
+    _mode, _type = 2, "cereal"
+
+
+@register_env
+class BatchedPickPlaceCan(_FixedPickPlace):
+    """the "Can" task of the robomimic benchmarks"""
+    _mode, _type = 2, "can"
