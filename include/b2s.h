@@ -260,6 +260,17 @@ int b2s_restore(b2s_sim* sim, const void* rows_dev, int n_rows, const int* src_r
  * the throughput path switches it off so that per-step HBM traffic is state + action + obs only */
 int b2s_set_export(b2s_sim* sim, int flag);
 
+/* Contact geometry without the full export (what check_contact / get_contacts / _check_grasp read from data.contact after
+ * env.step, utils/sim_utils.py, manipulation_env.py).  flag != 0 (default 0): the LAST substep of every b2s_env_step / b2s_step call
+ * writes ncon [n_env] and contact_geom [n_env, maxcon, 2], contact_dim, contact_dist, contact_pos [.., 3], contact_frame [.., 9] and
+ * contact_friction [.., 3]: the contacts of that substep's step1 in static-pair order (data.contact[:ncon] after mj_step with
+ * lite_physics), rows ncon .. maxcon - 1 with geom -1 and zeros.  All three schedules write the same bits, so b2s_env_step keeps the
+ * handle's mode (b2s_set_export = 1, which also writes these arrays, still runs the fused kernel).  The arrays are valid once the
+ * call's work on the handle's stream is done.  b2s_reset_envs writes the forward pass's contacts of the masked environments (with or
+ * without the flag, as b2s_forward does for all); after b2s_restore they are stale until the next step, like the other derived
+ * arrays.  They are not a snapshot section, and neither they nor the flag are part of the signature.  B2S_ERR_ARG: null handle. */
+int b2s_set_contact_export(b2s_sim* sim, int flag);
+
 /* Scheduling of b2s_env_step / b2s_step: 0 = fused (one kernel per call, state resident in shared memory for all
  * substeps), 1 = pipeline (per substep and environment group: phase 0, phase 1 (narrow phase + controller), the tail kernel and,
  * when the model has a small tail tier, its large-tier re-run, exchanging a workspace row through L2; one CUDA graph per group,

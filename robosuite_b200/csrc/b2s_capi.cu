@@ -806,6 +806,13 @@ int b2s_set_stream(b2s_sim* s, void* stream) {
 
 int b2s_set_export(b2s_sim* s, int flag) { if (!s) return fail(B2S_ERR_ARG, "null handle"); s->export_env_step = flag != 0; return B2S_OK; }
 
+int b2s_set_contact_export(b2s_sim* s, int flag) {
+  if (!s) return fail(B2S_ERR_ARG, "null handle");
+  with_real(s, [&](auto&, auto& st) { st.export_con = flag != 0; return 0; });
+  s->dirty = 1;
+  return B2S_OK;
+}
+
 int64_t b2s_launch_count(const b2s_sim* s) { return s ? s->launches : 0; }
 
 int b2s_array(b2s_sim* s, const char* name, void** dev_ptr, int* dtype, int* ndim, int64_t shape[4]) {

@@ -26,6 +26,35 @@ template <typename R> DEV void store_state(const Eng<R>& e, int env, R time, int
 }
 
 
+// The contacts of this substep's step1 -> contact_* / ncon, in static-pair order; rows ncon .. maxcon - 1 get geom -1 and zeros.
+// Reads only the contact regions of the workspace, which hold the gathered contacts from collide (fused) or gather_contacts (tail)
+// until the next substep: the constraint stage and the solve only read them, and no late load overlays them (layout_tail).
+// Compiled once per precision and called by every schedule, so all three write the same bits.
+template <typename R>
+DEVN void export_contacts(const Eng<R> e, int env, int ncon) {
+  const DModel<R>& m = e.model();
+  const WSLayout& L = e.lay();
+  const DState<R>& s = e.state();
+  int lane = e.lane;
+  size_t E = env;
+  const int* cint = e.pi(L.c_int);
+  for (int c = lane; c < m.maxcon; c += 32) {
+    bool v = c < ncon;
+    s.contact_geom[(E * m.maxcon + c) * 2] = v ? cint[5 * c] : -1;
+    s.contact_geom[(E * m.maxcon + c) * 2 + 1] = v ? cint[5 * c + 1] : -1;
+    s.contact_dim[E * m.maxcon + c] = v ? cint[5 * c + 2] : 0;
+    s.contact_dist[E * m.maxcon + c] = v ? e.p(L.c_dist)[c] : R(0);
+    for (int q = 0; q < 3; q++) s.contact_pos[(E * m.maxcon + c) * 3 + q] = v ? e.p(L.c_pos)[3 * c + q] : R(0);
+    {
+      R f9[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
+      if (v) { f9[0] = e.p(L.c_frame)[3 * c]; f9[1] = e.p(L.c_frame)[3 * c + 1]; f9[2] = e.p(L.c_frame)[3 * c + 2]; make_frame(f9); }
+      for (int q = 0; q < 9; q++) s.contact_frame[(E * m.maxcon + c) * 9 + q] = f9[q];
+    }
+    for (int q = 0; q < 3; q++) s.contact_friction[(E * m.maxcon + c) * 3 + q] = v ? e.p(L.c_fric)[3 * c + q] : R(0);
+  }
+  if (lane == 0) s.ncon[env] = ncon;
+}
+
 template <typename R>
 DEVN void export_step1(const Eng<R> e, int env, int ncon) {
   const DModel<R>& m = e.model();
@@ -47,22 +76,7 @@ DEVN void export_step1(const Eng<R> e, int env, int ncon) {
   load_row(s.cdof + E * 6 * m.nv, e.p(L.cdof), 6 * m.nv, lane);
   load_row(s.qfrc_bias + E * m.nv, e.p(L.bias), m.nv, lane);
   load_row(s.qfrc_passive + E * m.nv, e.p(L.passive), m.nv, lane);
-  const int* cint = e.pi(L.c_int);
-  for (int c = lane; c < m.maxcon; c += 32) {
-    bool v = c < ncon;
-    s.contact_geom[(E * m.maxcon + c) * 2] = v ? cint[5 * c] : -1;
-    s.contact_geom[(E * m.maxcon + c) * 2 + 1] = v ? cint[5 * c + 1] : -1;
-    s.contact_dim[E * m.maxcon + c] = v ? cint[5 * c + 2] : 0;
-    s.contact_dist[E * m.maxcon + c] = v ? e.p(L.c_dist)[c] : R(0);
-    for (int q = 0; q < 3; q++) s.contact_pos[(E * m.maxcon + c) * 3 + q] = v ? e.p(L.c_pos)[3 * c + q] : R(0);
-    {
-      R f9[9] = {0, 0, 0, 0, 0, 0, 0, 0, 0};
-      if (v) { f9[0] = e.p(L.c_frame)[3 * c]; f9[1] = e.p(L.c_frame)[3 * c + 1]; f9[2] = e.p(L.c_frame)[3 * c + 2]; make_frame(f9); }
-      for (int q = 0; q < 9; q++) s.contact_frame[(E * m.maxcon + c) * 9 + q] = f9[q];
-    }
-    for (int q = 0; q < 3; q++) s.contact_friction[(E * m.maxcon + c) * 3 + q] = v ? e.p(L.c_fric)[3 * c + q] : R(0);
-  }
-  if (lane == 0) s.ncon[env] = ncon;
+  export_contacts(e, env, ncon);
 }
 
 // constraint rows (the Jacobian overlays kinematics scratch, so this runs after make_constraint)
@@ -152,6 +166,7 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
       __syncthreads();
       ncon = collide(e, warn);
       if (ex) export_step1(e, env, ncon);
+      else if (live && s.export_con && sub == nsub - 1) export_contacts(e, env, ncon);
       __syncthreads();
       nefc = make_constraint(e, ncon, warn);
       if (ex) export_efc(e, env, nefc);

@@ -355,11 +355,15 @@ template <typename R> DEV int tail_newton(Eng<R>& e, int nefc, int ncon, int* ni
   return warn;
 }
 
-// Finish: Euler, the rows of the observables that sample on this substep (obs_due: all of them on the last substep without
-// modifiers), on the last substep of a control step the task rows, state write-back.
+// Finish: on the last substep of the call the contact records (b2s_set_contact_export), Euler, the rows of the observables that
+// sample on this substep (obs_due: all of them on the last substep without modifiers), on the last substep of a control step the
+// task rows, state write-back.  Only the tier that finishes the environment gets here: a small-tier overflow returned before touching
+// anything.
 template <typename R>
 DEV void tail_finish(Eng<R>& e, int env, int sub, int nsub, int phases, int ncon, int warn, unsigned long long* bar, unsigned& parity) {
   const DState<R>& s = e.state();
+  // first in the stage (after the call the caller keeps fewer values live than at the end: measured with -Xptxas -v)
+  if (s.export_con && sub == nsub - 1) export_contacts(e, env, ncon);
   e.env = env;  // Euler reads the environment's damping
   R time = s.time[env];
   if (!(phases & PH_NOINTEGRATE)) {

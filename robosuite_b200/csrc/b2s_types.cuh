@@ -126,6 +126,7 @@ struct DState {
   int* solve_ls;   // [n_env] line-search evaluations of the environment's last Newton solve
   int* slowlog;    // [64][12] convex work items above 131 k cycles: cycles, shape types, hull sizes, EPA nV nF, GJK cycles, hit, staged, geoms
   const struct ObsModDev* obs_mod;  // sampling rates and corruptors (b2s_obs_modifiers); null: every observable on the last substep, no noise
+  int export_con;  // b2s_set_contact_export: the last substep of a step call writes contact_* / ncon in every schedule
 };
 
 // offsets (in units of R) of the per-warp shared-memory workspace

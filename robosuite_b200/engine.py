@@ -114,6 +114,7 @@ def lib():
         L.b2s_task_objects.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]
         L.b2s_task_table.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.b2s_set_export.argtypes = [C.c_void_p, C.c_int]
+        L.b2s_set_contact_export.argtypes = [C.c_void_p, C.c_int]
         L.b2s_set_mode.argtypes = [C.c_void_p, C.c_int]
         L.b2s_launch_count.argtypes = [C.c_void_p]
         L.b2s_launch_count.restype = C.c_int64
@@ -403,6 +404,18 @@ class BatchedSim:
     def set_export(self, flag):
         """whether b2s_env_step also writes the derived arrays (xpos, contacts, ...) of its last substep to HBM"""
         self._check(self._L.b2s_set_export(self._h, int(bool(flag))))
+
+    def set_contact_export(self, flag):
+        """whether the last substep of every env_step / step writes the contact arrays (contacts()) in every mode, without the
+        rest of the derived-array export (b2s_set_contact_export)"""
+        self._check(self._L.b2s_set_contact_export(self._h, int(bool(flag))))
+
+    def contacts(self):
+        """device views of the contacts of the last substep: "ncon" [N], "geom" [N, maxcon, 2] (-1 beyond ncon), "dist"
+        [N, maxcon], "pos" [N, maxcon, 3], "frame" [N, maxcon, 9] (normal first) and "friction" [N, maxcon, 3].  Written by
+        env_step / step with set_contact_export(True) or set_export(True), and by forward / reset_envs (masked environments)"""
+        return {k: self.array(a) for k, a in (("ncon", "ncon"), ("geom", "contact_geom"), ("dist", "contact_dist"),
+                                              ("pos", "contact_pos"), ("frame", "contact_frame"), ("friction", "contact_friction"))}
 
     def set_mode(self, mode):
         """0 = fused single kernel, 1 = pipelined phase kernels, 2 = unit queue (one persistent kernel per control step);

@@ -18,6 +18,7 @@ import numpy as np
 from .. import controller_config as cc
 from ..engine import BatchedSim, CtrlCfg
 from ..mjcf.compiler import Model, compile_mjcf, load_model
+from .contacts import ContactQueries
 
 REGISTERED_ENVS = {}
 _ASSETS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "assets", "models")
@@ -104,8 +105,10 @@ SIM_WARN_BITS = {1: "singular mass matrix", 2: "non-finite state in the integrat
                  512: "object selection out of range (obj_sel, b2s_obs_objects): the selected-object observation rows were written as 0"}
 
 
-class BatchedMujocoEnv:
-    """N copies of one task on one GPU.  All returned arrays are torch.cuda tensors with leading dim N."""
+class BatchedMujocoEnv(ContactQueries):
+    """N copies of one task on one GPU.  All returned arrays are torch.cuda tensors with leading dim N.
+    contact_queries=True switches the contact export on (BatchedSim.set_contact_export) before the first reset, so that
+    check_contact / get_contacts / _check_grasp (envs/contacts.py) can read the contacts of the last substep."""
 
     maxcon = None  # per-environment contact / constraint-row capacity (None: engine defaults 32 / 64); overflow sets warn bit 4
     maxefc = None
@@ -120,7 +123,7 @@ class BatchedMujocoEnv:
                  ignore_done=False, reward_scale=1.0, reward_shaping=False, use_object_obs=True, seed=None,
                  initialization_noise="default", precision="f32", xml=None, has_renderer=False,
                  has_offscreen_renderer=False, use_camera_obs=False, hard_reset=False, lite_physics=True, model=None,
-                 kernel_mode="pipeline", sim_cls=None, **kwargs):
+                 kernel_mode="pipeline", sim_cls=None, contact_queries=False, **kwargs):
         import torch
 
         if has_renderer or has_offscreen_renderer or use_camera_obs:
@@ -164,6 +167,9 @@ class BatchedMujocoEnv:
         self.sim.obs_config(op, a, b)
         self._setup_task()
         self.sim.set_export(False)
+        self._contact_queries = bool(contact_queries)
+        if self._contact_queries:
+            self.sim.set_contact_export(True)
         # "pipeline": phase kernels + global collision work lists (fastest in steady state); "fused": one kernel per step
         self.sim.set_mode(1 if kernel_mode == "pipeline" else 0)
         self.rng = torch.Generator(device=self.device)
