@@ -64,15 +64,16 @@ int b2s_set_state(b2s_sim* sim, const void* in_dev);
 int b2s_name2id(const b2s_sim* sim, const char* type, const char* name);
 const char* b2s_id2name(const b2s_sim* sim, const char* type, int id);
 /* mj_fullM (controllers/parts/controller.py:226-229 builds the dense mass matrix from qM): out_dev [n_env, nv, nv], valid after
- * b2s_forward / b2s_step1 */
+ * b2s_forward / b2s_step1, and after b2s_env_step / b2s_step with b2s_set_export or b2s_set_step1_export on */
 int b2s_full_m(b2s_sim* sim, void* out_dev);
 /* MjData.get_body_jacp/jacr, get_geom_jacp/jacr (binding_utils.py:853-878 and the geom variants): Jacobian of the body frame origin /
- * geom centre, [n_env, 3, nv] device buffers (either may be NULL), valid after b2s_forward / b2s_step1 */
+ * geom centre (a colliding geom: the others have no pose), [n_env, 3, nv] device buffers (either may be NULL), valid after
+ * b2s_forward / b2s_step1, and after b2s_env_step / b2s_step with b2s_set_export or b2s_set_step1_export on */
 int b2s_jac_body(b2s_sim* sim, int body_id, void* jacp, void* jacr);
 int b2s_jac_geom(b2s_sim* sim, int geom_id, void* jacp, void* jacr);
 
 /* MjData.get_site_jacp/jacr (binding_utils.py:826-852): jacp/jacr are [n_env,3,nv] device buffers (either may be NULL);
- * valid after b2s_forward/b2s_step1. */
+ * valid after b2s_forward/b2s_step1, and after b2s_env_step / b2s_step with b2s_set_export or b2s_set_step1_export on. */
 int b2s_jac_site(b2s_sim* sim, int site_id, void* jacp, void* jacr);
 
 /* Fused control step = MujocoEnv.step's substep loop (environments/base.py:494-505):
@@ -270,6 +271,20 @@ int b2s_set_export(b2s_sim* sim, int flag);
  * without the flag, as b2s_forward does for all); after b2s_restore they are stale until the next step, like the other derived
  * arrays.  They are not a snapshot section, and neither they nor the flag are part of the signature.  B2S_ERR_ARG: null handle. */
 int b2s_set_contact_export(b2s_sim* sim, int flag);
+
+/* The step-1 arrays without the full export (what reward / success code, controllers and safety filters read from sim.data after
+ * env.step: body_xpos, get_site_xpos / xmat, get_site_jacp / jacr, mj_fullM).  flag != 0 (default 0): the LAST substep of every
+ * b2s_env_step / b2s_step call writes xpos [n_env, nbody, 3], xquat [.., 4], xmat [.., 9], site_xpos [n_env, nsite, 3], site_xmat
+ * [.., 9], geom_xpos [n_env, ngeom, 3] / geom_xmat [.., 9] of the colliding geoms, qM [n_env, nv, nv], cdof [n_env, nv, 6],
+ * qfrc_bias [n_env, nv] and qfrc_passive [n_env, nv]: the values of that substep's step1 (mj_step's position and velocity stages),
+ * the same bits in all three schedules, so b2s_env_step keeps the handle's mode (b2s_set_export = 1, which also writes these arrays,
+ * still runs the fused kernel).  The poses of non-colliding (visual) geoms are never computed: their rows keep whatever they held.
+ * The arrays are valid once the call's work on the handle's stream is done, and b2s_jac_site / b2s_jac_body / b2s_jac_geom and
+ * b2s_full_m, which read them, are then valid too.  b2s_reset_envs writes them for the masked environments (with or without the
+ * flag, through its forward pass, as b2s_forward does for all); after b2s_restore they are stale until the next step, like the
+ * other derived arrays.  They are not a snapshot section, and neither they nor the flag are part of the signature.  The step-2
+ * arrays (qfrc_actuator, qfrc_constraint, actuator_force, efc_*) still come with b2s_set_export only.  B2S_ERR_ARG: null handle. */
+int b2s_set_step1_export(b2s_sim* sim, int flag);
 
 /* Scheduling of b2s_env_step / b2s_step: 0 = fused (one kernel per call, state resident in shared memory for all
  * substeps), 1 = pipeline (per substep and environment group: phase 0, phase 1 (narrow phase + controller), the tail kernel and,

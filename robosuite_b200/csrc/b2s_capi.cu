@@ -813,6 +813,13 @@ int b2s_set_contact_export(b2s_sim* s, int flag) {
   return B2S_OK;
 }
 
+int b2s_set_step1_export(b2s_sim* s, int flag) {
+  if (!s) return fail(B2S_ERR_ARG, "null handle");
+  with_real(s, [&](auto&, auto& st) { st.export_kin = flag != 0; return 0; });
+  s->dirty = 1;
+  return B2S_OK;
+}
+
 int64_t b2s_launch_count(const b2s_sim* s) { return s ? s->launches : 0; }
 
 int b2s_array(b2s_sim* s, const char* name, void** dev_ptr, int* dtype, int* ndim, int64_t shape[4]) {
@@ -896,7 +903,8 @@ static int enqueue_group(b2s_sim* s, const DModel<R>& m, const DState<R>& st, in
   CUDA_TRY(cudaMemsetAsync(st.cl_cnt + CL_CNT_STRIDE * gi, 0, CL_CNT_STRIDE * sizeof(int), q));
   for (int sub = 0; sub < nsub; sub++) {
     g.sub = sub;
-    phase0_kernel<R><<<blocks0, s->wpb0 * 32, s->smem0, q>>>(phases, g);
+    // the last substep's node is marked whatever the step-1 export flag: the kernel reads the flag, so the graph stays valid when it changes
+    phase0_kernel<R><<<blocks0, s->wpb0 * 32, s->smem0, q>>>(sub == nsub - 1 ? phases | PH_LAST_SUB : phases, g);
     // phase 1: convex narrow phase | controller | analytic narrow phase as block roles of ONE launch (no forks in the graph).
     // Upper bounds of the candidate counts size the grid; warps / threads beyond the device-side counts exit at once.
     P1Cfg c{std::min(nG, cvx_blocks), ctrl_ext ? (g.nenv + OSC_TPB - 1) / OSC_TPB : 0, sub};

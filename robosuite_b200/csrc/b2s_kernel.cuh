@@ -55,8 +55,13 @@ DEVN void export_contacts(const Eng<R> e, int env, int ncon) {
   if (lane == 0) s.ncon[env] = ncon;
 }
 
+// The step-1 arrays of this substep -> xpos, xquat, xmat, site_xpos, site_xmat, geom_xpos / geom_xmat of the colliding geoms (the
+// others are never computed), qM, cdof, qfrc_bias, qfrc_passive.  Reads the workspace regions kinematics, velocity and crb wrote;
+// the fused kernel calls it after collide (whose candidate lists live in the scratch region), phase 0 after publishing its row (its
+// layout gives every one of these regions its own words; M over frne / ffl is written by crb after their last use).  Compiled once
+// per precision and called by every schedule, so all three write the same bits.
 template <typename R>
-DEVN void export_step1(const Eng<R> e, int env, int ncon) {
+DEVN void export_kinematics(const Eng<R> e, int env) {
   const DModel<R>& m = e.model();
   const WSLayout& L = e.lay();
   const DState<R>& s = e.state();
@@ -76,6 +81,11 @@ DEVN void export_step1(const Eng<R> e, int env, int ncon) {
   load_row(s.cdof + E * 6 * m.nv, e.p(L.cdof), 6 * m.nv, lane);
   load_row(s.qfrc_bias + E * m.nv, e.p(L.bias), m.nv, lane);
   load_row(s.qfrc_passive + E * m.nv, e.p(L.passive), m.nv, lane);
+}
+
+template <typename R>
+DEVN void export_step1(const Eng<R> e, int env, int ncon) {
+  export_kinematics(e, env);
   export_contacts(e, env, ncon);
 }
 
@@ -166,7 +176,10 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
       __syncthreads();
       ncon = collide(e, warn);
       if (ex) export_step1(e, env, ncon);
-      else if (live && s.export_con && sub == nsub - 1) export_contacts(e, env, ncon);
+      else if (live && sub == nsub - 1) {
+        if (s.export_kin) export_kinematics(e, env);
+        if (s.export_con) export_contacts(e, env, ncon);
+      }
       __syncthreads();
       nefc = make_constraint(e, ncon, warn);
       if (ex) export_efc(e, env, nefc);

@@ -396,7 +396,8 @@ constexpr int P0_THREADS = 256, P0_BLOCKS = 2;      // phase 0
 constexpr int TAIL_THREADS = 256, TAIL_BLOCKS = 2;  // tail kernel, two blocks per SM
 constexpr int TAIL_WIDE_THREADS = 512;              // tail kernel, one block per SM
 
-// ---- phase 0: kinematics, velocity stage + RNE bias, CRB -> M, broad phase -> global candidate work lists
+// ---- phase 0: kinematics, velocity stage + RNE bias, CRB -> M, broad phase -> global candidate work lists; with PH_LAST_SUB in
+// `phases` and b2s_set_step1_export, the step-1 arrays
 template <typename R>
 __global__ void __launch_bounds__(P0_THREADS, P0_BLOCKS) phase0_kernel(int phases, Grp g) {
   const DState<R>& s = cstate<R>(g.slot);
@@ -427,6 +428,8 @@ __global__ void __launch_bounds__(P0_THREADS, P0_BLOCKS) phase0_kernel(int phase
   baseA = __shfl_sync(B2S_FULL, baseA, 0);
   baseG = __shfl_sync(B2S_FULL, baseG, 0);
   phase0_publish(e, env, na, ng, warn, baseA, baseG, true);
+  // the call's last substep (its graph node carries PH_LAST_SUB): the step-1 arrays, last in the kernel, where the fewest values are live
+  if ((phases & PH_LAST_SUB) && s.export_kin) export_kinematics(e, env);
 #ifdef B2S_INSTR
   if (lane == 0 && s.cyc) s.cyc[((size_t)env * 32 + (g.sub & 31)) * 8] = (float)(clock64() - instr_t0);
 #endif

@@ -22,6 +22,7 @@ enum {
   PH_EXPORT = 8,     // write derived arrays (xpos, qM, contacts, efc ...) to HBM
   PH_CTRL = 16,      // run the fused controller between step1 and step2
   PH_CTRL_EXT = 512, // pipeline mode: the controller ran as its own kernel (ctrl_osc_kernel), `ctrl` is already in HBM
+  PH_LAST_SUB = 1024,  // pipeline mode: this phase-0 node is the call's last substep (b2s_set_step1_export)
   PH_OBS = 64        // write the observation row and the task outputs (after the last substep)
 };
 
@@ -127,6 +128,7 @@ struct DState {
   int* slowlog;    // [64][12] convex work items above 131 k cycles: cycles, shape types, hull sizes, EPA nV nF, GJK cycles, hit, staged, geoms
   const struct ObsModDev* obs_mod;  // sampling rates and corruptors (b2s_obs_modifiers); null: every observable on the last substep, no noise
   int export_con;  // b2s_set_contact_export: the last substep of a step call writes contact_* / ncon in every schedule
+  int export_kin;  // b2s_set_step1_export: the last substep of a step call writes the step-1 arrays (export_kinematics) in every schedule
 };
 
 // offsets (in units of R) of the per-warp shared-memory workspace

@@ -54,13 +54,15 @@ template <typename R> __global__ void unit_check_kernel(UnitQ q, int slot) {
 // rounds of the small role put block barriers between them, and a kernel body that inlines all of it is the kind of function nvcc 12.9
 // has mis-allocated before (DESIGN.md section 3).
 
-// phase 0; the environment owns fixed output slots: analytic candidate i -> env * cl_maxa + i, convex candidate i -> env * cl_maxg + i
-template <typename R> DEVN int unit_phase0(R* area, int lane, int slot, int env) {
+// phase 0; the environment owns fixed output slots: analytic candidate i -> env * cl_maxa + i, convex candidate i -> env * cl_maxg + i.
+// On the call's last substep (`last`) with b2s_set_step1_export, then the step-1 arrays, as in phase0_kernel.
+template <typename R> DEVN int unit_phase0(R* area, int lane, int slot, int env, bool last) {
   const DState<R>& s = cstate<R>(slot);
   Eng<R> e(area, lane, slot, LAY_P0);
   int na, ng;
   const int warn = phase0_env(e, env, na, ng);
   phase0_publish(e, env, na, ng, warn, env * s.cl_maxa, env * s.cl_maxg, false);
+  if (last && s.export_kin) export_kinematics(e, env);
   return na | (ng << 16);
 }
 
@@ -257,7 +259,7 @@ __global__ void __launch_bounds__(UNIT_THREADS, UNIT_BLOCKS) unit_kernel(int pha
     __syncthreads();
     UTICK(1)
     int nn = 0;
-    if (live) nn = unit_phase0<R>(area, lane, slot, env);
+    if (live) nn = unit_phase0<R>(area, lane, slot, env, sub == nsub - 1);
     __syncthreads();
     UTICK(2)
     if (live) unit_narrow<R>(area, q.stride, lane, slot, env, nn & 0xffff, nn >> 16);

@@ -115,6 +115,7 @@ def lib():
         L.b2s_task_table.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.b2s_set_export.argtypes = [C.c_void_p, C.c_int]
         L.b2s_set_contact_export.argtypes = [C.c_void_p, C.c_int]
+        L.b2s_set_step1_export.argtypes = [C.c_void_p, C.c_int]
         L.b2s_set_mode.argtypes = [C.c_void_p, C.c_int]
         L.b2s_launch_count.argtypes = [C.c_void_p]
         L.b2s_launch_count.restype = C.c_int64
@@ -220,6 +221,8 @@ class BatchedSim:
         self._L = lib()
         self._check(self._L.b2s_create(blob, len(blob), self.n_env, self.device, self.precision, C.byref(self._h)))
         self._cache = {}
+        self.full_export = True     # set_export (the library's default)
+        self.step1_export = False  # set_step1_export
         global _LIVE
         if _LIVE is None:
             import weakref
@@ -404,6 +407,24 @@ class BatchedSim:
     def set_export(self, flag):
         """whether b2s_env_step also writes the derived arrays (xpos, contacts, ...) of its last substep to HBM"""
         self._check(self._L.b2s_set_export(self._h, int(bool(flag))))
+        self.full_export = bool(flag)
+
+    def set_step1_export(self, flag):
+        """whether the last substep of every env_step / step writes the step-1 arrays (xpos, xquat, xmat, site / colliding-geom
+        poses, qM, cdof, qfrc_bias, qfrc_passive: what `data` reads) in every mode, without the rest of the derived-array export
+        (b2s_set_step1_export)"""
+        self._check(self._L.b2s_set_step1_export(self._h, int(bool(flag))))
+        self.step1_export = bool(flag)
+
+    @property
+    def data(self):
+        """the batched MjData view of the step-1 arrays (robosuite_b200/data.py); after env_step / step it needs
+        set_step1_export(True) or set_export(True)"""
+        if "_data" not in self.__dict__:
+            from .data import BatchedData
+
+            self._data = BatchedData(self)
+        return self._data
 
     def set_contact_export(self, flag):
         """whether the last substep of every env_step / step writes the contact arrays (contacts()) in every mode, without the

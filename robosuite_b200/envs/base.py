@@ -108,7 +108,9 @@ SIM_WARN_BITS = {1: "singular mass matrix", 2: "non-finite state in the integrat
 class BatchedMujocoEnv(ContactQueries):
     """N copies of one task on one GPU.  All returned arrays are torch.cuda tensors with leading dim N.
     contact_queries=True switches the contact export on (BatchedSim.set_contact_export) before the first reset, so that
-    check_contact / get_contacts / _check_grasp (envs/contacts.py) can read the contacts of the last substep."""
+    check_contact / get_contacts / _check_grasp (envs/contacts.py) can read the contacts of the last substep.  data_queries=True
+    does the same for the step-1 arrays (BatchedSim.set_step1_export), so that sim.data (robosuite_b200/data.py) reads the poses,
+    Jacobians and mass matrices of the last substep."""
 
     maxcon = None  # per-environment contact / constraint-row capacity (None: engine defaults 32 / 64); overflow sets warn bit 4
     maxefc = None
@@ -123,7 +125,7 @@ class BatchedMujocoEnv(ContactQueries):
                  ignore_done=False, reward_scale=1.0, reward_shaping=False, use_object_obs=True, seed=None,
                  initialization_noise="default", precision="f32", xml=None, has_renderer=False,
                  has_offscreen_renderer=False, use_camera_obs=False, hard_reset=False, lite_physics=True, model=None,
-                 kernel_mode="pipeline", sim_cls=None, contact_queries=False, **kwargs):
+                 kernel_mode="pipeline", sim_cls=None, contact_queries=False, data_queries=False, **kwargs):
         import torch
 
         if has_renderer or has_offscreen_renderer or use_camera_obs:
@@ -170,6 +172,8 @@ class BatchedMujocoEnv(ContactQueries):
         self._contact_queries = bool(contact_queries)
         if self._contact_queries:
             self.sim.set_contact_export(True)
+        if data_queries:
+            self.sim.set_step1_export(True)
         # "pipeline": phase kernels + global collision work lists (fastest in steady state); "fused": one kernel per step
         self.sim.set_mode(1 if kernel_mode == "pipeline" else 0)
         self.rng = torch.Generator(device=self.device)
