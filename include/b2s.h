@@ -48,6 +48,8 @@ int b2s_step(b2s_sim* sim, int n_substeps);
 /* Named device arrays, leading dimension n_env: qpos qvel qacc qacc_warmstart ctrl time xpos xquat xmat
  * site_xpos site_xmat geom_xpos geom_xmat qM(dense nv x nv) qfrc_bias qfrc_passive qfrc_actuator qfrc_constraint
  * actuator_force ncon contact_geom contact_dist contact_pos contact_frame nefc efc_force warn ...
+ * (contact_efc_address, i32 [n_env, maxcon]: each contact's first constraint row, mjContact.efc_address; -1 for a contact without
+ * rows - not penetrating, or dropped by the row budget - and for rows ncon .. maxcon - 1)
  * (the attributes the reference touches, SURVEY.md section 8b).  dtype is B2S_F32/F64/I32.  After the first pipeline-mode step also
  * tail_key (i32: each environment's tail cost class) and tail_order (i32: per group, the environment each warp position of the last
  * tail launch ran), the cost order the pipeline's tail hands environments to warps in; written when tail blocks hold 8 warps or more. */
@@ -282,9 +284,23 @@ int b2s_set_contact_export(b2s_sim* sim, int flag);
  * The arrays are valid once the call's work on the handle's stream is done, and b2s_jac_site / b2s_jac_body / b2s_jac_geom and
  * b2s_full_m, which read them, are then valid too.  b2s_reset_envs writes them for the masked environments (with or without the
  * flag, through its forward pass, as b2s_forward does for all); after b2s_restore they are stale until the next step, like the
- * other derived arrays.  They are not a snapshot section, and neither they nor the flag are part of the signature.  The step-2
- * arrays (qfrc_actuator, qfrc_constraint, actuator_force, efc_*) still come with b2s_set_export only.  B2S_ERR_ARG: null handle. */
+ * other derived arrays.  They are not a snapshot section, and neither they nor the flag are part of the signature.  B2S_ERR_ARG:
+ * null handle. */
 int b2s_set_step1_export(b2s_sim* sim, int flag);
+
+/* The step-2 arrays without the full export (what energy penalties, smoothness terms and contact-force rewards or safety checks
+ * read from sim.data after env.step: actuator_force, qfrc_actuator, qacc, efc_force through mj_contactForce).  flag != 0 (default
+ * 0): the LAST substep of every b2s_env_step / b2s_step call writes qfrc_actuator, qfrc_smooth, qacc_smooth, qfrc_constraint
+ * [n_env, nv], actuator_force [n_env, nu], nefc [n_env], efc_type (i32), efc_D, efc_R, efc_aref, efc_force [n_env, maxefc] (zeros
+ * from row nefc on), efc_J [n_env, maxefc, nv] (the first nefc * nv values of the row; the rest keep whatever they held),
+ * solver_niter [n_env] and contact_efc_address [n_env, maxcon]: the values of that substep's constraint stage and step2 (mj_step's
+ * forward dynamics and constraint solve), the same bits in all three schedules, so b2s_env_step keeps the handle's mode
+ * (b2s_set_export = 1, which also writes these arrays, still runs the fused kernel).  The arrays are valid once the call's work on
+ * the handle's stream is done.  b2s_reset_envs writes them for the masked environments (with or without the flag, through its
+ * forward pass, as b2s_forward does for all); after b2s_restore they are stale until the next step, like the other derived arrays.
+ * qacc is state and is written by every step.  They are not a snapshot section, and neither they nor the flag are part of the
+ * signature.  B2S_ERR_ARG: null handle. */
+int b2s_set_step2_export(b2s_sim* sim, int flag);
 
 /* Scheduling of b2s_env_step / b2s_step: 0 = fused (one kernel per call, state resident in shared memory for all
  * substeps), 1 = pipeline (per substep and environment group: phase 0, phase 1 (narrow phase + controller), the tail kernel and,

@@ -100,6 +100,7 @@ struct b2s_sim {
   std::vector<int> site_bodyid, cgid;
   std::map<std::string, std::vector<std::string>> names;  // object type -> names by id (MjModel name tables)
   int has_obs = 0, export_env_step = 1, dirty = 1, mode = 0, ngroups = 8;
+  int export_dyn = 0;  // b2s_set_step2_export (also in DState for the fused kernel): the pipeline and the unit queue launch the DYN kernels
   int ctrl_split = 1;  // pipeline: OSC controller as its own thread-per-environment kernel (B2S_CTRL_SPLIT=0: inside the tail kernel)
   // pipeline: one CUDA graph per environment group, replayed on the group's stream and joined to `stream` through gevents
   std::vector<cudaStream_t> gstreams;
@@ -440,6 +441,7 @@ template <typename R> static void build_state(b2s_sim* s, const DModel<R>& m, DS
   st.cdof = state_arr<R>(s, "cdof", nv, 6);
   st.ncon = state_arr_i(s, "ncon", 0); st.contact_geom = state_arr_i(s, "contact_geom", mc, 2);
   st.contact_dim = state_arr_i(s, "contact_dim", mc); st.nefc = state_arr_i(s, "nefc", 0);
+  st.contact_efc_address = state_arr_i(s, "contact_efc_address", mc);
   st.efc_type = state_arr_i(s, "efc_type", me); st.warn = state_arr_i(s, "warn", 0); st.solver_niter = state_arr_i(s, "solver_niter", 0);
   st.contact_dist = state_arr<R>(s, "contact_dist", mc); st.contact_pos = state_arr<R>(s, "contact_pos", mc, 3);
   st.contact_frame = state_arr<R>(s, "contact_frame", mc, 9); st.contact_friction = state_arr<R>(s, "contact_friction", mc, 3);
@@ -771,9 +773,12 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
       using R = real_of<decltype(m)>;
       cudaError_t e = optin_max_smem(step_kernel<R>, device);
       if (e == cudaSuccess) e = optin_max_smem(phase0_kernel<R>, device);
-      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_THREADS, false>, device);
-      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_THREADS, true>, device);
-      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_WIDE_THREADS, true>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_THREADS, false, false>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_THREADS, true, false>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_WIDE_THREADS, true, false>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_THREADS, false, true>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_THREADS, true, true>, device);
+      if (e == cudaSuccess) e = optin_max_smem(tail_kernel<R, TAIL_WIDE_THREADS, true, true>, device);
       if (e == cudaSuccess) e = optin_max_smem(phase1_kernel<R>, device);
       return e;
     });
@@ -816,6 +821,14 @@ int b2s_set_contact_export(b2s_sim* s, int flag) {
 int b2s_set_step1_export(b2s_sim* s, int flag) {
   if (!s) return fail(B2S_ERR_ARG, "null handle");
   with_real(s, [&](auto&, auto& st) { st.export_kin = flag != 0; return 0; });
+  s->dirty = 1;
+  return B2S_OK;
+}
+
+int b2s_set_step2_export(b2s_sim* s, int flag) {
+  if (!s) return fail(B2S_ERR_ARG, "null handle");
+  with_real(s, [&](auto&, auto& st) { st.export_dyn = flag != 0; return 0; });
+  s->export_dyn = flag != 0;
   s->dirty = 1;
   return B2S_OK;
 }
@@ -898,7 +911,7 @@ static int enqueue_group(b2s_sim* s, const DModel<R>& m, const DState<R>& st, in
   // them dismissed in a few microseconds: half a block per environment keeps every slow item on its own warp without flooding the
   // block scheduler with thousands of empty blocks per launch
   const int cvx_blocks = std::max(s->num_sms, g.nenv / 2);
-  const bool ctrl_ext = (phases & PH_CTRL_EXT) != 0;
+  const bool ctrl_ext = (phases & PH_CTRL_EXT) != 0, dyn = (phases & PH_EXPORT_DYN) != 0;
   // the group's work-list counters and both tail class sets for substep 0 (each tail launch zeroes them for the next substep)
   CUDA_TRY(cudaMemsetAsync(st.cl_cnt + CL_CNT_STRIDE * gi, 0, CL_CNT_STRIDE * sizeof(int), q));
   for (int sub = 0; sub < nsub; sub++) {
@@ -910,9 +923,11 @@ static int enqueue_group(b2s_sim* s, const DModel<R>& m, const DState<R>& st, in
     P1Cfg c{std::min(nG, cvx_blocks), ctrl_ext ? (g.nenv + OSC_TPB - 1) / OSC_TPB : 0, sub};
     int nAb = (nA + 31) / 32;
     if (c.nG + c.nC + nAb > 0) phase1_kernel<R><<<c.nG + c.nC + nAb, 32, p1smem, q>>>(action, g, c);
-    if (s->tail_wide) tail_kernel<R, TAIL_WIDE_THREADS, true><<<blocks5, s->wpb5 * 32, s->smem5, q>>>(phases, nsub, action, g, s->stride5, s->stride5l, s->nlw5);
-    else if (st.tail_sorted) tail_kernel<R, TAIL_THREADS, true><<<blocks5, s->wpb5 * 32, s->smem5, q>>>(phases, nsub, action, g, s->stride5, s->stride5l, s->nlw5);
-    else tail_kernel<R, TAIL_THREADS, false><<<blocks5, s->wpb5 * 32, s->smem5, q>>>(phases, nsub, action, g, s->stride5, s->stride5l, s->nlw5);
+    // the step-2 export (PH_EXPORT_DYN, part of the graph's key) selects the instantiation with the writer
+    auto kern = s->tail_wide ? (dyn ? tail_kernel<R, TAIL_WIDE_THREADS, true, true> : tail_kernel<R, TAIL_WIDE_THREADS, true, false>)
+              : st.tail_sorted ? (dyn ? tail_kernel<R, TAIL_THREADS, true, true> : tail_kernel<R, TAIL_THREADS, true, false>)
+                               : (dyn ? tail_kernel<R, TAIL_THREADS, false, true> : tail_kernel<R, TAIL_THREADS, false, false>);
+    kern<<<blocks5, s->wpb5 * 32, s->smem5, q>>>(phases, nsub, action, g, s->stride5, s->stride5l, s->nlw5);
   }
   CUDA_TRY(cudaGetLastError());
   return B2S_OK;
@@ -971,6 +986,7 @@ static int launch_pipeline(b2s_sim* s, int phases, int nsub, const void* action)
 #endif
     const bool osc = s->ctrl.kind == B2S_CTRL_OSC_POSE || s->ctrl.kind == B2S_CTRL_OSC_POSITION;
     if ((phases & PH_CTRL) && osc && s->ctrl_split) phases |= PH_CTRL_EXT;
+    if (s->export_dyn) phases |= PH_EXPORT_DYN;  // keys the captured graph too: switching the flag selects the other graph
     { int rc2 = rebuild_layouts(s); if (rc2 != B2S_OK) return rc2; }  // before the descriptors are (re)uploaded
     int rc = bind_constants(s);
     if (rc != B2S_OK) return rc;
@@ -1042,13 +1058,14 @@ static int launch_unit(b2s_sim* s, int phases, int nsub, const void* action) {
       int stride = std::max(std::max(s->lay[LAY_P0].total, s->lay[LAY_TS].total), EPA_AREA_WORDS(EPA_MAXV, EPA_MAXF) + 24 + 384);
       stride = (stride + 3) & ~3;
       int stride_l = (s->lay[LAY_TL].total + 3) & ~3;
-      CUDA_TRY(optin_max_smem(unit_kernel<R>, s->device));
+      CUDA_TRY(optin_max_smem(unit_kernel<R, false>, s->device));
+      CUDA_TRY(optin_max_smem(unit_kernel<R, true>, s->device));
       int best_w = 0, best_b = 0, best = 0;
       for (int w = UNIT_THREADS / 32; w >= 1; w--) {
         size_t sm = std::max((size_t)w * stride, tiered ? (size_t)stride_l : 0) * rsz;
         if (sm > 226 * 1024) continue;
         int b = 0;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, unit_kernel<R>, w * 32, sm) != cudaSuccess) { cudaGetLastError(); continue; }
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&b, unit_kernel<R, false>, w * 32, sm) != cudaSuccess) { cudaGetLastError(); continue; }
         if (w * b > best) { best = w * b; best_w = w; best_b = b; }
       }
       if (best == 0) return fail(B2S_ERR_UNSUPPORTED, "unit-queue mode: workspace does not fit shared memory");
@@ -1074,7 +1091,9 @@ static int launch_unit(b2s_sim* s, int phases, int nsub, const void* action) {
     q.prof = s->uq_prof;
 #endif
     unit_init_kernel<R><<<(total + 255) / 256, 256, 0, s->stream>>>(q, s->n_env);
-    unit_kernel<R><<<s->uq_grid, s->uq_wpb * 32, s->uq_smem, s->stream>>>(phases, nsub, (const R*)action, s->slot, q);
+    // the step-2 export runs the instantiation with the writer (both have 128 registers and the same shared memory, so one block shape)
+    if (s->export_dyn) unit_kernel<R, true><<<s->uq_grid, s->uq_wpb * 32, s->uq_smem, s->stream>>>(phases | PH_EXPORT_DYN, nsub, (const R*)action, s->slot, q);
+    else unit_kernel<R, false><<<s->uq_grid, s->uq_wpb * 32, s->uq_smem, s->stream>>>(phases, nsub, (const R*)action, s->slot, q);
     unit_check_kernel<R><<<8, 256, 0, s->stream>>>(q, s->slot);
     s->launches += 3;
     CUDA_TRY(cudaGetLastError());

@@ -89,14 +89,19 @@ DEVN void export_step1(const Eng<R> e, int env, int ncon) {
   export_contacts(e, env, ncon);
 }
 
-// constraint rows (the Jacobian overlays kinematics scratch, so this runs after make_constraint)
+// The constraint rows of this substep -> efc_type, efc_aref, efc_D, efc_R (zeros from row nefc on), efc_J (the first nefc * nv
+// entries), nefc, and contact_efc_address: a contact's first row, -1 for a contact without rows (not penetrating, or dropped by
+// the row budget) and for rows ncon .. maxcon - 1.  Reads J, the row headers and values and the contact headers, which
+// make_constraint writes and nothing after it rewrites before the next substep (the controller, actuation, acceleration and the
+// solve only read them), so it may run anywhere between make_constraint and the late pose load that overlays J (tail_finish).
 template <typename R>
-DEVN void export_efc(const Eng<R> e, int env, int nefc) {
+DEVN void export_efc(const Eng<R> e, int env, int ncon, int nefc) {
   const DModel<R>& m = e.model();
   const WSLayout& L = e.lay();
   const DState<R>& s = e.state();
   int lane = e.lane;
   size_t E = env;
+  B2S_LOOP
   for (int r = lane; r < m.maxefc; r += 32) {
     bool v = r < nefc;
     s.efc_type[E * m.maxefc + r] = v ? (e.pi(L.e_int)[r] & 255) : 0;
@@ -104,21 +109,34 @@ DEVN void export_efc(const Eng<R> e, int env, int nefc) {
     s.efc_D[E * m.maxefc + r] = v ? e.p(L.e_D)[r] : R(0);
     s.efc_R[E * m.maxefc + r] = v ? e.p(L.e_R)[r] : R(0);
   }
+  B2S_LOOP
   for (int k = lane; k < nefc * m.nv; k += 32) s.efc_J[E * m.maxefc * m.nv + k] = e.p(L.J)[k];
+  const int* cint = e.pi(L.c_int);
+  B2S_LOOP
+  for (int c = lane; c < m.maxcon; c += 32) s.contact_efc_address[E * m.maxcon + c] = c < ncon ? cint[5 * c + 3] : -1;
   if (lane == 0) s.nefc[env] = nefc;
 }
 
+// The step-2 arrays of this substep -> the constraint rows (export_efc), qfrc_actuator, qfrc_smooth, qacc_smooth,
+// qfrc_constraint, efc_force (zeros from row nefc on) and solver_niter; runs after the solve, before Euler.  actuator_force is
+// written by actuation itself, through the pointer its caller passes on the same substep.  Compiled once per precision and called
+// by every schedule (the fused kernel and the tail, right after the solve), so all three write the same bits.
 template <typename R>
-DEVN void export_step2(const Eng<R> e, int env, int nefc, int niter) {
+DEVN void export_dynamics(const Eng<R> e, int env, int ncon, int nefc, int niter) {
   const DModel<R>& m = e.model();
   const WSLayout& L = e.lay();
   const DState<R>& s = e.state();
   int lane = e.lane;
   size_t E = env;
-  load_row(s.qfrc_actuator + E * m.nv, e.p(L.qact), m.nv, lane);
-  load_row(s.qfrc_smooth + E * m.nv, e.p(L.qsmooth), m.nv, lane);
-  load_row(s.qacc_smooth + E * m.nv, e.p(L.qaccs), m.nv, lane);
-  load_row(s.qfrc_constraint + E * m.nv, e.p(L.qcon), m.nv, lane);
+  export_efc(e, env, ncon, nefc);
+  B2S_LOOP
+  for (int i = lane; i < m.nv; i += 32) {
+    s.qfrc_actuator[E * m.nv + i] = e.p(L.qact)[i];
+    s.qfrc_smooth[E * m.nv + i] = e.p(L.qsmooth)[i];
+    s.qacc_smooth[E * m.nv + i] = e.p(L.qaccs)[i];
+    s.qfrc_constraint[E * m.nv + i] = e.p(L.qcon)[i];
+  }
+  B2S_LOOP
   for (int r = lane; r < m.maxefc; r += 32) s.efc_force[E * m.maxefc + r] = r < nefc ? e.p(L.e_force)[r] : R(0);
   if (lane == 0) s.solver_niter[env] = niter;
 }
@@ -182,15 +200,17 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
       }
       __syncthreads();
       nefc = make_constraint(e, ncon, warn);
-      if (ex) export_efc(e, env, nefc);
+      if (ex && !(phases & PH_STEP2)) export_efc(e, env, ncon, nefc);  // b2s_step1: no solve follows, the rows alone
     }
     if (phases & PH_CTRL) ctrl_run(e, cs, env, sub == 0 ? action : (const R*)nullptr);
     if (phases & PH_STEP2) {
-      e.actuation(ex ? s.actuator_force + E * m.nu : nullptr);
+      // the full export, or the call's last substep with b2s_set_step2_export: one call site for both
+      const bool dyn = ex || (live && s.export_dyn && sub == nsub - 1);
+      e.actuation(dyn ? s.actuator_force + E * m.nu : nullptr);
       if (e.acceleration()) warn |= 1;
       __syncthreads();
       niter = solve(e, nefc, ncon, warn);
-      if (ex) export_step2(e, env, nefc, niter);
+      if (dyn) export_dynamics(e, env, ncon, nefc, niter);
       if (!(phases & PH_NOINTEGRATE)) {
         { int eb = e.euler(&time); if (eb & 32) warn |= 32; else if (eb) warn |= 2; }
       }

@@ -343,9 +343,10 @@ template <typename R> DEV void tail_ctrl(Eng<R>& e, int env, int sub, const R* a
 }
 
 // Dynamics, in two parts (the unit queue puts a block barrier between them): actuation + smooth acceleration, then the Newton solve.
-// Both return warn bits; the solve also reports its Newton iterations.
-template <typename R> DEV int tail_accel(Eng<R>& e) {
-  e.actuation((R*)nullptr);
+// Both return warn bits; the solve also reports its Newton iterations.  act_force_out: where actuation writes actuator_force (the
+// step-2 export's last substep), nullptr otherwise.
+template <typename R> DEV int tail_accel(Eng<R>& e, R* act_force_out = nullptr) {
+  e.actuation(act_force_out);
   return e.acceleration() ? 1 : 0;
 }
 template <typename R> DEV int tail_newton(Eng<R>& e, int nefc, int ncon, int* niter = nullptr) {
@@ -353,6 +354,15 @@ template <typename R> DEV int tail_newton(Eng<R>& e, int nefc, int ncon, int* ni
   const int it = solve(e, nefc, ncon, warn);
   if (niter) *niter = it;
   return warn;
+}
+
+// The step-2 export (b2s_set_step2_export) in the tail: on the call's last substep, actuation writes actuator_force and, right after
+// the solve (before Euler and before tail_finish's late pose load overlays J), export_dynamics writes the rest; only the tier that
+// finishes the environment gets there.  The tail kernels and the unit queue have an instantiation with it (DYN, launched with
+// PH_EXPORT_DYN) and one without, whose code is the tail's as it was before the export existed: with the writer compiled in but not
+// called, NutAssemblyRound's pipeline ran 1.2 % slower (DESIGN.md section 6).
+template <typename R> DEV R* tail_act_force_out(const Eng<R>& e, int env, bool last) {
+  return last ? e.state().actuator_force + (size_t)env * e.model().nu : (R*)nullptr;
 }
 
 // Finish: on the last substep of the call the contact records (b2s_set_contact_export), Euler, the rows of the observables that
@@ -467,7 +477,7 @@ template <typename R> DEV int tail_env_at(const Grp& g, int p, int lane) {
 // the layout.  Compiled separately: the kernel calls it for both tiers.  SORTED (the cost order): `env` is the environment for the
 // large tier; for the small tier it is the warp's position in the launch, resolved here (tail_env_at, recorded in tail_order) so that
 // the kernel body keeps no loaded value live across the call; the cost class of the environment is written for the next substep.
-template <typename R, bool SORTED>
+template <typename R, bool SORTED, bool DYN>
 DEVN int tail_env(R* area, int lane, int lid, Grp g, int env, int nsub, int phases, const R* action, unsigned long long* bar, unsigned& parity) {
   const int sub = g.sub;
   if (SORTED && lid == LAY_TS) {
@@ -485,10 +495,12 @@ DEVN int tail_env(R* area, int lane, int lid, Grp g, int env, int nsub, int phas
   const int ncon = TAIL_NCON(pk), nefc = TAIL_NEFC(pk);
   int warn = TAIL_WARN(pk);
   if ((phases & PH_CTRL) && !(phases & PH_CTRL_EXT)) tail_ctrl(e, env, sub, action);
-  warn |= tail_accel(e);
+  if constexpr (DYN) warn |= tail_accel(e, tail_act_force_out(e, env, sub == nsub - 1));
+  else warn |= tail_accel(e);
   int niter;
   warn |= tail_newton(e, nefc, ncon, &niter);
   if (SORTED && lane == 0) e.state().tail_key[env] = tail_cost_key(niter, nefc, lid == LAY_TL);
+  if constexpr (DYN) if (sub == nsub - 1) export_dynamics(e, env, ncon, nefc, niter);
   tail_finish(e, env, sub, nsub, phases, ncon, warn, bar, parity);
 #ifdef B2S_INSTR
   if (lane == 0 && s.cyc) {
@@ -506,7 +518,7 @@ DEVN int tail_env(R* area, int lane, int lid, Grp g, int env, int nsub, int phas
 // or by id; an environment that does not fit is left in the block's overflow list.  After a block barrier the first `nlw` warps re-run
 // the block's overflowed environments with the full-capacity layout (`stride_l` words per warp, over the small tier's dead areas).
 // An overflowed environment waits for its own block only, not for the whole group.
-template <typename R, int THREADS, bool SORTED>
+template <typename R, int THREADS, bool SORTED, bool DYN>
 __global__ void __launch_bounds__(THREADS, THREADS == TAIL_WIDE_THREADS ? 1 : TAIL_BLOCKS) tail_kernel(int phases, int nsub, const R* action, Grp g, int stride, int stride_l, int nlw) {
   const DState<R>& s = cstate<R>(g.slot);
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -525,7 +537,7 @@ __global__ void __launch_bounds__(THREADS, THREADS == TAIL_WIDE_THREADS ? 1 : TA
   unsigned parity = 0;
   const int p = blockIdx.x * wpb + warp;
   int o = -1;
-  if (p < g.nenv && tail_env<R, SORTED>(smem + (size_t)warp * stride, lane, LAY_TS, g, SORTED ? p : g.env0 + p, nsub, phases, action, &mbar[warp], parity)) o = p;
+  if (p < g.nenv && tail_env<R, SORTED, DYN>(smem + (size_t)warp * stride, lane, LAY_TS, g, SORTED ? p : g.env0 + p, nsub, phases, action, &mbar[warp], parity)) o = p;
   if (lane == 0) ovf[warp] = o;
   // the small tier's areas are dead from here on (every fitting environment has stored its state, ws_store waited for its bulk
   // stores); order this thread's generic accesses to them before the large tier's bulk loads into the same shared memory
@@ -534,6 +546,6 @@ __global__ void __launch_bounds__(THREADS, THREADS == TAIL_WIDE_THREADS ? 1 : TA
   if (warp < nlw)
     for (int k = warp; k < wpb; k += nlw)
       if (ovf[k] >= 0)
-        tail_env<R, SORTED>(smem + (size_t)warp * stride_l, lane, LAY_TL, g, SORTED ? s.tail_order[g.env0 + ovf[k]] : g.env0 + ovf[k], nsub, phases, action, &mbar[warp], parity);
+        tail_env<R, SORTED, DYN>(smem + (size_t)warp * stride_l, lane, LAY_TL, g, SORTED ? s.tail_order[g.env0 + ovf[k]] : g.env0 + ovf[k], nsub, phases, action, &mbar[warp], parity);
   INSTR_END(s, g, 3)
 }

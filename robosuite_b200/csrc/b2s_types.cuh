@@ -23,6 +23,7 @@ enum {
   PH_CTRL = 16,      // run the fused controller between step1 and step2
   PH_CTRL_EXT = 512, // pipeline mode: the controller ran as its own kernel (ctrl_osc_kernel), `ctrl` is already in HBM
   PH_LAST_SUB = 1024,  // pipeline mode: this phase-0 node is the call's last substep (b2s_set_step1_export)
+  PH_EXPORT_DYN = 2048,  // pipeline / unit queue: b2s_set_step2_export is on - the launch runs the tail instantiation with the writer
   PH_OBS = 64        // write the observation row and the task outputs (after the last substep)
 };
 
@@ -129,6 +130,9 @@ struct DState {
   const struct ObsModDev* obs_mod;  // sampling rates and corruptors (b2s_obs_modifiers); null: every observable on the last substep, no noise
   int export_con;  // b2s_set_contact_export: the last substep of a step call writes contact_* / ncon in every schedule
   int export_kin;  // b2s_set_step1_export: the last substep of a step call writes the step-1 arrays (export_kinematics) in every schedule
+  int export_dyn;  // b2s_set_step2_export: the fused kernel's last substep of a step call writes the step-2 arrays (export_dynamics); the
+                   // pipeline and the unit queue launch their DYN instantiations instead (PH_EXPORT_DYN)
+  int* contact_efc_address;  // [n_env, maxcon] first constraint row of each contact (mjContact.efc_address), -1: no rows / no contact
 };
 
 // offsets (in units of R) of the per-warp shared-memory workspace

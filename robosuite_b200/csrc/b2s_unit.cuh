@@ -120,6 +120,20 @@ template <typename R> DEVN int unit_tail_solve(R* area, int lane, int slot, int 
   e.env = env;
   return tail_newton(e, nefc, ncon);
 }
+// the same two stages with the step-2 export (unit_kernel<R, true>): on the call's last substep (`last`) actuator_force, then after
+// the solve the other step-2 arrays
+template <typename R> DEVN int unit_tail_acc_dyn(R* area, int lane, int slot, int env, bool last) {
+  Eng<R> e(area, lane, slot, LAY_TS);
+  return tail_accel(e, tail_act_force_out(e, env, last));
+}
+template <typename R> DEVN int unit_tail_solve_dyn(R* area, int lane, int slot, int env, int nefc, int ncon, bool last) {
+  Eng<R> e(area, lane, slot, LAY_TS);
+  e.env = env;
+  int niter;
+  const int warn = tail_newton(e, nefc, ncon, &niter);
+  if (last) export_dynamics(e, env, ncon, nefc, niter);
+  return warn;
+}
 template <typename R>
 DEVN void unit_tail_end(R* area, int lane, int slot, int env, int sub, int nsub, int phases, int ncon, int warn, unsigned long long* bar, unsigned& parity) {
   Eng<R> e(area, lane, slot, LAY_TS);
@@ -146,7 +160,8 @@ DEV void unit_finish(const UnitQ& q, int n_env, int env, int sub, int nsub, int 
 // 4 warps x 4 blocks 158 k, free-running warps (no block barriers) 80 k.
 constexpr int UNIT_THREADS = 512, UNIT_BLOCKS = 1;
 
-template <typename R>
+// DYN: the step-2 export's instantiation (launched with PH_EXPORT_DYN; the other one has no writer code, see tail_act_force_out)
+template <typename R, bool DYN>
 __global__ void __launch_bounds__(UNIT_THREADS, UNIT_BLOCKS) unit_kernel(int phases, int nsub, const R* action, int slot, UnitQ q) {
   const DState<R>& s = cstate<R>(slot);
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -184,8 +199,15 @@ __global__ void __launch_bounds__(UNIT_THREADS, UNIT_BLOCKS) unit_kernel(int pha
       const int ncon = TAIL_NCON(pk);
       int warn = TAIL_WARN(pk);
       if (phases & PH_CTRL) tail_ctrl(e, env, sub, action);
-      warn |= tail_accel(e);
-      warn |= tail_newton(e, TAIL_NEFC(pk), ncon);
+      if constexpr (DYN) {
+        warn |= tail_accel(e, tail_act_force_out(e, env, sub == nsub - 1));
+        int niter;
+        warn |= tail_newton(e, TAIL_NEFC(pk), ncon, &niter);
+        if (sub == nsub - 1) export_dynamics(e, env, ncon, TAIL_NEFC(pk), niter);
+      } else {
+        warn |= tail_accel(e);
+        warn |= tail_newton(e, TAIL_NEFC(pk), ncon);
+      }
       tail_finish(e, env, sub, nsub, phases, ncon, warn, &mbar[warp], parity);
       unit_finish(q, n_env, env, sub, nsub, lane);
     }
@@ -284,10 +306,12 @@ __global__ void __launch_bounds__(UNIT_THREADS, UNIT_BLOCKS) unit_kernel(int pha
     if (live && (phases & PH_CTRL)) unit_tail_ctrl<R>(area, lane, slot, env, sub, action);
     __syncthreads();
     UTICK(5)
-    if (live) warn |= unit_tail_acc<R>(area, lane, slot);
+    if constexpr (DYN) { if (live) warn |= unit_tail_acc_dyn<R>(area, lane, slot, env, sub == nsub - 1); }
+    else if (live) warn |= unit_tail_acc<R>(area, lane, slot);
     __syncthreads();
     UTICK(6)
-    if (live) warn |= unit_tail_solve<R>(area, lane, slot, env, nefc, ncon);
+    if constexpr (DYN) { if (live) warn |= unit_tail_solve_dyn<R>(area, lane, slot, env, nefc, ncon, sub == nsub - 1); }
+    else if (live) warn |= unit_tail_solve<R>(area, lane, slot, env, nefc, ncon);
     __syncthreads();
     UTICK(7)
     if (live) {

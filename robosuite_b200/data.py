@@ -19,7 +19,16 @@ The arrays are written by forward / reset (the masked environments) and, after e
 step-1 export (set_step1_export, make(..., data_queries=True)) or its full export (set_export) is on.  A read on a handle with
 both off raises instead of answering from the poses of an earlier forward.  Poses of non-colliding (visual) geoms are never
 computed: asking for one raises ValueError.  After restore / clone_envs no physics runs, so the arrays keep the poses the
-environments had before until the next step."""
+environments had before until the next step.
+
+The step-2 half (recalled the same way: mujoco.MjData fields the reference's code reads after env.step, and mujoco.mj_contactForce):
+qacc (state, always current), qfrc_actuator, actuator_force, qfrc_smooth, qacc_smooth, qfrc_constraint [N, nv] / [N, nu], nefc [N],
+the constraint rows efc_type, efc_D, efc_R, efc_aref, efc_force [N, maxefc] and efc_J [N, maxefc, nv] kept at capacity (the first
+nefc[e] rows of environment e are valid), and solver_niter [N].  They need the step-2 export (set_step2_export,
+make(..., dynamics_queries=True)) or the full export.  contact_force() is mj_contactForce for elliptic cones: contact c's force
+and torque in its own frame (normal first, then the tangential and the torsional / rolling components) are
+efc_force[efc_address : efc_address + dim], zero-padded to 6; a contact without rows (efc_address -1: not penetrating, or
+dropped by the row budget) has zero force.  It also needs the contact records (set_contact_export, or the full export)."""
 
 
 class BatchedData:
@@ -40,6 +49,16 @@ class BatchedData:
 
     def _array(self, name):
         self._check()
+        return getattr(self._sim, name)
+
+    def _check2(self):
+        s = self._sim
+        if not (s.full_export or getattr(s, "step2_export", False)):
+            raise RuntimeError("sim.data reads the step-2 arrays, which env_step / step write only with the step-2 export on: create "
+                               "the environment with make(..., dynamics_queries=True) or call BatchedSim.set_step2_export(True)")
+
+    def _array2(self, name):
+        self._check2()
         return getattr(self._sim, name)
 
     def _id(self, kind, obj):
@@ -70,6 +89,58 @@ class BatchedData:
     cdof = property(lambda self: self._array("cdof"))
     qfrc_bias = property(lambda self: self._array("qfrc_bias"))
     qfrc_passive = property(lambda self: self._array("qfrc_passive"))
+
+    # ---- the step-2 arrays, [N, ...] device views; the row arrays at capacity (nefc says how many rows are valid)
+    qacc = property(lambda self: self._sim.qacc)  # state: written by every step
+    qfrc_actuator = property(lambda self: self._array2("qfrc_actuator"))
+    actuator_force = property(lambda self: self._array2("actuator_force"))
+    qfrc_smooth = property(lambda self: self._array2("qfrc_smooth"))
+    qacc_smooth = property(lambda self: self._array2("qacc_smooth"))
+    qfrc_constraint = property(lambda self: self._array2("qfrc_constraint"))
+    nefc = property(lambda self: self._array2("nefc"))
+    efc_type = property(lambda self: self._array2("efc_type"))
+    efc_J = property(lambda self: self._array2("efc_J"))
+    efc_D = property(lambda self: self._array2("efc_D"))
+    efc_R = property(lambda self: self._array2("efc_R"))
+    efc_aref = property(lambda self: self._array2("efc_aref"))
+    efc_force = property(lambda self: self._array2("efc_force"))
+    solver_niter = property(lambda self: self._array2("solver_niter"))
+
+    def contact_force(self, contact=None):
+        """mj_contactForce of every contact slot, [N, maxcon, 6], or of slot `contact` (an int), [N, 6]: force and torque in the
+        contact's frame (contact_frame), zeros for a contact without constraint rows and for slots at or beyond ncon.  Elliptic
+        cones only (a pyramidal cone's forces are not rows of the contact frame)."""
+        s = self._sim
+        if int(getattr(s.model, "opt_cone", 1)) != 1:
+            raise NotImplementedError("contact_force() supports elliptic friction cones (cone=\"elliptic\") only; this model uses "
+                                      "pyramidal cones")
+        self._check2()
+        if not (s.full_export or getattr(s, "contact_export", False)):
+            raise RuntimeError("contact_force() also reads the contact records, which env_step / step write only with the contact "
+                               "export on: create the environment with make(..., dynamics_queries=True) or call "
+                               "BatchedSim.set_contact_export(True)")
+        import torch
+
+        adr, dim, ncon, f, nefc = s.contact_efc_address, s.contact_dim, s.ncon, s.efc_force, s.nefc
+        mc = adr.shape[1]
+        if contact is not None:
+            c = int(contact)
+            if not 0 <= c < mc:
+                raise ValueError("contact index {} out of range [0, {})".format(c, mc))
+            adr, dim = adr[:, c:c + 1], dim[:, c:c + 1]
+            slot = torch.full((1,), c, device=adr.device)
+        else:
+            slot = torch.arange(mc, device=adr.device)
+        k = torch.arange(6, device=adr.device)
+        live = (adr >= 0) & (slot[None, :] < ncon[:, None].to(slot.dtype))                  # [N, C]
+        # only rows below nefc: if the contact records and the rows come from different steps (one export switched on after the
+        # other's last write), a stale dim must not index past the rows the solve wrote - or past efc_force itself
+        row = adr[..., None].long() + k
+        take = live[..., None] & (k < dim[..., None]) & (row < nefc[:, None, None].long())  # [N, C, 6]
+        idx = torch.where(take, row, torch.zeros((), dtype=torch.long, device=adr.device)).clamp_(0, f.shape[1] - 1)
+        out = torch.gather(f, 1, idx.reshape(idx.shape[0], -1)).reshape(idx.shape)
+        out = torch.where(take, out, torch.zeros((), dtype=f.dtype, device=f.device))
+        return out[:, 0] if contact is not None else out
 
     def full_m(self):
         """mj_fullM: the dense mass matrices [N, nv, nv] (a copy)"""

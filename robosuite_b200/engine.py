@@ -116,6 +116,7 @@ def lib():
         L.b2s_set_export.argtypes = [C.c_void_p, C.c_int]
         L.b2s_set_contact_export.argtypes = [C.c_void_p, C.c_int]
         L.b2s_set_step1_export.argtypes = [C.c_void_p, C.c_int]
+        L.b2s_set_step2_export.argtypes = [C.c_void_p, C.c_int]
         L.b2s_set_mode.argtypes = [C.c_void_p, C.c_int]
         L.b2s_launch_count.argtypes = [C.c_void_p]
         L.b2s_launch_count.restype = C.c_int64
@@ -223,6 +224,8 @@ class BatchedSim:
         self._cache = {}
         self.full_export = True     # set_export (the library's default)
         self.step1_export = False  # set_step1_export
+        self.step2_export = False  # set_step2_export
+        self.contact_export = False  # set_contact_export
         global _LIVE
         if _LIVE is None:
             import weakref
@@ -416,10 +419,18 @@ class BatchedSim:
         self._check(self._L.b2s_set_step1_export(self._h, int(bool(flag))))
         self.step1_export = bool(flag)
 
+    def set_step2_export(self, flag):
+        """whether the last substep of every env_step / step writes the step-2 arrays (qfrc_actuator, actuator_force, qfrc_smooth,
+        qacc_smooth, qfrc_constraint, nefc, efc_*, solver_niter, contact_efc_address: what `data`'s dynamics properties and
+        contact_force() read) in every mode, without the rest of the derived-array export (b2s_set_step2_export)"""
+        self._check(self._L.b2s_set_step2_export(self._h, int(bool(flag))))
+        self.step2_export = bool(flag)
+
     @property
     def data(self):
-        """the batched MjData view of the step-1 arrays (robosuite_b200/data.py); after env_step / step it needs
-        set_step1_export(True) or set_export(True)"""
+        """the batched MjData view of the step-1 and step-2 arrays (robosuite_b200/data.py); after env_step / step it needs
+        set_step1_export(True) (poses, Jacobians, mass matrices), set_step2_export(True) (forces, constraint rows; contact_force()
+        also set_contact_export(True)) or set_export(True)"""
         if "_data" not in self.__dict__:
             from .data import BatchedData
 
@@ -430,6 +441,7 @@ class BatchedSim:
         """whether the last substep of every env_step / step writes the contact arrays (contacts()) in every mode, without the
         rest of the derived-array export (b2s_set_contact_export)"""
         self._check(self._L.b2s_set_contact_export(self._h, int(bool(flag))))
+        self.contact_export = bool(flag)
 
     def contacts(self):
         """device views of the contacts of the last substep: "ncon" [N], "geom" [N, maxcon, 2] (-1 beyond ncon), "dist"

@@ -110,7 +110,9 @@ class BatchedMujocoEnv(ContactQueries):
     contact_queries=True switches the contact export on (BatchedSim.set_contact_export) before the first reset, so that
     check_contact / get_contacts / _check_grasp (envs/contacts.py) can read the contacts of the last substep.  data_queries=True
     does the same for the step-1 arrays (BatchedSim.set_step1_export), so that sim.data (robosuite_b200/data.py) reads the poses,
-    Jacobians and mass matrices of the last substep."""
+    Jacobians and mass matrices of the last substep.  dynamics_queries=True switches on the step-2 export
+    (BatchedSim.set_step2_export) and the contact export, so that sim.data reads the actuator, smooth and constraint forces, the
+    constraint rows and the per-contact forces (sim.data.contact_force()) of the last substep."""
 
     maxcon = None  # per-environment contact / constraint-row capacity (None: engine defaults 32 / 64); overflow sets warn bit 4
     maxefc = None
@@ -125,7 +127,8 @@ class BatchedMujocoEnv(ContactQueries):
                  ignore_done=False, reward_scale=1.0, reward_shaping=False, use_object_obs=True, seed=None,
                  initialization_noise="default", precision="f32", xml=None, has_renderer=False,
                  has_offscreen_renderer=False, use_camera_obs=False, hard_reset=False, lite_physics=True, model=None,
-                 kernel_mode="pipeline", sim_cls=None, contact_queries=False, data_queries=False, **kwargs):
+                 kernel_mode="pipeline", sim_cls=None, contact_queries=False, data_queries=False,
+                 dynamics_queries=False, **kwargs):
         import torch
 
         if has_renderer or has_offscreen_renderer or use_camera_obs:
@@ -169,11 +172,13 @@ class BatchedMujocoEnv(ContactQueries):
         self.sim.obs_config(op, a, b)
         self._setup_task()
         self.sim.set_export(False)
-        self._contact_queries = bool(contact_queries)
+        self._contact_queries = bool(contact_queries or dynamics_queries)  # contact_force() reads the contact records too
         if self._contact_queries:
             self.sim.set_contact_export(True)
         if data_queries:
             self.sim.set_step1_export(True)
+        if dynamics_queries:
+            self.sim.set_step2_export(True)
         # "pipeline": phase kernels + global collision work lists (fastest in steady state); "fused": one kernel per step
         self.sim.set_mode(1 if kernel_mode == "pipeline" else 0)
         self.rng = torch.Generator(device=self.device)
