@@ -100,7 +100,6 @@ struct b2s_sim {
   std::vector<int> site_bodyid, cgid;
   std::map<std::string, std::vector<std::string>> names;  // object type -> names by id (MjModel name tables)
   int has_obs = 0, export_env_step = 1, dirty = 1, mode = 0, ngroups = 8;
-  int export_dyn = 0;  // b2s_set_step2_export (also in DState for the fused kernel): the pipeline and the unit queue launch the DYN kernels
   int ctrl_split = 1;  // pipeline: OSC controller as its own thread-per-environment kernel (B2S_CTRL_SPLIT=0: inside the tail kernel)
   // pipeline: one CUDA graph per environment group, replayed on the group's stream and joined to `stream` through gevents
   std::vector<cudaStream_t> gstreams;
@@ -811,27 +810,20 @@ int b2s_set_stream(b2s_sim* s, void* stream) {
 
 int b2s_set_export(b2s_sim* s, int flag) { if (!s) return fail(B2S_ERR_ARG, "null handle"); s->export_env_step = flag != 0; return B2S_OK; }
 
-int b2s_set_contact_export(b2s_sim* s, int flag) {
+// the three array-group exports: DState::export_con / export_kin / export_dyn hold their EXP_* bit when on
+static int set_export_bit(b2s_sim* s, int bit, int flag) {
   if (!s) return fail(B2S_ERR_ARG, "null handle");
-  with_real(s, [&](auto&, auto& st) { st.export_con = flag != 0; return 0; });
+  with_real(s, [&](auto&, auto& st) {
+    int& f = bit == EXP_CONTACTS ? st.export_con : bit == EXP_STEP1 ? st.export_kin : st.export_dyn;
+    f = flag ? bit : 0;
+    return 0;
+  });
   s->dirty = 1;
   return B2S_OK;
 }
-
-int b2s_set_step1_export(b2s_sim* s, int flag) {
-  if (!s) return fail(B2S_ERR_ARG, "null handle");
-  with_real(s, [&](auto&, auto& st) { st.export_kin = flag != 0; return 0; });
-  s->dirty = 1;
-  return B2S_OK;
-}
-
-int b2s_set_step2_export(b2s_sim* s, int flag) {
-  if (!s) return fail(B2S_ERR_ARG, "null handle");
-  with_real(s, [&](auto&, auto& st) { st.export_dyn = flag != 0; return 0; });
-  s->export_dyn = flag != 0;
-  s->dirty = 1;
-  return B2S_OK;
-}
+int b2s_set_contact_export(b2s_sim* s, int flag) { return set_export_bit(s, EXP_CONTACTS, flag); }
+int b2s_set_step1_export(b2s_sim* s, int flag) { return set_export_bit(s, EXP_STEP1, flag); }
+int b2s_set_step2_export(b2s_sim* s, int flag) { return set_export_bit(s, EXP_STEP2, flag); }
 
 int64_t b2s_launch_count(const b2s_sim* s) { return s ? s->launches : 0; }
 
@@ -986,7 +978,7 @@ static int launch_pipeline(b2s_sim* s, int phases, int nsub, const void* action)
 #endif
     const bool osc = s->ctrl.kind == B2S_CTRL_OSC_POSE || s->ctrl.kind == B2S_CTRL_OSC_POSITION;
     if ((phases & PH_CTRL) && osc && s->ctrl_split) phases |= PH_CTRL_EXT;
-    if (s->export_dyn) phases |= PH_EXPORT_DYN;  // keys the captured graph too: switching the flag selects the other graph
+    if (st.export_dyn) phases |= PH_EXPORT_DYN;  // keys the captured graph too: switching the flag selects the other graph
     { int rc2 = rebuild_layouts(s); if (rc2 != B2S_OK) return rc2; }  // before the descriptors are (re)uploaded
     int rc = bind_constants(s);
     if (rc != B2S_OK) return rc;
@@ -1092,7 +1084,7 @@ static int launch_unit(b2s_sim* s, int phases, int nsub, const void* action) {
 #endif
     unit_init_kernel<R><<<(total + 255) / 256, 256, 0, s->stream>>>(q, s->n_env);
     // the step-2 export runs the instantiation with the writer (both have 128 registers and the same shared memory, so one block shape)
-    if (s->export_dyn) unit_kernel<R, true><<<s->uq_grid, s->uq_wpb * 32, s->uq_smem, s->stream>>>(phases | PH_EXPORT_DYN, nsub, (const R*)action, s->slot, q);
+    if (st.export_dyn) unit_kernel<R, true><<<s->uq_grid, s->uq_wpb * 32, s->uq_smem, s->stream>>>(phases | PH_EXPORT_DYN, nsub, (const R*)action, s->slot, q);
     else unit_kernel<R, false><<<s->uq_grid, s->uq_wpb * 32, s->uq_smem, s->stream>>>(phases, nsub, (const R*)action, s->slot, q);
     unit_check_kernel<R><<<8, 256, 0, s->stream>>>(q, s->slot);
     s->launches += 3;

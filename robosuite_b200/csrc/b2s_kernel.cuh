@@ -83,12 +83,6 @@ DEVN void export_kinematics(const Eng<R> e, int env) {
   load_row(s.qfrc_passive + E * m.nv, e.p(L.passive), m.nv, lane);
 }
 
-template <typename R>
-DEVN void export_step1(const Eng<R> e, int env, int ncon) {
-  export_kinematics(e, env);
-  export_contacts(e, env, ncon);
-}
-
 // The constraint rows of this substep -> efc_type, efc_aref, efc_D, efc_R (zeros from row nefc on), efc_J (the first nefc * nv
 // entries), nefc, and contact_efc_address: a contact's first row, -1 for a contact without rows (not penetrating, or dropped by
 // the row budget) and for rows ncon .. maxcon - 1.  Reads J, the row headers and values and the contact headers, which
@@ -181,7 +175,8 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
   int warn = 0;
   for (int sub = 0; sub < nsub; sub++) {
     int ncon = 0, nefc = 0, niter = 0;
-    bool ex = live && (phases & PH_EXPORT) && sub == nsub - 1;
+    const bool last = live && sub == nsub - 1, ex = last && (phases & PH_EXPORT);
+    const int xm = ex ? EXP_ALL : last ? s.export_con | s.export_kin | s.export_dyn : 0;  // the array groups this substep writes
     __syncthreads();
     if (phases & PH_STEP1) {
       if (e.kinematics()) {  // diverged state reset to the model defaults (mj_checkPos / mj_checkVel)
@@ -193,19 +188,15 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
       e.crb();
       __syncthreads();
       ncon = collide(e, warn);
-      if (ex) export_step1(e, env, ncon);
-      else if (live && sub == nsub - 1) {
-        if (s.export_kin) export_kinematics(e, env);
-        if (s.export_con) export_contacts(e, env, ncon);
-      }
+      if (xm & EXP_STEP1) export_kinematics(e, env);
+      if (xm & EXP_CONTACTS) export_contacts(e, env, ncon);
       __syncthreads();
       nefc = make_constraint(e, ncon, warn);
       if (ex && !(phases & PH_STEP2)) export_efc(e, env, ncon, nefc);  // b2s_step1: no solve follows, the rows alone
     }
     if (phases & PH_CTRL) ctrl_run(e, cs, env, sub == 0 ? action : (const R*)nullptr);
     if (phases & PH_STEP2) {
-      // the full export, or the call's last substep with b2s_set_step2_export: one call site for both
-      const bool dyn = ex || (live && s.export_dyn && sub == nsub - 1);
+      const bool dyn = (xm & EXP_STEP2) != 0;
       e.actuation(dyn ? s.actuator_force + E * m.nu : nullptr);
       if (e.acceleration()) warn |= 1;
       __syncthreads();

@@ -27,6 +27,11 @@ enum {
   PH_OBS = 64        // write the observation row and the task outputs (after the last substep)
 };
 
+// the array groups the last substep of a step call writes (DState::export_*; PH_EXPORT writes all three): the contact records
+// (export_contacts), the step-1 arrays (export_kinematics) and the step-2 arrays (export_dynamics; the pipeline and the unit queue
+// run it in their DYN instantiations, launched with PH_EXPORT_DYN)
+enum { EXP_CONTACTS = 1, EXP_STEP1 = 2, EXP_STEP2 = 4, EXP_ALL = EXP_CONTACTS | EXP_STEP1 | EXP_STEP2 };
+
 template <typename R>
 struct DModel {
   int nq, nv, nu, nbody, njnt, ngeom, nsite, npair, ncg, nment, maxdepth, maxcon, maxefc, nmocap, nfl, nlim, nspr, hc_stride, max_treesize;
@@ -128,10 +133,9 @@ struct DState {
   int* solve_ls;   // [n_env] line-search evaluations of the environment's last Newton solve
   int* slowlog;    // [64][12] convex work items above 131 k cycles: cycles, shape types, hull sizes, EPA nV nF, GJK cycles, hit, staged, geoms
   const struct ObsModDev* obs_mod;  // sampling rates and corruptors (b2s_obs_modifiers); null: every observable on the last substep, no noise
-  int export_con;  // b2s_set_contact_export: the last substep of a step call writes contact_* / ncon in every schedule
-  int export_kin;  // b2s_set_step1_export: the last substep of a step call writes the step-1 arrays (export_kinematics) in every schedule
-  int export_dyn;  // b2s_set_step2_export: the fused kernel's last substep of a step call writes the step-2 arrays (export_dynamics); the
-                   // pipeline and the unit queue launch their DYN instantiations instead (PH_EXPORT_DYN)
+  // the array groups the last substep of a step call writes in every schedule, each field its EXP_* bit or 0 (three fields, not one
+  // mask: testing a bit of one cost the unit queue's flag-off kernel spill slots, DESIGN.md section 4)
+  int export_con, export_kin, export_dyn;  // b2s_set_contact_export, b2s_set_step1_export, b2s_set_step2_export
   int* contact_efc_address;  // [n_env, maxcon] first constraint row of each contact (mjContact.efc_address), -1: no rows / no contact
 };
 

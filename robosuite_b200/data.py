@@ -33,7 +33,7 @@ dropped by the row budget) has zero force.  It also needs the contact records (s
 
 class BatchedData:
     """The batched MjData of a BatchedSim (or a stand-in with the same surface: the named arrays as attributes, jac_site /
-    jac_body / jac_geom, full_m, `model`, and the `full_export` / `step1_export` flags)."""
+    jac_body / jac_geom, full_m, `model`, and the `full_export` / `step1_export` / `step2_export` / `contact_export` flags)."""
 
     def __init__(self, sim):
         self._sim = sim
@@ -41,24 +41,24 @@ class BatchedData:
         self._count = {"body": int(m.nbody), "site": int(m.nsite), "geom": int(m.ngeom)}
         self._colliding = {int(g) for p in m.pair_geom for g in p}
 
-    def _check(self):
-        s = self._sim
-        if not (s.full_export or s.step1_export):
-            raise RuntimeError("sim.data reads the step-1 arrays, which env_step / step write only with the step-1 export on: create "
-                               "the environment with make(..., data_queries=True) or call BatchedSim.set_step1_export(True)")
+    # what each kind of read needs: the BatchedSim flag of its export (the full export also serves) and the error without either
+    _NEEDS = {
+        "step1": ("step1_export", "sim.data reads the step-1 arrays, which env_step / step write only with the step-1 export on: "
+                  "create the environment with make(..., data_queries=True) or call BatchedSim.set_step1_export(True)"),
+        "step2": ("step2_export", "sim.data reads the step-2 arrays, which env_step / step write only with the step-2 export on: "
+                  "create the environment with make(..., dynamics_queries=True) or call BatchedSim.set_step2_export(True)"),
+        "contacts": ("contact_export", "contact_force() also reads the contact records, which env_step / step write only with the "
+                     "contact export on: create the environment with make(..., dynamics_queries=True) or call "
+                     "BatchedSim.set_contact_export(True)"),
+    }
 
-    def _array(self, name):
-        self._check()
-        return getattr(self._sim, name)
+    def _require(self, kind):
+        flag, msg = self._NEEDS[kind]
+        if not (self._sim.full_export or getattr(self._sim, flag)):
+            raise RuntimeError(msg)
 
-    def _check2(self):
-        s = self._sim
-        if not (s.full_export or getattr(s, "step2_export", False)):
-            raise RuntimeError("sim.data reads the step-2 arrays, which env_step / step write only with the step-2 export on: create "
-                               "the environment with make(..., dynamics_queries=True) or call BatchedSim.set_step2_export(True)")
-
-    def _array2(self, name):
-        self._check2()
+    def _array(self, name, kind):
+        self._require(kind)
         return getattr(self._sim, name)
 
     def _id(self, kind, obj):
@@ -78,33 +78,33 @@ class BatchedData:
         return i
 
     # ---- the data attributes, [N, k, ...] device views
-    body_xpos = property(lambda self: self._array("xpos"))
-    body_xquat = property(lambda self: self._array("xquat"))
-    body_xmat = property(lambda self: self._array("xmat"))
-    site_xpos = property(lambda self: self._array("site_xpos"))
-    site_xmat = property(lambda self: self._array("site_xmat"))
-    geom_xpos = property(lambda self: self._array("geom_xpos"))
-    geom_xmat = property(lambda self: self._array("geom_xmat"))
-    qM = property(lambda self: self._array("qM"))
-    cdof = property(lambda self: self._array("cdof"))
-    qfrc_bias = property(lambda self: self._array("qfrc_bias"))
-    qfrc_passive = property(lambda self: self._array("qfrc_passive"))
+    body_xpos = property(lambda self: self._array("xpos", "step1"))
+    body_xquat = property(lambda self: self._array("xquat", "step1"))
+    body_xmat = property(lambda self: self._array("xmat", "step1"))
+    site_xpos = property(lambda self: self._array("site_xpos", "step1"))
+    site_xmat = property(lambda self: self._array("site_xmat", "step1"))
+    geom_xpos = property(lambda self: self._array("geom_xpos", "step1"))
+    geom_xmat = property(lambda self: self._array("geom_xmat", "step1"))
+    qM = property(lambda self: self._array("qM", "step1"))
+    cdof = property(lambda self: self._array("cdof", "step1"))
+    qfrc_bias = property(lambda self: self._array("qfrc_bias", "step1"))
+    qfrc_passive = property(lambda self: self._array("qfrc_passive", "step1"))
 
     # ---- the step-2 arrays, [N, ...] device views; the row arrays at capacity (nefc says how many rows are valid)
     qacc = property(lambda self: self._sim.qacc)  # state: written by every step
-    qfrc_actuator = property(lambda self: self._array2("qfrc_actuator"))
-    actuator_force = property(lambda self: self._array2("actuator_force"))
-    qfrc_smooth = property(lambda self: self._array2("qfrc_smooth"))
-    qacc_smooth = property(lambda self: self._array2("qacc_smooth"))
-    qfrc_constraint = property(lambda self: self._array2("qfrc_constraint"))
-    nefc = property(lambda self: self._array2("nefc"))
-    efc_type = property(lambda self: self._array2("efc_type"))
-    efc_J = property(lambda self: self._array2("efc_J"))
-    efc_D = property(lambda self: self._array2("efc_D"))
-    efc_R = property(lambda self: self._array2("efc_R"))
-    efc_aref = property(lambda self: self._array2("efc_aref"))
-    efc_force = property(lambda self: self._array2("efc_force"))
-    solver_niter = property(lambda self: self._array2("solver_niter"))
+    qfrc_actuator = property(lambda self: self._array("qfrc_actuator", "step2"))
+    actuator_force = property(lambda self: self._array("actuator_force", "step2"))
+    qfrc_smooth = property(lambda self: self._array("qfrc_smooth", "step2"))
+    qacc_smooth = property(lambda self: self._array("qacc_smooth", "step2"))
+    qfrc_constraint = property(lambda self: self._array("qfrc_constraint", "step2"))
+    nefc = property(lambda self: self._array("nefc", "step2"))
+    efc_type = property(lambda self: self._array("efc_type", "step2"))
+    efc_J = property(lambda self: self._array("efc_J", "step2"))
+    efc_D = property(lambda self: self._array("efc_D", "step2"))
+    efc_R = property(lambda self: self._array("efc_R", "step2"))
+    efc_aref = property(lambda self: self._array("efc_aref", "step2"))
+    efc_force = property(lambda self: self._array("efc_force", "step2"))
+    solver_niter = property(lambda self: self._array("solver_niter", "step2"))
 
     def contact_force(self, contact=None):
         """mj_contactForce of every contact slot, [N, maxcon, 6], or of slot `contact` (an int), [N, 6]: force and torque in the
@@ -114,11 +114,8 @@ class BatchedData:
         if int(getattr(s.model, "opt_cone", 1)) != 1:
             raise NotImplementedError("contact_force() supports elliptic friction cones (cone=\"elliptic\") only; this model uses "
                                       "pyramidal cones")
-        self._check2()
-        if not (s.full_export or getattr(s, "contact_export", False)):
-            raise RuntimeError("contact_force() also reads the contact records, which env_step / step write only with the contact "
-                               "export on: create the environment with make(..., dynamics_queries=True) or call "
-                               "BatchedSim.set_contact_export(True)")
+        self._require("step2")
+        self._require("contacts")
         import torch
 
         adr, dim, ncon, f, nefc = s.contact_efc_address, s.contact_dim, s.ncon, s.efc_force, s.nefc
@@ -144,21 +141,21 @@ class BatchedData:
 
     def full_m(self):
         """mj_fullM: the dense mass matrices [N, nv, nv] (a copy)"""
-        self._check()
+        self._require("step1")
         return self._sim.full_m()
 
     # ---- poses
     def _pos(self, kind, obj):
-        return self._array({"body": "xpos"}.get(kind, kind + "_xpos"))[:, self._id(kind, obj)]
+        return self._array({"body": "xpos"}.get(kind, kind + "_xpos"), "step1")[:, self._id(kind, obj)]
 
     def _mat(self, kind, obj):
-        return self._array({"body": "xmat"}.get(kind, kind + "_xmat"))[:, self._id(kind, obj)].reshape(-1, 3, 3)
+        return self._array({"body": "xmat"}.get(kind, kind + "_xmat"), "step1")[:, self._id(kind, obj)].reshape(-1, 3, 3)
 
     def get_body_xpos(self, body):
         return self._pos("body", body)
 
     def get_body_xquat(self, body):
-        return self._array("xquat")[:, self._id("body", body)]
+        return self._array("xquat", "step1")[:, self._id("body", body)]
 
     def get_body_xmat(self, body):
         return self._mat("body", body)
@@ -177,7 +174,7 @@ class BatchedData:
 
     # ---- Jacobians and point velocities
     def _jac(self, kind, obj):
-        self._check()
+        self._require("step1")
         return getattr(self._sim, "jac_" + kind)(self._id(kind, obj))
 
     def _vel(self, jac):

@@ -412,19 +412,26 @@ class BatchedSim:
         self._check(self._L.b2s_set_export(self._h, int(bool(flag))))
         self.full_export = bool(flag)
 
+    # the array-group exports: the library's setter and the attribute that records the flag
+    _EXPORTS = {"contacts": ("b2s_set_contact_export", "contact_export"), "step1": ("b2s_set_step1_export", "step1_export"),
+                "step2": ("b2s_set_step2_export", "step2_export")}
+
+    def _set_group_export(self, group, flag):
+        fn, attr = self._EXPORTS[group]
+        self._check(getattr(self._L, fn)(self._h, int(bool(flag))))
+        setattr(self, attr, bool(flag))
+
     def set_step1_export(self, flag):
         """whether the last substep of every env_step / step writes the step-1 arrays (xpos, xquat, xmat, site / colliding-geom
         poses, qM, cdof, qfrc_bias, qfrc_passive: what `data` reads) in every mode, without the rest of the derived-array export
         (b2s_set_step1_export)"""
-        self._check(self._L.b2s_set_step1_export(self._h, int(bool(flag))))
-        self.step1_export = bool(flag)
+        self._set_group_export("step1", flag)
 
     def set_step2_export(self, flag):
         """whether the last substep of every env_step / step writes the step-2 arrays (qfrc_actuator, actuator_force, qfrc_smooth,
         qacc_smooth, qfrc_constraint, nefc, efc_*, solver_niter, contact_efc_address: what `data`'s dynamics properties and
         contact_force() read) in every mode, without the rest of the derived-array export (b2s_set_step2_export)"""
-        self._check(self._L.b2s_set_step2_export(self._h, int(bool(flag))))
-        self.step2_export = bool(flag)
+        self._set_group_export("step2", flag)
 
     @property
     def data(self):
@@ -440,8 +447,7 @@ class BatchedSim:
     def set_contact_export(self, flag):
         """whether the last substep of every env_step / step writes the contact arrays (contacts()) in every mode, without the
         rest of the derived-array export (b2s_set_contact_export)"""
-        self._check(self._L.b2s_set_contact_export(self._h, int(bool(flag))))
-        self.contact_export = bool(flag)
+        self._set_group_export("contacts", flag)
 
     def contacts(self):
         """device views of the contacts of the last substep: "ncon" [N], "geom" [N, maxcon, 2] (-1 beyond ncon), "dist"

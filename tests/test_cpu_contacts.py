@@ -1,11 +1,11 @@
 """CPU: the environment's contact queries (check_contact, get_contacts, _check_grasp, contact_geoms; robosuite_b200/envs/contacts.py)
-on the oracle-backed stand-in with the contact export (tests/oracle_sim_contacts.py): geom resolution, the reference's matching
+on the oracle-backed stand-in with the contact export (tests/oracle_sim_export.py): geom resolution, the reference's matching
 rules against the numpy restatement (tests/contact_ref.py), and the errors."""
 import numpy as np
 import pytest
 
 from tests import contact_ref as ref
-from tests.oracle_sim_contacts import ContactOracleSim
+from tests.oracle_sim_export import ExportOracleSim
 
 torch = pytest.importorskip("torch")
 
@@ -13,7 +13,7 @@ torch = pytest.importorskip("torch")
 def _env(n=2, contact_queries=True, task="Lift"):
     import robosuite_b200 as suite
 
-    return suite.make(task, robots="Panda", num_envs=n, seed=3, sim_cls=ContactOracleSim, precision="f64",
+    return suite.make(task, robots="Panda", num_envs=n, seed=3, sim_cls=ExportOracleSim, precision="f64",
                       contact_queries=contact_queries)
 
 

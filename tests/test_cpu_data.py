@@ -1,10 +1,10 @@
 """CPU: the batched MjData view (BatchedSim.data, robosuite_b200/data.py) on the oracle-backed stand-in with the step-1 export
-(tests/oracle_sim_data.py): name and id resolution, shapes, the xmat reshapes, the point velocities restated in numpy, and the
+(tests/oracle_sim_export.py): name and id resolution, shapes, the xmat reshapes, the point velocities restated in numpy, and the
 errors."""
 import numpy as np
 import pytest
 
-from tests.oracle_sim_data import DataOracleSim
+from tests.oracle_sim_export import ExportOracleSim
 
 torch = pytest.importorskip("torch")
 
@@ -14,7 +14,7 @@ SITE, BODY, GEOM = "gripper0_right_grip_site", "cube_main", "cube_g0"
 def _env(n=2, data_queries=True, task="Lift"):
     import robosuite_b200 as suite
 
-    return suite.make(task, robots="Panda", num_envs=n, seed=3, sim_cls=DataOracleSim, precision="f64", data_queries=data_queries)
+    return suite.make(task, robots="Panda", num_envs=n, seed=3, sim_cls=ExportOracleSim, precision="f64", data_queries=data_queries)
 
 
 @pytest.fixture(scope="module")

@@ -1,6 +1,6 @@
 """CPU: the step-2 half of the batched MjData view (BatchedSim.data's forces, constraint rows and contact_force(),
 robosuite_b200/data.py) on the oracle-backed stand-in with the step-2 export and the contact records
-(tests/oracle_sim_step2.py): make(..., dynamics_queries=True), shapes, contact_force() against the oracle's rows contact by
+(tests/oracle_sim_export.py): make(..., dynamics_queries=True), shapes, contact_force() against the oracle's rows contact by
 contact, the resting cube's contact forces summing to its weight, and the errors."""
 import copy
 import types
@@ -8,7 +8,7 @@ import types
 import numpy as np
 import pytest
 
-from tests.oracle_sim_step2 import Step2OracleSim
+from tests.oracle_sim_export import ExportOracleSim
 
 torch = pytest.importorskip("torch")
 
@@ -18,7 +18,7 @@ N = 2
 def _env(dynamics_queries=True, **kw):
     import robosuite_b200 as suite
 
-    return suite.make("Lift", robots="Panda", num_envs=N, seed=3, sim_cls=Step2OracleSim, precision="f64",
+    return suite.make("Lift", robots="Panda", num_envs=N, seed=3, sim_cls=ExportOracleSim, precision="f64",
                       dynamics_queries=dynamics_queries, **kw)
 
 

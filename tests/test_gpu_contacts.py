@@ -1,8 +1,6 @@
-"""GPU: the contact export (b2s_set_contact_export, BatchedSim.contacts) and the environment's contact queries.
+"""GPU: the contact export (b2s_set_contact_export, BatchedSim.contacts) and the environment's contact queries (every schedule
+writing the full export's records: tests/test_gpu_exports.py).
 
-* the pipeline and the unit queue write the same contact records as the fused kernel with the full export, bit for bit, through a
-  masked reset and with a small tier that sends environments to the large one;
-* switching the export on changes no other output in any schedule;
 * in f64 the records match the CPU oracle's data.contact (pairs and order exactly, geometry to 1e-12);
 * check_contact / get_contacts / _check_grasp equal the numpy restatement of the reference (tests/contact_ref.py) on the exported
   arrays, and _check_grasp of the task object equals the device's own grasp flag on the recorded grasp episodes;
@@ -11,68 +9,14 @@ import numpy as np
 import pytest
 
 from tests import contact_ref as ref
-from tests.oracle_sim_contacts import ContactOracleSim
-from tests.schedules import make_env, random_actions, switches
+from tests.oracle_sim_export import ExportOracleSim
+from tests.schedules import make_env, random_actions
 
 torch = pytest.importorskip("torch")
 
 pytestmark = pytest.mark.gpu
 
 TASKS = ["Lift", "Stack", "Door", "NutAssemblyRound", "PickPlace"]
-STATE = ("qpos", "qvel", "qacc", "ctrl", "obs", "task_out", "warn")
-TIER = (4, 20)  # small-tier capacities (contacts, rows): a cube resting on the table already needs more rows (4 contacts, 21 rows)
-
-
-def _rollout(task, precision, mode, export, n=16, steps=6):
-    """states after every step (and the masked reset before step 3), and the contact arrays when exported.  export: None, "contacts"
-    (make(contact_queries=True)) or "full" (set_export(True): the fused kernel with every derived array)"""
-    with switches(gjk_cache=False, ctrl_split=False):
-        env = make_env(task, n, mode, 5, gjk_cache=False, ctrl_split=False, tier_small=TIER, precision=precision,
-                       contact_queries=export == "contacts")
-        if export == "full":
-            env.sim.set_export(True)
-        acts = random_actions(env, steps)
-        acts[2:, : n // 2, 2] = -1  # half of the arms push down onto the table and the objects: more contacts
-        states, cons = [], []
-
-        def record():
-            states.append([getattr(env.sim, f).clone() for f in STATE])
-            if export:
-                cons.append([t.clone() for t in env.sim.contacts().values()] + ([env.sim.nefc.clone()] if export == "full" else []))
-
-        for t in range(steps):
-            if t == steps // 2:
-                mask = torch.zeros(n, dtype=torch.bool, device=env.device)
-                mask[::3] = True
-                env.reset(mask=mask)
-                record()
-            env.step(acts[t])
-            record()
-        torch.cuda.synchronize()
-        env.close()
-    return states, cons
-
-
-def _equal(a, b, tag):
-    for k, (x, y) in enumerate(zip(a, b)):
-        assert torch.equal(x, y), (tag, k)
-
-
-@pytest.mark.parametrize("precision", ["f32", "f64"])
-@pytest.mark.parametrize("task", TASKS)
-def test_schedules_write_the_fused_kernels_records(task, precision):
-    _, full = _rollout(task, precision, 0, "full")
-    # environments whose last substep did not fit the small tier (more contacts or rows than it holds) ran in the large one; the
-    # Door's arms touch the door only by chance, and its environments stay in the small tier
-    over = torch.stack([(c[0] > TIER[0]) | (c[-1] > TIER[1]) for c in full])
-    assert task == "Door" or bool(over.any()), task
-    for mode in (0, 1, 2):
-        s_off, _ = _rollout(task, precision, mode, None)
-        s_on, con = _rollout(task, precision, mode, "contacts")
-        for t, (a, b) in enumerate(zip(s_off, s_on)):
-            _equal(a, b, (task, precision, mode, "state", t))
-        for t, (a, b) in enumerate(zip(full, con)):
-            _equal(a, b, (task, precision, mode, "contacts", t))
 
 
 def _sync(cpu, dev):
@@ -108,7 +52,7 @@ def test_records_match_the_oracle_in_f64(task):
     n = 4
     kw = dict(robots="Panda", num_envs=n, seed=11, contact_queries=True)
     dev = suite.make(task, precision="f64", **kw)
-    cpu = suite.make(task, sim_cls=ContactOracleSim, precision="f64", **kw)
+    cpu = suite.make(task, sim_cls=ExportOracleSim, precision="f64", **kw)
     rng = np.random.default_rng(2)
     knife = compared = 0
     for t in range(5):

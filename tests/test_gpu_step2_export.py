@@ -1,11 +1,7 @@
 """GPU: the step-2 export (b2s_set_step2_export, BatchedSim.set_step2_export, make(..., dynamics_queries=True)) and the step-2
-half of the batched MjData view.
+half of the batched MjData view (every schedule writing the full export's arrays, and the flag changing no other output:
+tests/test_gpu_exports.py).
 
-* the pipeline (with the default group count and with one group), the unit queue and the fused kernel with the flag write the
-  same step-2 arrays and contact_efc_address as the fused kernel with the full export, bit for bit, through a masked reset and
-  with a small tier that sends environments to the large one;
-* switching the export on changes no other output (state, observations, task rows, contact records, step-1 arrays) in any
-  schedule, with the schedule-comparison switches and in the default configuration (GJK warm start on, OSC a phase-1 role);
 * in the default pipeline configuration, where the late pose load overlays the constraint Jacobian on the last substep, the
   exported arrays agree with themselves: qfrc_constraint = efc_J^T efc_force, qfrc_actuator = gear * actuator_force, and the
   exported qacc passes the solve's optimality certificate on the exported problem (tests/constraint_ref.py, with the gates of
@@ -23,7 +19,7 @@ import numpy as np
 import pytest
 
 from tests import constraint_ref as cr
-from tests.schedules import make_env, random_actions, switches
+from tests.schedules import make_env, random_actions
 from tests.test_gpu_constraint import GATES
 
 torch = pytest.importorskip("torch")
@@ -31,98 +27,11 @@ torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
 
 TASKS = ["Lift", "Stack", "Door", "NutAssemblyRound", "PickPlace"]
-STATE = ("qpos", "qvel", "qacc", "ctrl", "obs", "task_out", "warn")
-STEP1 = ("xpos", "xquat", "xmat", "site_xpos", "site_xmat", "geom_xpos", "geom_xmat", "qM", "cdof", "qfrc_bias", "qfrc_passive")
 STEP2 = ("qfrc_actuator", "actuator_force", "qfrc_smooth", "qacc_smooth", "qfrc_constraint", "nefc", "solver_niter",
          "contact_efc_address")
 ROWS = ("efc_type", "efc_D", "efc_R", "efc_aref", "efc_force")
-TIER = (4, 20)  # small-tier capacities (contacts, rows): a cube resting on the table already needs more rows (4 contacts, 21 rows)
 QCON_F32 = 5e-7
 CERT_F64 = 2e-6
-
-
-def _valid(sim):
-    """the step-2 arrays with only the valid rows of efc_* (the first nefc, and the first nefc * nv of efc_J), flattened"""
-    nefc = sim.nefc.long()
-    out = [getattr(sim, f).clone() for f in STEP2]
-    me = sim.efc_force.shape[1]
-    rows = torch.arange(me, device=nefc.device)[None, :] < nefc[:, None]
-    out += [getattr(sim, f)[rows].clone() for f in ROWS]
-    J = sim.efc_J.reshape(sim.efc_J.shape[0], -1)
-    out.append(J[torch.arange(J.shape[1], device=nefc.device)[None, :] < (nefc * sim.model.nv)[:, None]].clone())
-    return out
-
-
-def _rollout(task, precision, mode, export, groups=None, n=16, steps=6, default=False):
-    """outputs after every step (and the masked reset before step 3).  export: "off" (contact and step-1 exports), "on" (the same
-    and the step-2 export: make(dynamics_queries=True)) or "full" (set_export(True): the fused kernel with every derived array).
-    default: the library's default configuration (GJK warm start, OSC role, no small-tier override).  Returns (states, arrays):
-    states = the contact records (ncon first), the STATE fields, task_vec and the step-1 arrays; arrays = _valid's list, then
-    ncon (with the step-2 or the full export)"""
-    sw = dict(gjk_cache=default, ctrl_split=default, groups=groups)
-    with switches(**sw):
-        env = make_env(task, n, mode, 5, tier_small=None if default else TIER, precision=precision, contact_queries=True,
-                       data_queries=True, dynamics_queries=export == "on", **sw)
-        sim = env.sim
-        if export == "full":
-            sim.set_export(True)
-        acts = random_actions(env, steps)
-        acts[2:, : n // 2, 2] = -1  # half of the arms push down onto the table and the objects: more contacts
-        fields = STATE + (("task_vec",) if hasattr(sim, "task_vec") else ()) + STEP1
-        states, arrays = [], []
-
-        def record():
-            states.append([t.clone() for t in sim.contacts().values()] + [getattr(sim, f).clone() for f in fields])
-            if export != "off":
-                arrays.append(_valid(sim) + [sim.ncon.clone()])
-
-        for t in range(steps):
-            if t == steps // 2:
-                mask = torch.zeros(n, dtype=torch.bool, device=env.device)
-                mask[::3] = True
-                env.reset(mask=mask)
-                record()
-            env.step(acts[t])
-            record()
-        torch.cuda.synchronize()
-        env.close()
-    return states, arrays
-
-
-def _equal(a, b, tag):
-    assert len(a) == len(b), tag
-    for k, (x, y) in enumerate(zip(a, b)):
-        assert torch.equal(x, y), (tag, k)
-
-
-@pytest.mark.parametrize("precision", ["f32", "f64"])
-@pytest.mark.parametrize("task", TASKS)
-def test_schedules_write_the_fused_kernels_arrays(task, precision):
-    _, full = _rollout(task, precision, 0, "full")
-    # environments whose last substep did not fit the small tier ran in the large one; the Door's arms touch the door only by
-    # chance, and its environments stay in the small tier
-    nefc_at = STEP2.index("nefc")
-    over = torch.stack([(a[-1] > TIER[0]) | (a[nefc_at] > TIER[1]) for a in full])
-    assert task == "Door" or bool(over.any()), task
-    # the arrays are fresh after every step: the forces change
-    assert all(not torch.equal(full[t][0], full[t + 1][0]) for t in range(len(full) - 1))
-    for mode, groups in ((0, None), (1, None), (1, 1), (2, None)):
-        s_off, _ = _rollout(task, precision, mode, "off", groups)
-        s_on, arr = _rollout(task, precision, mode, "on", groups)
-        for t, (a, b) in enumerate(zip(s_off, s_on)):
-            _equal(a, b, (task, precision, mode, groups, "state", t))
-        for t, (a, b) in enumerate(zip(full, arr)):
-            _equal(a, b, (task, precision, mode, groups, "step2", t))
-
-
-@pytest.mark.parametrize("precision", ["f32", "f64"])
-@pytest.mark.parametrize("task", TASKS)
-def test_flag_changes_nothing_else_in_the_default_configuration(task, precision):
-    for mode in (0, 1, 2):
-        s_off, _ = _rollout(task, precision, mode, "off", default=True)
-        s_on, _ = _rollout(task, precision, mode, "on", default=True)
-        for t, (a, b) in enumerate(zip(s_off, s_on)):
-            _equal(a, b, (task, precision, mode, "default", t))
 
 
 def _blocks(model, efc_type, efc_J, ncon, adr, dim, fric, n, rd):
