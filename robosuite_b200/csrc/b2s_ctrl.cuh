@@ -8,9 +8,12 @@
 //   FixedBaseRobot.control (clip to ctrlrange)              robosuite/robots/fixed_base_robot.py:149-153
 #pragma once
 #include "b2s_solver.cuh"
+#include "b2s_oscmath.h"
 
 // small dense algebra of the controller runs in CA (double keeps Lambda = (J M^-1 J^T)^-1 well conditioned even
-// when the arm is near a singular pose; the blocks are 7x7 / 6x6 so the cost is negligible)
+// when the arm is near a singular pose; the blocks are 7x7 / 6x6 so the cost is negligible).  The operational-space inverses
+// keep numpy's pinv meaning (control_utils.py:74-76) with b2s_oscmath.h's tests: Cholesky / closed form far from the cut-off,
+// the Jacobi pseudo-inverse near it.
 typedef double CA;
 
 template <typename R> struct CtrlState {
@@ -256,7 +259,6 @@ DEVN void ctrl_run(Eng<R> e, CtrlState<R>& cs, int env, const R* action) {
   }
   __syncwarp();
   // Cholesky of the arm mass matrix (na x na) - column by column, lanes = rows
-  int bad = 0;
   for (int j = 0; j < na; j++) {
     if (lane >= j && lane < na) {
       CA sacc = Lc[lane * na + j];
@@ -265,7 +267,7 @@ DEVN void ctrl_run(Eng<R> e, CtrlState<R>& cs, int env, const R* action) {
     }
     __syncwarp();
     CA d = Lc[j * na + j];
-    if (!(d > 1e-300)) { bad = 1; d = 1e-300; }
+    if (!(d > 1e-300)) d = 1e-300;
     CA inv = rsqrt(d);
     __syncwarp();
     if (lane > j && lane < na) Lc[lane * na + j] *= inv;
@@ -302,24 +304,19 @@ DEVN void ctrl_run(Eng<R> e, CtrlState<R>& cs, int env, const R* action) {
     }
     for (int a = 0; a < na; a++) X[a * 6 + lane] = x[a];
   }
-  // 3x3 blocks: closed-form inverses -> decoupled wrench (lanes 6 / 7)
-  if (lane == 6 || lane == 7) {
+  // 3x3 blocks -> decoupled wrench (lanes 6 / 7): pinv of the packed block, closed form unless near numpy's cut-off
+  if (cc.uncouple && (lane == 6 || lane == 7)) {
     int o = lane == 6 ? 0 : 3;
-    CA a00 = Lf[(o + 0) * 6 + o], a01 = Lf[(o + 0) * 6 + o + 1], a02 = Lf[(o + 0) * 6 + o + 2];
-    CA a11 = Lf[(o + 1) * 6 + o + 1], a12 = Lf[(o + 1) * 6 + o + 2], a22 = Lf[(o + 2) * 6 + o + 2];
-    CA c00 = a11 * a22 - a12 * a12, c01 = a02 * a12 - a01 * a22, c02 = a01 * a12 - a02 * a11;
-    CA c11 = a00 * a22 - a02 * a02, c12 = a01 * a02 - a00 * a12, c22 = a00 * a11 - a01 * a01;
-    CA det = a00 * c00 + a01 * c01 + a02 * c02;
-    CA id = det != 0 ? 1.0 / det : 0.0;
-    CA f0 = F[o], f1 = F[o + 1], f2 = F[o + 2];
-    if (cc.uncouple) {
-      W[o] = (c00 * f0 + c01 * f1 + c02 * f2) * id;
-      W[o + 1] = (c01 * f0 + c11 * f1 + c12 * f2) * id;
-      W[o + 2] = (c02 * f0 + c12 * f1 + c22 * f2) * id;
-    }
+    const CA blk[6] = {Lf[o * 6 + o], Lf[(o + 1) * 6 + o], Lf[(o + 1) * 6 + o + 1],
+                       Lf[(o + 2) * 6 + o], Lf[(o + 2) * 6 + o + 1], Lf[(o + 2) * 6 + o + 2]};
+    osc_block3_apply(blk, 0, F + o, W + o);
   }
   __syncwarp();
-  // full 6x6: Cholesky of lambda_full_inv in Lw, inverse into Lf (lane = column of the identity)
+  // full 6x6: Cholesky of lambda_full_inv in Lw, inverse into Lf (lane = column of the identity).  The smallest pivot over the
+  // largest diagonal entry decides, as in osc_torques, whether the matrix may be within pinv's cut-off of singular: then lane 0
+  // replaces Lf (still lambda_full_inv) by its Jacobi pseudo-inverse instead.
+  CA dmax = 0, pmin = 1e300;
+  for (int j = 0; j < 6; j++) dmax = fmax(dmax, Lf[j * 7]);
   for (int j = 0; j < 6; j++) {
     if (lane >= j && lane < 6) {
       CA sacc = Lw[lane * 6 + j];
@@ -328,14 +325,17 @@ DEVN void ctrl_run(Eng<R> e, CtrlState<R>& cs, int env, const R* action) {
     }
     __syncwarp();
     CA d = Lw[j * 6 + j];
-    if (!(d > 1e-300)) { bad = 1; d = 1e-300; }
+    if (d < pmin) pmin = d;
+    if (!(d > 1e-300)) d = 1e-300;
     CA inv = rsqrt(d);
     __syncwarp();
     if (lane > j && lane < 6) Lw[lane * 6 + j] *= inv;
     if (lane == j) Lw[j * 6 + j] = inv;
     __syncwarp();
   }
-  if (lane < 6) {
+  if (!(dmax > 0 && pmin / dmax > 1e-11)) {
+    if (lane == 0) osc_pinv_sym_jacobi(Lf, 6);
+  } else if (lane < 6) {
     CA x[6];
     for (int a = 0; a < 6; a++) {
       CA sacc = a == lane ? 1.0 : 0.0;
@@ -391,7 +391,6 @@ DEVN void ctrl_run(Eng<R> e, CtrlState<R>& cs, int env, const R* action) {
     R lo = m.act_ctrlrange[2 * u], hi = m.act_ctrlrange[2 * u + 1];
     ctrl[u] = r_clamp(R(0.5) * (hi + lo) + R(0.5) * (hi - lo) * cs.grip[lane], lo, hi);
   }
-  (void)bad;
   __syncwarp();
 }
 

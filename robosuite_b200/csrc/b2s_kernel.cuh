@@ -194,7 +194,9 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
       nefc = make_constraint(e, ncon, warn);
       if (ex && !(phases & PH_STEP2)) export_efc(e, env, ncon, nefc);  // b2s_step1: no solve follows, the rows alone
     }
-    if (phases & PH_CTRL) ctrl_run(e, cs, env, sub == 0 ? action : (const R*)nullptr);
+    // a shadow warp skips the controller: the joint controllers update their state in HBM in place, and a second warp doing so
+    // for the same environment would race it (the joint-velocity integral and derivative ring taking the substep twice)
+    if (live && (phases & PH_CTRL)) ctrl_run(e, cs, env, sub == 0 ? action : (const R*)nullptr);
     if (phases & PH_STEP2) {
       const bool dyn = (xm & EXP_STEP2) != 0;
       e.actuation(dyn ? s.actuator_force + E * m.nu : nullptr);

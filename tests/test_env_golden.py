@@ -56,7 +56,7 @@ def test_oracle_env_step_matches_reference_stack(task):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("task", TASKS + ["Lift_JOINT_POSITION", "Lift_JOINT_TORQUE"])
+@pytest.mark.parametrize("task", TASKS + ["Lift_JOINT_POSITION", "Lift_JOINT_TORQUE", "Lift_OSC_POSITION"])
 def test_env_api_matches_reference_stack(task):
     """observations (layout, order, sampling instant, lagged object-in-gripper poses), rewards and state after every control
     step, fp32 engine vs the reference stack on the fp64 oracle"""
@@ -68,7 +68,7 @@ def test_env_api_matches_reference_stack(task):
     m = _model(task, G)
     n = 2
     kw = {}
-    if "JOINT" in task:
+    if "JOINT" in task or "OSC_POSITION" in task:
         from robosuite_b200 import controller_config as cc
 
         kw["controller_configs"] = cc.refactor_composite_controller_config(cc.load_part_controller_config(task.split("_", 1)[1]), "Panda", ["right"])
