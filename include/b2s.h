@@ -106,6 +106,26 @@ typedef struct {
   int jv_use_vel_limits, jv_torque_comp;
 } b2s_ctrl_cfg;
 int b2s_ctrl_config(b2s_sim* sim, const b2s_ctrl_cfg* cfg);
+/* impedance_mode of OSC_POSE, OSC_POSITION and JOINT_POSITION, for the controller b2s_ctrl_config configured last (which itself
+ * always configures FIXED, so b2s_ctrl_cfg keeps its size and every field its offset).  FIXED uses the gains of b2s_ctrl_cfg.
+ * VARIABLE and VARIABLE_KP take the gains from the action at every policy step (osc.py / joint_pos.py set_goal, recalled from
+ * robosuite v1.5; no reference checkout was available to check them against).  With d = 6 for both OSC kinds (OSC_POSITION keeps a
+ * 6-dim kp and holds orientation with kp[3:6]) and d = n_arm for JOINT_POSITION, and od = 3 / 6 / n_arm delta entries:
+ *   VARIABLE     action = [damping_ratio (d), kp (d), delta (od), gripper]   kp = clip(kp, kp_min, kp_max),
+ *                                                                           kd = 2 sqrt(kp) clip(damping_ratio, dr_min, dr_max)
+ *   VARIABLE_KP  action = [kp (d), delta (od), gripper]                      kp = clip(kp, kp_min, kp_max), kd = 2 sqrt(kp)
+ * so action_dim is 2 d + od + 1 or d + od + 1.  The gain parts are only clipped (input_* / output_* scale the delta).  The gains of
+ * each environment live in the array "ctrl_gain" [n_env, 16] f64 (kp[8], kd[8]) in both precisions; this call and b2s_ctrl_reset
+ * (so b2s_reset_envs) write the configured gains (kd = 2 sqrt(kp) damping_ratio) into it, as the reference rebuilds its controllers
+ * at reset.  While a variable mode is configured the array is a snapshot section.  B2S_ERR_ARG: an unknown mode, and in a variable
+ * mode: another kind, a limit among the first d entries that is non-finite or negative or has min > max, or an action_dim other than
+ * the layout's; the handle then stays in FIXED mode. */
+enum { B2S_IMPEDANCE_FIXED = 0, B2S_IMPEDANCE_VARIABLE = 1, B2S_IMPEDANCE_VARIABLE_KP = 2 };
+typedef struct {
+  int impedance_mode; /* B2S_IMPEDANCE_* */
+  double kp_min[8], kp_max[8], damping_ratio_min[8], damping_ratio_max[8];
+} b2s_impedance_cfg;
+int b2s_ctrl_impedance(b2s_sim* sim, const b2s_impedance_cfg* cfg);
 /* controller.reset_goal + update_initial_joints (osc.py:520-544) for masked envs (NULL = all); needs a prior forward */
 int b2s_ctrl_reset(b2s_sim* sim, const uint8_t* env_mask);
 int b2s_env_step(b2s_sim* sim, const void* action, int n_substeps);
@@ -232,6 +252,7 @@ int b2s_task_table(b2s_sim* sim, int n, const int* op, const int* a, const int* 
  *   always           qpos qvel qacc qacc_warmstart ctrl time, warn (i32), ctrl_goal_pos ctrl_goal_ori ctrl_initial_joint ctrl_grip_state
  *                    ctrl_jv_state ctrl_torque, gjk_cache (npair x 3; written as zeros and ignored on restore while the handle has no
  *                    cache: fused mode before the pipeline's first use, or B2S_NO_GJK_CACHE)
+ *   variable impedance  ctrl_gain (f64), while b2s_ctrl_impedance has a variable mode configured; the mode is then part of the signature
  *   b2s_obs_config   obs, obs_fresh (i32), task_out
  *   b2s_obs_modifiers  obs_timer (f64), obs_sampled (i32), obs_nsample (i32), while configured
  *   b2s_task_table   task_vec

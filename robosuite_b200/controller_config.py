@@ -4,6 +4,11 @@ Accepts the reference's composite controller JSON/dict schema unchanged
 (`robosuite/controllers/config/robots/default_panda.json`, `config/default/parts/osc_pose.json`; selection logic
 `robosuite/controllers/parts/controller_factory.py:145-159`) and resolves the model indices the way
 `robosuite/robots/robot.py:302-332,911-979` does (joint / actuator / site name lookups by naming prefix).
+
+OSC_POSE, OSC_POSITION and JOINT_POSITION take `impedance_mode` "fixed", "variable" or "variable_kp" with `kp_limits` and
+`damping_ratio_limits`: in the variable modes the policy sets the gains at every control step through the action (see `_impedance`
+for the layout; `action_dim` and `BatchedMujocoEnv.action_spec` follow it).  Not implemented, with NotImplementedError: absolute
+inputs, `input_ref_frame` "world", interpolators and `qpos_limits`.
 """
 import json
 import os
@@ -86,6 +91,32 @@ def _arr(v, n):
     return np.full(n, float(a)) if a.ndim == 0 else a.astype(np.float64)
 
 
+# impedance_mode (osc.py, joint_pos.py IMPEDANCE_MODES) -> b2s_ctrl_cfg.impedance_mode (B2S_IMPEDANCE_*); the arm kinds that have one
+IMPEDANCE_MODES = {"fixed": 0, "variable": 1, "variable_kp": 2}
+IMPEDANCE_KINDS = ("OSC_POSE", "OSC_POSITION", "JOINT_POSITION")
+
+
+def _impedance(c, arm, d, od):
+    """impedance_mode, the gain limits (nums2array: broadcast to d = 6 for OSC, n_arm for JOINT_POSITION) and action_dim: the
+    action is [damping_ratio (d), kp (d), delta (od), gripper] in "variable" mode, [kp (d), delta (od), gripper] in "variable_kp",
+    [delta (od), gripper] in "fixed".  These layouts and the clip of the gains are recalled from robosuite v1.5 (osc.py,
+    joint_pos.py set_goal / control_limits); no reference checkout was available to check them against."""
+    mode = IMPEDANCE_MODES[arm.get("impedance_mode", "fixed")]
+    c.action_dim = (0 if mode == 0 else d if mode == 2 else 2 * d) + od + 1
+    if mode == 0:
+        return
+    if "impedance_mode" not in (f for f, _ in type(c)._fields_):
+        raise NotImplementedError(f"{type(c).__name__} has no variable impedance fields")
+    kpl, drl = arm.get("kp_limits", [0, 300]), arm.get("damping_ratio_limits", [0, 10])
+    lim = [_arr(kpl[0], d), _arr(kpl[1], d), _arr(drl[0], d), _arr(drl[1], d)]
+    c.impedance_mode = mode
+    for name, v in zip(("kp_min", "kp_max", "damping_ratio_min", "damping_ratio_max"), lim):
+        if v.shape != (d,):
+            raise ValueError(f"{name}: expected a scalar or {d} values, got {v.shape}")
+        for k in range(d):
+            getattr(c, name)[k] = v[k]
+
+
 def resolve(model, composite_cfg, cfg_struct_cls, robot_prefix="robot0_", gripper_prefix="gripper0_right_", gripper="panda"):
     """Build the C struct (engine.CtrlCfg or the oracle's CtrlCfg: same layout) for one fixed-base arm + gripper."""
     if composite_cfg.get("type", "BASIC") != "BASIC":
@@ -93,14 +124,16 @@ def resolve(model, composite_cfg, cfg_struct_cls, robot_prefix="robot0_", grippe
     arm = composite_cfg["body_parts"]["arms"]["right"]
     if arm["type"] not in ("OSC_POSE", "OSC_POSITION", "JOINT_VELOCITY", "JOINT_POSITION", "JOINT_TORQUE"):
         raise NotImplementedError(f"arm controller type {arm['type']} not implemented in the fused path")
-    if arm["type"] == "JOINT_POSITION" and (arm.get("impedance_mode", "fixed") != "fixed" or arm.get("input_type", "delta") != "delta"
-                                            or arm.get("qpos_limits") is not None):
-        raise NotImplementedError("JOINT_POSITION: fixed impedance, delta inputs, no qpos_limits")
+    if arm["type"] in IMPEDANCE_KINDS and arm.get("impedance_mode", "fixed") not in IMPEDANCE_MODES:
+        # the reference asserts the same at construction (osc.py, joint_pos.py: `impedance_mode in IMPEDANCE_MODES`)
+        raise ValueError(f"{arm['type']}: unsupported impedance mode {arm.get('impedance_mode')!r}, not one of {sorted(IMPEDANCE_MODES)}")
+    if arm["type"] == "JOINT_POSITION" and (arm.get("input_type", "delta") != "delta" or arm.get("qpos_limits") is not None):
+        raise NotImplementedError("JOINT_POSITION: delta inputs, no qpos_limits")
     if arm["type"] == "JOINT_TORQUE" and arm.get("torque_limits") is not None:
         raise NotImplementedError("JOINT_TORQUE: torque_limits other than the actuator limits are not implemented")
-    if arm["type"] in ("OSC_POSE", "OSC_POSITION") and (arm.get("impedance_mode", "fixed") != "fixed" or arm.get("input_type", "delta") != "delta"
-                                      or arm.get("input_ref_frame", "base") != "base" or arm.get("interpolation") is not None):
-        raise NotImplementedError("fused OSC path implements fixed impedance, delta inputs in the base frame")
+    if arm["type"] in ("OSC_POSE", "OSC_POSITION") and (arm.get("input_type", "delta") != "delta"
+                                                        or arm.get("input_ref_frame", "base") != "base" or arm.get("interpolation") is not None):
+        raise NotImplementedError("fused OSC path implements delta inputs in the base frame")
     if arm.get("interpolation") is not None:
         raise NotImplementedError("interpolators are not implemented")
     if arm["type"] in ("OSC_POSE", "OSC_POSITION"):
@@ -146,6 +179,8 @@ def resolve(model, composite_cfg, cfg_struct_cls, robot_prefix="robot0_", grippe
         c.null_kp = 10.0
         c.uncouple_pos_ori = 1
         c.n_obs_site = 0
+        if arm["type"] == "JOINT_POSITION":
+            _impedance(c, arm, n, n)
         return c
     if arm["type"] == "JOINT_VELOCITY":
         n = c.n_arm
@@ -169,7 +204,6 @@ def resolve(model, composite_cfg, cfg_struct_cls, robot_prefix="robot0_", grippe
         c.n_obs_site = 0
         return c
     od = 3 if arm["type"] == "OSC_POSITION" else 6
-    c.action_dim = od + 1
     kp, dr = _arr6(arm["kp"]), _arr6(arm["damping_ratio"])
 
     def _lim(v):  # OSC_POSITION carries 3-vectors (osc.py:165): pad the unused orientation slots
@@ -184,4 +218,5 @@ def resolve(model, composite_cfg, cfg_struct_cls, robot_prefix="robot0_", grippe
     c.null_kp = 10.0
     c.uncouple_pos_ori = int(bool(arm.get("uncouple_pos_ori", True)))
     c.n_obs_site = 0
+    _impedance(c, arm, 6, od)
     return c

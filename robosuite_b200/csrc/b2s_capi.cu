@@ -71,6 +71,7 @@ uint64_t Blob::hash() const {
 struct ArrayInfo { void* ptr; int dtype; int ndim; int64_t shape[4]; };
 struct SnapSecHost { std::string name; int64_t off, count; int dtype; void* ptr; };  // off: bytes into the row; count: elements per env
 #define SNAP_MAXSEC 128
+#define B2S_MAX_ACTION 32  // action entries per environment the pipeline stages (joint position with variable impedance: 3 n_arm + 1)
 
 struct b2s_sim {
   int n_env = 0, device = 0, precision = B2S_F32;
@@ -140,6 +141,11 @@ struct b2s_sim {
   // whether a configuration is active, the model's timestep in fp64
   ObsModDev* obs_mod_dev = nullptr;
   int obs_arr_n = 0, obs_mod_on = 0;
+  // variable impedance (b2s_ctrl_impedance): the device table and the gain rows [n_env, 16] f64, both allocated at the first
+  // configuration with a variable mode and kept; CtrlCfgDev::imp / gain point at them only while such a mode is configured
+  ImpDev* imp_dev = nullptr;
+  double* gain_rows = nullptr;
+  int imp_mode = 0;
   double timestep_h = 0;
   std::vector<char> body_free_h;  // body b has a free joint (b2s_obs_objects takes only such bodies)
 };
@@ -945,7 +951,7 @@ template <typename R> static int ensure_ws(b2s_sim* s, const DModel<R>& m, DStat
     st.cl_outA = dev_zeros<R>(s, ne * st.cl_maxa * CL_RECA); st.cl_outG = dev_zeros<R>(s, ne * st.cl_maxg * 8);
     st.cl_env = dev_zeros<int>(s, ne * CL_ENVW(st));
     st.gjk_cache = getenv("B2S_NO_GJK_CACHE") ? nullptr : dev_zeros<R>(s, ne * (size_t)m.npair * 3);
-    s->action_buf = dev_zeros<R>(s, ne * 16);
+    s->action_buf = dev_zeros<R>(s, ne * B2S_MAX_ACTION);
 #ifdef B2S_INSTR
     st.st_begin = dev_zeros<unsigned long long>(s, 64 * 32 * 8); st.st_end = dev_zeros<unsigned long long>(s, 64 * 32 * 8);
     st.stats = dev_zeros<int>(s, 512); st.cyc = dev_zeros<float>(s, ne * 32 * 8); st.solve_ls = dev_zeros<int>(s, ne);
@@ -994,7 +1000,7 @@ static int launch_pipeline(b2s_sim* s, int phases, int nsub, const void* action)
     const R* act_in = (const R*)action;
     if (action) {
       int ad = s->ctrl.action_dim > 0 ? s->ctrl.action_dim : 1;
-      if (ad > 16) return fail(B2S_ERR_UNSUPPORTED, "action_dim > 16");
+      if (ad > B2S_MAX_ACTION) return fail(B2S_ERR_UNSUPPORTED, "action_dim > 32");
       CUDA_TRY(cudaMemcpyAsync(s->action_buf, action, (size_t)s->n_env * ad * sizeof(R), cudaMemcpyDeviceToDevice, s->stream));
       act_in = (const R*)s->action_buf;
     }
@@ -1263,9 +1269,64 @@ int b2s_ctrl_config(b2s_sim* s, const b2s_ctrl_cfg* c) {
     d.jv_in_max[i] = c->jv_in_max[i]; d.jv_in_min[i] = c->jv_in_min[i]; d.jv_out_max[i] = c->jv_out_max[i]; d.jv_out_min[i] = c->jv_out_min[i];
   }
   d.jv_vel_lo = c->jv_vel_lo; d.jv_vel_hi = c->jv_vel_hi; d.jv_use_vel_limits = c->jv_use_vel_limits; d.jv_torque_comp = c->jv_torque_comp;
+  d.imp = nullptr; d.gain = nullptr;  // fixed impedance until b2s_ctrl_impedance
+  s->arrays.erase("ctrl_gain");
+  s->imp_mode = B2S_IMPEDANCE_FIXED;
   s->has_ctrl = c->kind != B2S_CTRL_NONE;
   s->dirty = 1;
   s->layout_version++;  // the controller kind is part of the snapshot signature
+  return B2S_OK;
+}
+
+int b2s_ctrl_impedance(b2s_sim* s, const b2s_impedance_cfg* c) {
+  if (!s || !c) return fail(B2S_ERR_ARG, "b2s_ctrl_impedance: bad argument");
+  const int mode = c->impedance_mode;
+  if (mode != B2S_IMPEDANCE_FIXED && mode != B2S_IMPEDANCE_VARIABLE && mode != B2S_IMPEDANCE_VARIABLE_KP)
+    return fail(B2S_ERR_ARG, "b2s_ctrl_impedance: unknown impedance_mode " + std::to_string(mode));
+  CtrlCfgDev& d = s->ctrl;
+  ImpDev im{};
+  if (mode != B2S_IMPEDANCE_FIXED) {
+    if (d.kind != B2S_CTRL_OSC_POSE && d.kind != B2S_CTRL_OSC_POSITION && d.kind != B2S_CTRL_JOINT_POSITION)
+      return fail(B2S_ERR_ARG, "b2s_ctrl_impedance: variable impedance needs OSC_POSE, OSC_POSITION or JOINT_POSITION");
+    const bool joint = d.kind == B2S_CTRL_JOINT_POSITION;
+    im.mode = mode; im.d = joint ? d.n_arm : 6; im.off = mode == B2S_IMPEDANCE_VARIABLE ? 2 * im.d : im.d;
+    for (int k = 0; k < im.d; k++) {
+      const double v[4] = {c->kp_min[k], c->kp_max[k], c->damping_ratio_min[k], c->damping_ratio_max[k]};
+      for (double x : v)
+        if (!std::isfinite(x) || x < 0) return fail(B2S_ERR_ARG, "b2s_ctrl_impedance: limits must be finite and non-negative");
+      if (v[0] > v[1] || v[2] > v[3]) return fail(B2S_ERR_ARG, "b2s_ctrl_impedance: a limit has min > max");
+      im.kp_min[k] = v[0]; im.kp_max[k] = v[1]; im.dr_min[k] = v[2]; im.dr_max[k] = v[3];
+    }
+    const int od = joint ? d.n_arm : (d.kind == B2S_CTRL_OSC_POSITION ? 3 : 6);
+    if (d.action_dim != im.off + od + 1)
+      return fail(B2S_ERR_ARG, "b2s_ctrl_impedance: action_dim " + std::to_string(d.action_dim) + " does not match the layout (" +
+                               std::to_string(im.off + od + 1) + ")");
+  }
+  d.imp = nullptr; d.gain = nullptr;
+  s->arrays.erase("ctrl_gain");
+  s->imp_mode = mode;
+  if (mode != B2S_IMPEDANCE_FIXED) {
+    CUDA_TRY(cudaSetDevice(s->device));
+    const bool joint = d.kind == B2S_CTRL_JOINT_POSITION;
+    std::vector<double> rows((size_t)s->n_env * 16, 0.0);  // the configured gains, as b2s_ctrl_reset writes them
+    for (size_t e = 0; e < (size_t)s->n_env; e++)
+      for (int k = 0; k < im.d; k++) {
+        rows[e * 16 + k] = joint ? d.jv_kp[k] : d.kp[k];
+        rows[e * 16 + 8 + k] = joint ? d.jv_kd[k] : d.kd[k];
+      }
+    try {
+      if (!s->imp_dev) s->imp_dev = dev_zeros<ImpDev>(s, 1);
+      if (!s->gain_rows) s->gain_rows = dev_zeros<double>(s, (size_t)s->n_env * 16);
+    } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
+    // stream-ordered behind the kernels that read the previous table / rows
+    CUDA_TRY(cudaMemcpyAsync(s->imp_dev, &im, sizeof(im), cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaMemcpyAsync(s->gain_rows, rows.data(), rows.size() * sizeof(double), cudaMemcpyHostToDevice, s->stream));
+    CUDA_TRY(cudaStreamSynchronize(s->stream));  // pageable sources
+    d.imp = s->imp_dev; d.gain = s->gain_rows;
+    s->arrays["ctrl_gain"] = ArrayInfo{s->gain_rows, B2S_F64, 2, {s->n_env, 16, 0, 0}};
+  }
+  s->dirty = 1;
+  s->layout_version++;  // the gain rows and the mode are part of the snapshot layout and signature
   return B2S_OK;
 }
 
@@ -1743,6 +1804,7 @@ static int ensure_snap(b2s_sim* s) {
     add("warn", st.warn, 1, B2S_I32);
     add("ctrl_goal_pos", st.goal_pos, 3, R); add("ctrl_goal_ori", st.goal_ori, 9, R); add("ctrl_initial_joint", st.init_qpos_arm, 8, R);
     add("ctrl_grip_state", st.grip_state, 4, R); add("ctrl_jv_state", st.jv_state, 72, R); add("ctrl_torque", st.ctrl_torque, 8, R);
+    if (s->ctrl.gain) add("ctrl_gain", s->ctrl.gain, 16, B2S_F64);
     add("gjk_cache", st.gjk_cache, (int64_t)m.npair * 3, R);  // null until the pipeline's first use, or with B2S_NO_GJK_CACHE
     if (s->has_obs) { add("obs", st.obs, s->ctrl.obs_dim, R); add("obs_fresh", st.obs_fresh, 1, B2S_I32); add("task_out", st.task_out, 8, R); }
     if (s->obs_mod_on) {
@@ -1792,6 +1854,7 @@ static int ensure_snap(b2s_sim* s) {
   h = fnv1a(h, &no, sizeof(int)); h = fnv1a(h, s->obs_tab_h.data(), sizeof(int) * no);
   h = fnv1a(h, &nt, sizeof(int)); h = fnv1a(h, s->task_tab_h.data(), sizeof(int) * nt);
   h = fnv1a(h, &s->blob_hash, sizeof(uint64_t));
+  if (s->ctrl.gain) h = fnv1a(h, &s->imp_mode, sizeof(int));  // variable impedance: the action layout (fixed mode hashes nothing new)
   if (s->ctrl.n_sel > 0) {  // the object list (a handle without one hashes what it always did)
     h = fnv1a(h, &s->ctrl.n_sel, sizeof(int)); h = fnv1a(h, s->ctrl.sel_body, sizeof(int) * s->ctrl.n_sel);
   }

@@ -75,9 +75,12 @@ DEVN void ctrl_run_joint(Eng<R> e, CtrlState<R>& cs, int env, const R* action) {
   R* st = s.jv_state + (size_t)env * 72;
   R* ctrl = e.p(L.ctrl);
   int k = lane < na ? lane : 0, dof = cc.arm_dof[k], u = cc.arm_act[k];
+  const int off = cc.imp ? cc.imp->off : 0;  // variable impedance: the delta follows the gains
+  const size_t G = (size_t)env * 16;  // this environment's gain row
   R goal = st[k];
   if (action && lane < na) {
-    R a = r_clamp(action[(size_t)env * cc.action_dim + k], (R)cc.jv_in_min[k], (R)cc.jv_in_max[k]);
+    if (cc.gain) imp_gain(cc.imp, action + (size_t)env * cc.action_dim, k, cc.gain + G + k, cc.gain + G + 8 + k);  // before the goal
+    R a = r_clamp(action[(size_t)env * cc.action_dim + off + k], (R)cc.jv_in_min[k], (R)cc.jv_in_max[k]);
     R scale = (R)(fabs(cc.jv_out_max[k] - cc.jv_out_min[k]) / fabs(cc.jv_in_max[k] - cc.jv_in_min[k]));
     R sc = (a - (R)(0.5 * (cc.jv_in_max[k] + cc.jv_in_min[k]))) * scale + (R)(0.5 * (cc.jv_out_max[k] + cc.jv_out_min[k]));
     goal = cc.kind == 3 ? e.p(L.qpos)[cc.arm_qpos[k]] + sc : r_clamp(sc, m.act_ctrlrange[2 * u], m.act_ctrlrange[2 * u + 1]);
@@ -85,7 +88,9 @@ DEVN void ctrl_run_joint(Eng<R> e, CtrlState<R>& cs, int env, const R* action) {
   }
   R tau;
   if (cc.kind == 3) {
-    R des = lane < na ? (goal - e.p(L.qpos)[cc.arm_qpos[k]]) * (R)cc.jv_kp[k] - e.p(L.qvel)[dof] * (R)cc.jv_kd[k] : R(0);
+    R kp = (R)cc.jv_kp[k], kd = (R)cc.jv_kd[k];
+    if (cc.gain) { kp = (R)cc.gain[G + k]; kd = (R)cc.gain[G + 8 + k]; }
+    R des = lane < na ? (goal - e.p(L.qpos)[cc.arm_qpos[k]]) * kp - e.p(L.qvel)[dof] * kd : R(0);
     tau = 0;
     for (int b = 0; b < na; b++) {
       R db = __shfl_sync(B2S_FULL, des, b);
@@ -100,7 +105,7 @@ DEVN void ctrl_run_joint(Eng<R> e, CtrlState<R>& cs, int env, const R* action) {
     ctrl[u] = r_clamp(tau, m.act_ctrlrange[2 * u], m.act_ctrlrange[2 * u + 1]);
   }
   if (action) {
-    R ga = action[(size_t)env * cc.action_dim + na];
+    R ga = action[(size_t)env * cc.action_dim + off + na];
     R sg = ga > 0 ? R(1) : (ga < 0 ? R(-1) : R(0));
     for (int g = 0; g < cc.n_grip; g++) cs.grip[g] = r_clamp(cs.grip[g] + (R)(cc.grip_sign[g] * cc.grip_speed) * sg, R(-1), R(1));
   }
@@ -179,8 +184,11 @@ DEVN void ctrl_run(Eng<R> e, CtrlState<R>& cs, int env, const R* action) {
   int lane = e.lane, nv = m.nv, na = cc.n_arm;
   const R* ref_pos = e.p(L.spos) + 3 * cc.eef_site; const R* ref_ori = e.p(L.smat) + 9 * cc.eef_site;
   const R* org_pos = e.p(L.spos) + 3 * cc.base_site; const R* org_ori = e.p(L.smat) + 9 * cc.base_site;
+  const size_t G = (size_t)env * 16;  // this environment's gain row (variable impedance)
   if (policy_step) {
     const R* act = action + (size_t)env * cc.action_dim;
+    if (cc.gain && lane < 6) imp_gain(cc.imp, act, lane, cc.gain + G + lane, cc.gain + G + 8 + lane);  // before the goal, as set_goal
+    if (cc.imp) act += cc.imp->off;  // the delta follows the gains
     const int od = cc.kind == 5 ? 3 : 6;  // OSC_POSITION (osc.py:152-166, 259-270): 3-dim arm action, zero orientation delta
     R sd[6] = {0, 0, 0, 0, 0, 0};
     for (int k = 0; k < od; k++) {
@@ -255,7 +263,10 @@ DEVN void ctrl_run(Eng<R> e, CtrlState<R>& cs, int env, const R* action) {
     const R* bv = cvel + 6 * bb;
     v3cross(t, bv, org_pos);
     bvel[0] = bv[3] + t[0]; bvel[1] = bv[4] + t[1]; bvel[2] = bv[5] + t[2]; bvel[3] = bv[0]; bvel[4] = bv[1]; bvel[5] = bv[2];
-    if (lane < 6) F[lane] = (CA)err[lane] * cc.kp[lane] - ((CA)vel[lane] - (CA)bvel[lane]) * cc.kd[lane];
+    if (lane < 6) {  // this lane wrote its own gains on a policy substep
+      const CA kp = cc.gain ? cc.gain[G + lane] : cc.kp[lane], kd = cc.gain ? cc.gain[G + 8 + lane] : cc.kd[lane];
+      F[lane] = (CA)err[lane] * kp - ((CA)vel[lane] - (CA)bvel[lane]) * kd;
+    }
   }
   __syncwarp();
   // Cholesky of the arm mass matrix (na x na) - column by column, lanes = rows
@@ -614,4 +625,10 @@ __global__ void ctrl_reset_kernel(const uint8_t* mask, int slot) {
   for (int k = 0; k < 72; k++) s.jv_state[E * 72 + k] = k == 64 ? R(4) : R(0);  // ring pointer starts at length - 1
   if (cc.kind == 3)  // JointPositionController.reset_goal: goal <- current joint positions
     for (int k = 0; k < cc.n_arm; k++) s.jv_state[E * 72 + k] = s.qpos[E * m.nq + cc.arm_qpos[k]];
+  if (cc.gain)  // variable impedance: the rebuilt controller starts from the configured gains
+    for (int k = 0; k < 8; k++) {
+      const bool osc = cc.kind != 3, on = k < (osc ? 6 : cc.n_arm);
+      cc.gain[E * 16 + k] = on ? (osc ? cc.kp[k] : cc.jv_kp[k]) : 0.0;
+      cc.gain[E * 16 + 8 + k] = on ? (osc ? cc.kd[k] : cc.jv_kd[k]) : 0.0;
+    }
 }

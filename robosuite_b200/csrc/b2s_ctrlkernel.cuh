@@ -45,6 +45,10 @@ DEV void ctrl_osc_block(int sub, const R* action, int env0, int nenv, int gid, i
   for (int k = 0; k < 4; k++) grip[k] = s.grip_state[E * 4 + k];
   if (sub == 0 && action != nullptr) {  // policy step: set_goal (osc.py:225-283) + gripper format_action
     const R* act = action + E * cc.action_dim;
+    if (cc.gain) {  // variable impedance: the gains first, then the delta that follows them
+      for (int k = 0; k < 6; k++) imp_gain(cc.imp, act, k, cc.gain + E * 16 + k, cc.gain + E * 16 + 8 + k);
+      act += cc.imp->off;
+    }
     const int od = cc.kind == 5 ? 3 : 6;  // OSC_POSITION: no orientation delta, goal_ori re-anchored to the current orientation
     R sd[6] = {0, 0, 0, 0, 0, 0};
     for (int k = 0; k < od; k++) {
@@ -93,7 +97,8 @@ DEV void ctrl_osc_block(int sub, const R* action, int env0, int nenv, int gid, i
   osc_jac_col(cve, rp, vel);   // site velocity [linear; angular] from the owning body's spatial velocity
   osc_jac_col(cvb, op, bvel);
   double F[6], pt[OSC_NA_MAX], bias[OSC_NA_MAX], tau[OSC_NA_MAX];
-  osc_wrench(rp, ro, op, oo, goal_pos, goal_ori, vel, bvel, cc.kp, cc.kd, F);
+  if (cc.gain) osc_wrench(rp, ro, op, oo, goal_pos, goal_ori, vel, bvel, cc.gain + E * 16, cc.gain + E * 16 + 8, F);
+  else osc_wrench(rp, ro, op, oo, goal_pos, goal_ori, vel, bvel, cc.kp, cc.kd, F);
   const double kv = 2.0 * sqrt(cc.null_kp);
 #pragma unroll
   for (int a = 0; a < OSC_NA_MAX; a++) {

@@ -208,6 +208,24 @@ struct ObsModDev {
 };
 enum { OBS_CORRUPT_NONE = 0, OBS_CORRUPT_GAUSSIAN = 1, OBS_CORRUPT_UNIFORM = 2 };  // = B2S_CORRUPT_* (include/b2s.h)
 
+// Variable impedance (b2s_ctrl_config's impedance_mode), kept in device memory (the constant bank is nearly full): the mode
+// (B2S_IMPEDANCE_* of include/b2s.h), the gain count d, the action offset of the delta (d or 2 d) and the clip limits.  The gains
+// themselves are the per-environment row CtrlCfgDev::gain.
+struct ImpDev {
+  int mode, d, off;
+  double kp_min[8], kp_max[8], dr_min[8], dr_max[8];
+};
+enum { IMP_FIXED = 0, IMP_VARIABLE = 1, IMP_VARIABLE_KP = 2 };  // = B2S_IMPEDANCE_* (include/b2s.h)
+
+// kp, kd = 2 sqrt(kp) dr of gain k from the gain part of one environment's action (set_goal of osc.py / joint_pos.py): the same
+// operation order as the host's fixed gains, so the configured gains in the action give the fixed mode's bits
+template <typename R> __device__ __forceinline__ void imp_gain(const ImpDev* im, const R* act, int k, double* kp, double* kd) {
+  const bool var = im->mode == IMP_VARIABLE;
+  const double p = fmin(fmax((double)act[(var ? im->d : 0) + k], im->kp_min[k]), im->kp_max[k]);
+  *kp = p;
+  *kd = var ? 2.0 * sqrt(p) * fmin(fmax((double)act[k], im->dr_min[k]), im->dr_max[k]) : 2.0 * sqrt(p);
+}
+
 struct CtrlCfgDev {
   int kind, action_dim, n_arm, eef_site, base_site, n_grip, uncouple;
   int obs_dim; const int* obs_op; const int* obs_a; const int* obs_b;  // device arrays
@@ -222,6 +240,9 @@ struct CtrlCfgDev {
   int jv_use_vel_limits, jv_torque_comp;
   int arm_dof[8], arm_qpos[8], arm_act[8], grip_act[4];
   double grip_sign[4], grip_speed, kp[6], kd[6], input_max[6], input_min[6], output_max[6], output_min[6], null_kp;
+  // variable impedance: the table and the gain rows [n_env, 16] (kp[8], kd[8]); both null in fixed mode, where every controller
+  // reads kp / kd / jv_kp / jv_kd above
+  const ImpDev* imp; double* gain;
 };
 
 // ---- constant-memory descriptors, one slot per live handle (b2s_create takes a free slot, b2s_destroy returns it).  Device code

@@ -33,7 +33,14 @@ class CtrlCfg(C.Structure):
         ("jv_kp", C.c_double * 8), ("jv_ki", C.c_double * 8), ("jv_kd", C.c_double * 8), ("jv_in_max", C.c_double * 8),
         ("jv_in_min", C.c_double * 8), ("jv_out_max", C.c_double * 8), ("jv_out_min", C.c_double * 8),
         ("jv_vel_lo", C.c_double), ("jv_vel_hi", C.c_double), ("jv_use_vel_limits", C.c_int), ("jv_torque_comp", C.c_int),
+        # b2s_ctrl_cfg ends here.  Then b2s_impedance_cfg (include/b2s.h), which ctrl_config passes to b2s_ctrl_impedance:
+        # IMPEDANCE_* and the clip limits of the gains taken from the action
+        ("impedance_mode", C.c_int), ("kp_min", C.c_double * 8), ("kp_max", C.c_double * 8),
+        ("damping_ratio_min", C.c_double * 8), ("damping_ratio_max", C.c_double * 8),
     ]
+
+
+IMPEDANCE_FIXED, IMPEDANCE_VARIABLE, IMPEDANCE_VARIABLE_KP = 0, 1, 2
 
 
 # per-environment model fields that are whole dof vectors (model_override(field) with no object id)
@@ -301,7 +308,10 @@ class BatchedSim:
         return jp, jr
 
     def ctrl_config(self, cfg: CtrlCfg):
+        """b2s_ctrl_config, then b2s_ctrl_impedance with the impedance block that trails the struct"""
         self._check(self._L.b2s_ctrl_config(self._h, C.byref(cfg)))
+        if cfg.impedance_mode:
+            self._check(self._L.b2s_ctrl_impedance(self._h, C.byref(cfg, CtrlCfg.impedance_mode.offset)))
 
     def reset_envs(self, mask=None, qpos=None):
         """masked episode reset entirely on the device (b2s_reset_envs): mask uint8 [n_env] or None, qpos [n_env, nq] or None (qpos0)"""

@@ -294,15 +294,25 @@ class BatchedMujocoEnv(ContactQueries):
 
     @property
     def action_spec(self):
-        """(low, high) bounds (robot_env.py:271-285): OSC input limits + gripper [-1, 1]"""
+        """(low, high) bounds (robot_env.py:271-285): the arm controller's control_limits, then the gripper's [-1, 1].  The arm's
+        are its input limits (od entries: 6 for OSC_POSE, 3 for OSC_POSITION, n_arm for the joint-space kinds), preceded in the
+        variable impedance modes by the gain limits: [damping_ratio_min, kp_min, input_min] in "variable", [kp_min, input_min] in
+        "variable_kp" (d entries each: 6 for OSC, n_arm for JOINT_POSITION)"""
         c = self._ctrl_cfg
         if c.kind in (2, 3, 4):  # joint-space controllers: per-joint input limits
-            n = c.n_arm
-            return (np.array(list(c.jv_in_min)[:n] + [-1.0] * (c.action_dim - n)),
-                    np.array(list(c.jv_in_max)[:n] + [1.0] * (c.action_dim - n)))
-        low = np.array(list(c.input_min)[:6] + [-1.0] * (c.action_dim - 6))
-        high = np.array(list(c.input_max)[:6] + [1.0] * (c.action_dim - 6))
-        return low, high
+            od = d = c.n_arm
+            low, high = list(c.jv_in_min)[:od], list(c.jv_in_max)[:od]
+        else:
+            od, d = (3 if c.kind == 5 else 6), 6
+            low, high = list(c.input_min)[:od], list(c.input_max)[:od]
+        mode = getattr(c, "impedance_mode", 0)
+        if mode == 2:
+            low, high = list(c.kp_min)[:d] + low, list(c.kp_max)[:d] + high
+        elif mode == 1:
+            low = list(c.damping_ratio_min)[:d] + list(c.kp_min)[:d] + low
+            high = list(c.damping_ratio_max)[:d] + list(c.kp_max)[:d] + high
+        n = c.action_dim - len(low)
+        return np.array(low + [-1.0] * n), np.array(high + [1.0] * n)
 
     def _fingerpad_geoms(self):
         """left / right fingerpad geom id lists (models/grippers/*_gripper.py `_important_geoms`)"""
