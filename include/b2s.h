@@ -144,6 +144,49 @@ int b2s_reset_envs(b2s_sim* sim, const uint8_t* env_mask, const void* qpos_new);
  * pose: override them too (pose = parent pose * local pose).  At most 4 bodies per handle. */
 int b2s_body_pose_override(b2s_sim* sim, int body_id);
 
+/* Object placement (the reference's UniformRandomSampler / SequentialCompositeSampler.sample, utils/placement_samplers.py, recalled
+ * from robosuite v1.5; no reference checkout was available to check it against).  b2s_place_config copies a program of n <= 32
+ * entries, one per object in placement order (n = 0 clears it).  It is handle configuration: not a snapshot section, not part of the
+ * signature.  b2s_place_objects then places every entry for the masked environments (env_mask: n_env device bytes, NULL = all) in
+ * ONE launch on the handle's stream, one warp per environment, without host data.  Entry o of environment e:
+ *   base    = base[]                                            when ref = -1
+ *           = (x_r, y_r, z_r + ref_dz) of entry ref (< o)      otherwise (ref_dz: the referenced object's top offset when on_top, else 0)
+ *   z       = (z_offset + base_z) - bottom_dz                  (bottom_dz: the object's bottom offset when on_top, else 0)
+ *   try t   = 0 .. 4999:  x = (x_min + (x_max - x_min) u_x) + base_x,  y likewise with u_y  (the caller has already shrunk the ranges
+ *             by the radius for ensure_object_boundary_in_range; an inverted range works as numpy's uniform does)
+ *   valid   = not ensure_valid, or for every earlier entry j:
+ *             not ( sqrt(dx*dx + dy*dy) <= radius_j + radius  and  z - z_j <= top_j - bottom )
+ * The first valid try is taken (lanes evaluate 32 tries per round; the ballot's lowest valid lane is the sequential loop's first
+ * success).  Its rotation: pair c = min(floor(u_c * n_rot), n_rot - 1) (0 when n_rot = 1), angle = rot_min[c] + (rot_max[c] -
+ * rot_min[c]) u_a, quaternion (cos a/2, sin a/2 * unit axis) w-first about axis 0 / 1 / 2 = x / y / z.  A fixed angle is the pair
+ * (a, a); U[0, 2 pi) is (0, 2 pi).
+ * Draws: Philox4x32-10 with key = seed, u = 53 bits of two output words formed as in b2s_perturb_model.  Counter (e, counter, o, t):
+ * u_x from words (0, 1), u_y from words (2, 3).  Counter (e, counter, o, 0xFFFFFFFF): u_c from words (0, 1), u_a from words (2, 3).
+ * Arithmetic in fp64, every operation rounded once (no contraction), in the order written above; sin / cos of a/2 by the library's
+ * own fixed sequence (csrc/b2s_place.cuh place_sincos: reduction by pi/2 with fdlibm's split and fdlibm's kernel polynomials), so a
+ * host restatement reproduces every bit.  An environment's placement depends only on (seed, counter, e, program).
+ * Targets: qpos_adr >= 0 writes qpos[e, qpos_adr .. +7] = (x, y, z, quaternion) of the float64 [n_env, nq] device array `qpos` (the
+ * sampled states b2s_reset_envs then takes, converted to the handle's precision by the caller); body >= 0 writes the body's pose
+ * override (b2s_body_pose_override) and the override of every overridden body welded to it (at the time of b2s_place_config), as
+ * placed pose * pose relative to the body (composed local poses), rounded to the handle's precision last.  Unmasked environments
+ * are not written.
+ * An environment in which some object has no valid try keeps that object's last try and gets warn bit 1024.  b2s_place_objects leaves
+ * the bit pending; the next b2s_reset_envs writes it into `warn` for the environments it resets (it clears every other bit).
+ * B2S_ERR_ARG: n outside [0, 32]; in an entry a non-finite field, n_rot outside [1, 8], axis outside [0, 2], ref not -1 or an earlier
+ * entry, neither or both of qpos_adr / body, a qpos_adr that is not the first address of a free joint, a body without a pose
+ * override, a joint or body placed twice; in b2s_place_objects a counter >= 2^32 or qpos NULL while an entry writes qpos.  Without a
+ * program b2s_place_objects does nothing. */
+#define B2S_PLACE_MAXROT 8
+typedef struct {
+  int qpos_adr, body, ref, ensure_valid, axis, n_rot;
+  double x_min, x_max, y_min, y_max;
+  double base[3], ref_dz, z_offset, bottom_dz;
+  double radius, bottom, top; /* horizontal_radius, bottom_offset z, top_offset z */
+  double rot_min[B2S_PLACE_MAXROT], rot_max[B2S_PLACE_MAXROT];
+} b2s_place;
+int b2s_place_config(b2s_sim* sim, const b2s_place* entries_host, int n);
+int b2s_place_objects(b2s_sim* sim, double* qpos, const uint8_t* env_mask, uint64_t seed, uint64_t counter);
+
 /* Per-environment model values (domain randomisation; the reference draws e.g. Lift's cube size per model build,
  * environments/manipulation/lift.py:311-314).  Declares a per-environment copy of `field` for object `id`: afterwards the array
  * "<field>:<id>" (fetch it with b2s_array) holds one value per environment, initialised to the model's, and every step reads it.

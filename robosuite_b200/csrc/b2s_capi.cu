@@ -3,6 +3,7 @@
 #include "../../include/b2s.h"
 #include "b2s_unit.cuh"
 #include "b2s_snapshot.cuh"
+#include "b2s_place.cuh"
 
 #include <cmath>
 #include <cstdio>
@@ -148,6 +149,14 @@ struct b2s_sim {
   int imp_mode = 0;
   double timestep_h = 0;
   std::vector<char> body_free_h;  // body b has a free joint (b2s_obs_objects takes only such bodies)
+  // b2s_place_config: the program on the device (replaced tables stay allocated), its length, whether an entry writes qpos, and the
+  // per-environment warn bits of the last b2s_place_objects that the next b2s_reset_envs carries into `warn`
+  PlaceDev* place_dev = nullptr;
+  int place_n = 0, place_qpos = 0;
+  int* place_pending = nullptr;
+  std::vector<char> free_qadr_h;                   // qpos address a is the first of a free joint
+  std::vector<int> body_parent_h;
+  std::vector<double> body_pos_h, body_quat_h;     // local poses (model constants)
 };
 
 // Every entry point picks the handle's precision once: f(DModel<R>&, DState<R>&) runs with R = float or double, and
@@ -736,8 +745,16 @@ int b2s_create(const void* blob_host, size_t nbytes, int n_env, int device, int 
     {
       int64_t nj = 0;
       const int* jt = b.i32("jnt_type", &nj); const int* jb = b.i32("jnt_bodyid");
+      const int* jq = b.i32("jnt_qposadr");
       s->body_free_h.assign(s->nbody, 0);
+      s->free_qadr_h.assign(s->nq, 0);
       for (int64_t j = 0; j < nj; j++) if (jt[j] == JNT_FREE && jb[j] >= 0 && jb[j] < s->nbody) s->body_free_h[jb[j]] = 1;
+      for (int64_t j = 0; j < nj; j++) if (jt[j] == JNT_FREE && jq[j] >= 0 && jq[j] + 7 <= s->nq) s->free_qadr_h[jq[j]] = 1;
+      const int* bp = b.i32("body_parentid");
+      s->body_parent_h.assign(bp, bp + s->nbody);
+      const double* bpos = b.f64("body_pos"); const double* bquat = b.f64("body_quat");
+      s->body_pos_h.assign(bpos, bpos + 3 * s->nbody);
+      s->body_quat_h.assign(bquat, bquat + 4 * s->nbody);
     }
     for (const char* ty : {"body", "joint", "geom", "site", "actuator", "mesh", "camera", "light"}) {
       std::string key = std::string("names_") + ty;
@@ -1350,7 +1367,7 @@ int b2s_reset_envs(b2s_sim* s, const uint8_t* mask, const void* qpos_new) {
   int threads = 128, blocks = (s->n_env + threads - 1) / threads;
   with_real(s, [&](auto& m, auto&) {
     using R = real_of<decltype(m)>;
-    reset_envs_kernel<R><<<blocks, threads, 0, s->stream>>>(mask, (const R*)qpos_new, s->slot);
+    reset_envs_kernel<R><<<blocks, threads, 0, s->stream>>>(mask, (const R*)qpos_new, s->slot, s->place_n ? s->place_pending : nullptr);
   });
   s->launches++;
   CUDA_TRY(cudaGetLastError());
@@ -1585,6 +1602,100 @@ int b2s_body_pose_override(b2s_sim* s, int body_id) {
   if (s->body_weldid_h[body_id] != 0) return fail(B2S_ERR_UNSUPPORTED, "b2s_body_pose_override: the body is not welded to the world (move it through qpos)");
   CUDA_TRY(cudaSetDevice(s->device));
   return with_real(s, [&](auto&, auto& st) { return body_pose_override_t(s, st, body_id); });
+}
+
+int b2s_place_config(b2s_sim* s, const b2s_place* entries, int n) {
+  if (!s || n < 0 || n > B2S_PLACE_MAX || (n > 0 && !entries)) return fail(B2S_ERR_ARG, "b2s_place_config: bad argument");
+  std::vector<PlaceDev> prog(n);
+  std::vector<int> seen_q, seen_b;
+  int has_q = 0;
+  for (int i = 0; i < n; i++) {
+    const b2s_place& e = entries[i];
+    const std::string at = "b2s_place_config: entry " + std::to_string(i) + ": ";
+    PlaceDev& d = prog[i];
+    const double f[] = {e.x_min, e.x_max, e.y_min, e.y_max, e.base[0], e.base[1], e.base[2], e.ref_dz, e.z_offset, e.bottom_dz,
+                        e.radius, e.bottom, e.top};
+    for (double v : f) if (!std::isfinite(v)) return fail(B2S_ERR_ARG, at + "non-finite field");
+    if (e.n_rot < 1 || e.n_rot > B2S_PLACE_MAXROT) return fail(B2S_ERR_ARG, at + "n_rot must be in [1, 8]");
+    for (int k = 0; k < e.n_rot; k++)
+      if (!std::isfinite(e.rot_min[k]) || !std::isfinite(e.rot_max[k])) return fail(B2S_ERR_ARG, at + "non-finite rotation range");
+    if (e.axis < 0 || e.axis > 2) return fail(B2S_ERR_ARG, at + "axis must be 0, 1 or 2");
+    if (e.ref < -1 || e.ref >= i) return fail(B2S_ERR_ARG, at + "ref must be -1 or an earlier entry");
+    if ((e.qpos_adr >= 0) == (e.body >= 0)) return fail(B2S_ERR_ARG, at + "exactly one of qpos_adr and body must be given");
+    d.x_min = e.x_min; d.x_max = e.x_max; d.y_min = e.y_min; d.y_max = e.y_max;
+    for (int k = 0; k < 3; k++) d.base[k] = e.base[k];
+    d.ref_dz = e.ref_dz; d.z_offset = e.z_offset; d.bottom_dz = e.bottom_dz; d.radius = e.radius; d.bottom = e.bottom; d.top = e.top;
+    for (int k = 0; k < 8; k++) { d.rot_min[k] = k < e.n_rot ? e.rot_min[k] : 0; d.rot_max[k] = k < e.n_rot ? e.rot_max[k] : 0; }
+    d.qpos_adr = e.qpos_adr; d.ref = e.ref; d.ensure_valid = e.ensure_valid != 0; d.axis = e.axis; d.n_rot = e.n_rot; d.nov = 0;
+    if (e.qpos_adr >= 0) {
+      if (e.qpos_adr >= s->nq || !s->free_qadr_h[e.qpos_adr]) return fail(B2S_ERR_ARG, at + "qpos_adr is not the first qpos address of a free joint");
+      if (std::count(seen_q.begin(), seen_q.end(), e.qpos_adr)) return fail(B2S_ERR_ARG, at + "the free joint is placed twice");
+      seen_q.push_back(e.qpos_adr);
+      has_q = 1;
+      continue;
+    }
+    if (e.body >= s->nbody) return fail(B2S_ERR_ARG, at + "body id out of range");
+    if (std::count(seen_b.begin(), seen_b.end(), e.body)) return fail(B2S_ERR_ARG, at + "the body is placed twice");
+    seen_b.push_back(e.body);
+    // override 0: the body itself; then every overridden body welded to it, with its pose relative to the body (composed local poses)
+    const int rc = with_real(s, [&](auto&, auto& st) -> int {
+      int own = -1;
+      for (int k = 0; k < st.n_ov; k++) if (st.ov_body[k] == e.body) own = k;
+      if (own < 0) return fail(B2S_ERR_ARG, at + "the body has no pose override (b2s_body_pose_override)");
+      auto add = [&](int k, const double* lp, const double* lq) {
+        d.ov_pos[d.nov] = st.ov_pos[k]; d.ov_quat[d.nov] = st.ov_quat[k];
+        for (int r = 0; r < 3; r++) d.ov_lp[d.nov][r] = lp[r];
+        for (int r = 0; r < 4; r++) d.ov_lq[d.nov][r] = lq[r];
+        d.nov++;
+      };
+      const double zp[3] = {0, 0, 0}, iq[4] = {1, 0, 0, 0};
+      add(own, zp, iq);
+      for (int k = 0; k < st.n_ov; k++) {
+        int c = st.ov_body[k], up = c;
+        std::vector<int> chain;
+        while (up > 0 && up != e.body) { chain.push_back(up); up = s->body_parent_h[up]; }
+        if (c == e.body || up != e.body) continue;
+        double lp[3] = {0, 0, 0}, lq[4] = {1, 0, 0, 0};
+        for (auto it = chain.rbegin(); it != chain.rend(); ++it) {  // (lp, lq) <- (lp, lq) * local pose of *it
+          double M[9], q2[4];
+          h_quat2mat(M, lq);
+          const double* bp = &s->body_pos_h[3 * *it];
+          for (int r = 0; r < 3; r++) lp[r] += M[3 * r] * bp[0] + M[3 * r + 1] * bp[1] + M[3 * r + 2] * bp[2];
+          h_qmul(q2, lq, &s->body_quat_h[4 * *it]);
+          for (int r = 0; r < 4; r++) lq[r] = q2[r];
+        }
+        add(k, lp, lq);
+      }
+      return B2S_OK;
+    });
+    if (rc != B2S_OK) return rc;
+  }
+  CUDA_TRY(cudaSetDevice(s->device));
+  try {
+    if (n && !s->place_pending) s->place_pending = dev_upload(s, std::vector<int>(s->n_env, 0));
+    s->place_dev = n ? dev_upload(s, prog) : nullptr;
+  } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
+  s->place_n = n;
+  s->place_qpos = has_q;
+  return B2S_OK;
+}
+
+int b2s_place_objects(b2s_sim* s, double* qpos, const uint8_t* env_mask, uint64_t seed, uint64_t counter) {
+  if (!s) return fail(B2S_ERR_ARG, "null handle");
+  if (counter >> 32) return fail(B2S_ERR_ARG, "b2s_place_objects: the counter must be below 2^32");
+  if (s->place_n == 0) return B2S_OK;
+  if (s->place_qpos && !qpos) return fail(B2S_ERR_ARG, "b2s_place_objects: the program places free joints: qpos is required");
+  CUDA_TRY(cudaSetDevice(s->device));
+  const int wpb = 4;
+  const unsigned blocks = (unsigned)((s->n_env + wpb - 1) / wpb);
+  with_real(s, [&](auto& m, auto&) {
+    using R = real_of<decltype(m)>;
+    place_kernel<R><<<blocks, wpb * 32, 0, s->stream>>>(s->place_dev, s->place_n, qpos, s->nq, env_mask, s->n_env, seed, (unsigned)counter,
+                                                        s->place_pending);
+  });
+  s->launches++;
+  CUDA_TRY(cudaGetLastError());
+  return B2S_OK;
 }
 
 int b2s_env_step(b2s_sim* s, const void* action, int nsub) {

@@ -228,9 +228,10 @@ __global__ void __launch_bounds__(512, 1) step_kernel(int phases, int nsub, cons
 }
 
 // masked episode reset without a host round trip: selected environments take their generalized positions from `qpos_new` (a pool of
-// sampled initial states, [n_env, nq]; nullptr: the model's qpos0), everything else is cleared the way reset_kernel does
+// sampled initial states, [n_env, nq]; nullptr: the model's qpos0), everything else is cleared the way reset_kernel does.  `carry`
+// (nullptr without a placement program): warn bits b2s_place_objects left for this reset, which it takes and clears
 template <typename R>
-__global__ void reset_envs_kernel(const uint8_t* mask, const R* qpos_new, int slot) {
+__global__ void reset_envs_kernel(const uint8_t* mask, const R* qpos_new, int slot, int* carry) {
   const DModel<R>& m = cmodel<R>(slot);
   const DState<R>& s = cstate<R>(slot);
   int env = blockIdx.x * blockDim.x + threadIdx.x;
@@ -241,7 +242,8 @@ __global__ void reset_envs_kernel(const uint8_t* mask, const R* qpos_new, int sl
   for (int i = 0; i < m.nv; i++) { s.qvel[E * m.nv + i] = 0; s.qacc[E * m.nv + i] = 0; s.qacc_ws[E * m.nv + i] = 0; }
   for (int i = 0; i < m.nu; i++) s.ctrl[E * m.nu + i] = 0;
   s.time[env] = 0;
-  s.warn[env] = 0;
+  s.warn[env] = carry ? carry[env] : 0;
+  if (carry) carry[env] = 0;
   if (s.obs_fresh) s.obs_fresh[env] = 1;
 }
 

@@ -52,6 +52,17 @@ PERTURB_SCALE, PERTURB_SHIFT = 0, 1
 
 CORRUPT_NONE, CORRUPT_GAUSSIAN, CORRUPT_UNIFORM = 0, 1, 2
 
+PLACE_MAXROT = 8
+
+
+class PlaceSpec(C.Structure):
+    """b2s_place: one object of b2s_place_config's program (include/b2s.h)"""
+    _fields_ = [("qpos_adr", C.c_int), ("body", C.c_int), ("ref", C.c_int), ("ensure_valid", C.c_int), ("axis", C.c_int),
+                ("n_rot", C.c_int), ("x_min", C.c_double), ("x_max", C.c_double), ("y_min", C.c_double), ("y_max", C.c_double),
+                ("base", C.c_double * 3), ("ref_dz", C.c_double), ("z_offset", C.c_double), ("bottom_dz", C.c_double),
+                ("radius", C.c_double), ("bottom", C.c_double), ("top", C.c_double), ("rot_min", C.c_double * PLACE_MAXROT),
+                ("rot_max", C.c_double * PLACE_MAXROT)]
+
 
 class ObsMod(C.Structure):
     """b2s_obs_mod: period (s) and corruptor of one observable (b2s_obs_modifiers)"""
@@ -113,6 +124,8 @@ def lib():
         L.b2s_set_const.argtypes = [C.c_void_p, C.c_void_p]
         L.b2s_perturb_config.argtypes = [C.c_void_p, C.POINTER(PerturbSpec), C.c_int]
         L.b2s_perturb_model.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64]
+        L.b2s_place_config.argtypes = [C.c_void_p, C.POINTER(PlaceSpec), C.c_int]
+        L.b2s_place_objects.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_uint64]
         L.b2s_obs_config.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]
         L.b2s_obs_modifiers.argtypes = [C.c_void_p, C.c_int, C.c_void_p, C.POINTER(ObsMod), C.c_uint64]
         L.b2s_obs_objects.argtypes = [C.c_void_p, C.c_int, C.c_void_p]
@@ -356,6 +369,34 @@ class BatchedSim:
         derived constants follow at the next set_const() or reset."""
         self._check(self._L.b2s_perturb_model(self._h, None if mask is None else C.c_void_p(mask.data_ptr()), int(seed) & (2 ** 64 - 1),
                                               int(counter)))
+
+    def place_config(self, entries):
+        """the placement program (b2s_place_config): a list of dicts with the fields of b2s_place (include/b2s.h), "rot" a list of
+        (min, max) pairs; an empty list clears it"""
+        arr = (PlaceSpec * max(len(entries), 1))()
+        for k, e in enumerate(entries):
+            rot = list(e["rot"])
+            if not 1 <= len(rot) <= PLACE_MAXROT:
+                raise ValueError("a placement entry takes 1 to %d rotation ranges, got %d" % (PLACE_MAXROT, len(rot)))
+            pad = [0.0] * (PLACE_MAXROT - len(rot))
+            arr[k] = PlaceSpec(int(e["qpos_adr"]), int(e["body"]), int(e["ref"]), int(bool(e["ensure_valid"])), int(e["axis"]), len(rot),
+                               *(float(e[f]) for f in ("x_min", "x_max", "y_min", "y_max")), (C.c_double * 3)(*map(float, e["base"])),
+                               *(float(e[f]) for f in ("ref_dz", "z_offset", "bottom_dz", "radius", "bottom", "top")),
+                               (C.c_double * PLACE_MAXROT)(*[float(a) for a, _ in rot], *pad),
+                               (C.c_double * PLACE_MAXROT)(*[float(b) for _, b in rot], *pad))
+        self._check(self._L.b2s_place_config(self._h, arr, len(entries)))
+
+    def place_objects(self, qpos, mask=None, seed=0, counter=0):
+        """place the configured objects of the masked environments (uint8 [n_env] device mask, None = all) in one launch
+        (b2s_place_objects): free joints into qpos (float64 [n_env, nq] on the device), world-welded bodies into their pose overrides.
+        Philox4x32-10 keyed by `seed`, counter (env, counter, entry, try); an environment without a valid try for some object gets
+        warn bit 1024 at the next reset_envs"""
+        if qpos is not None:
+            import torch
+
+            assert qpos.is_cuda and qpos.dtype == torch.float64 and qpos.is_contiguous() and qpos.shape == (self.n_env, self.model.nq)
+        self._check(self._L.b2s_place_objects(self._h, None if qpos is None else C.c_void_p(qpos.data_ptr()),
+                                              None if mask is None else C.c_void_p(mask.data_ptr()), int(seed) & (2 ** 64 - 1), int(counter)))
 
     def set_const(self, mask=None):
         """recompute the derived constants of the masked environments (uint8 [n_env] device mask, None = all) from their

@@ -102,7 +102,9 @@ SIM_WARN_BITS = {1: "singular mass matrix", 2: "non-finite state in the integrat
                       "triangle inequality, non-finite or negative damping, armature or friction loss, or a non-finite solref / "
                       "solimp component)",
                  256: "restore source row out of range (b2s_restore): the environment was left untouched",
-                 512: "object selection out of range (obj_sel, b2s_obs_objects): the selected-object observation rows were written as 0"}
+                 512: "object selection out of range (obj_sel, b2s_obs_objects): the selected-object observation rows were written as 0",
+                 1024: "no valid placement (placement_initializer, b2s_place_objects): an object kept its last of 5000 tries, where the "
+                       "reference raises RandomizationError"}
 
 
 class BatchedMujocoEnv(ContactQueries):
@@ -112,7 +114,10 @@ class BatchedMujocoEnv(ContactQueries):
     does the same for the step-1 arrays (BatchedSim.set_step1_export), so that sim.data (robosuite_b200/data.py) reads the poses,
     Jacobians and mass matrices of the last substep.  dynamics_queries=True switches on the step-2 export
     (BatchedSim.set_step2_export) and the contact export, so that sim.data reads the actuator, smooth and constraint forces, the
-    constraint rows and the per-contact forces (sim.data.contact_force()) of the last substep."""
+    constraint rows and the per-contact forces (sim.data.contact_force()) of the last substep.
+    placement_initializer: a robosuite_b200.placement_samplers UniformRandomSampler or SequentialCompositeSampler naming the task's
+    objects; every reset then places them by the reference's rules on the device (see _setup_placement).  None: the task's default
+    placement."""
 
     maxcon = None  # per-environment contact / constraint-row capacity (None: engine defaults 32 / 64); overflow sets warn bit 4
     maxefc = None
@@ -128,7 +133,7 @@ class BatchedMujocoEnv(ContactQueries):
                  initialization_noise="default", precision="f32", xml=None, has_renderer=False,
                  has_offscreen_renderer=False, use_camera_obs=False, hard_reset=False, lite_physics=True, model=None,
                  kernel_mode="pipeline", sim_cls=None, contact_queries=False, data_queries=False,
-                 dynamics_queries=False, **kwargs):
+                 dynamics_queries=False, placement_initializer=None, **kwargs):
         import torch
 
         if has_renderer or has_offscreen_renderer or use_camera_obs:
@@ -185,6 +190,9 @@ class BatchedMujocoEnv(ContactQueries):
         self.seed = seed
         if seed is not None:
             self.rng.manual_seed(int(seed))
+        self.placement_initializer = placement_initializer
+        if placement_initializer is not None:
+            self._setup_placement()
         self.timestep = torch.zeros(self.num_envs, dtype=torch.long, device=self.device)
         self.done = torch.zeros(self.num_envs, dtype=torch.bool, device=self.device)
         self.cur_time = 0.0
@@ -276,6 +284,44 @@ class BatchedMujocoEnv(ContactQueries):
     def _sample_reset_state(self, n):
         raise NotImplementedError
 
+    def _placement_objects(self):
+        """the task's objects for a placement_initializer: name -> dict(radius, bottom, top, qpos_adr, body) (lower() in
+        placement_samplers.py), in the order the reference's _load_model adds them; None: the task takes no sampler"""
+        return None
+
+    def _setup_placement(self):
+        """what the reference's _load_model does with a given sampler: reset() and add_objects(the task's objects) for a single
+        sampler; a SequentialCompositeSampler keeps the objects its samplers name (its reset() would drop them).  The program is
+        lowered once and configured on the handle; the Philox key comes from make(seed=...) under a tag of its own."""
+        from ..placement_samplers import SequentialCompositeSampler, lower
+
+        objects = self._placement_objects()
+        if objects is None:
+            raise NotImplementedError("{} does not take a placement_initializer".format(type(self).__name__))
+        sampler = self.placement_initializer
+        if not isinstance(sampler, SequentialCompositeSampler):
+            sampler.reset()
+            sampler.add_objects(list(objects))
+        self._placement_names, entries = lower(sampler, objects)
+        self.sim.place_config(entries)
+        self._place_seed = self._tagged_seed(0x504C4143)  # "PLAC"
+        self._place_counter = 0
+
+    def _place_objects(self, q):
+        """the sampler's placements of the environments being reset (the mask reset() was given) in one launch: free joints into q
+        (float64 [N, nq], before any parking), world-welded bodies into their pose overrides.  The counter advances on the host."""
+        import torch
+
+        mask = self._reset_mask_arg
+        self._place_mask8 = None if mask is None else mask.to(device=self.device, dtype=torch.uint8).contiguous()  # kept alive
+        self.sim.place_objects(q, self._place_mask8, self._place_seed, self._place_counter)
+        self._place_counter = (self._place_counter + 1) & 0xFFFFFFFF
+
+    def _tagged_seed(self, tag):
+        """a 64-bit key derived from make(seed=...) (a seed drawn once when seed is None) and a tag of the stream's own"""
+        base = int(self.seed) if self.seed is not None else int(np.random.SeedSequence().generate_state(1, np.uint64)[0])
+        return int(np.random.SeedSequence([base & (2 ** 64 - 1), tag]).generate_state(1, np.uint64)[0])
+
     def _randomize_model(self, mask):
         """per-reset draws that live outside qpos, applied to the masked environments before the engine's reset: placements the
         reference writes into MODEL constants (Door: door.py:417-427) and the drawn object of single_object_mode 1 (PickPlace,
@@ -333,6 +379,7 @@ class BatchedMujocoEnv(ContactQueries):
 
         # the two hooks run in this order, both over all num_envs rows: _randomize_model applies to the masked environments what
         # _sample_reset_state drew besides qpos (single_object_mode 1 hands its object draw over in `_sel_draw`, envs/single_object.py)
+        self._reset_mask_arg = mask  # the environments a placement_initializer places (_place_objects)
         q = self._sample_reset_state(self.num_envs).to(self.dtype).contiguous()
         self._randomize_model(None if mask is None else mask.to(device=self.device).bool())
         if mask is None:
@@ -495,9 +542,8 @@ class BatchedMujocoEnv(ContactQueries):
         spec = [(1.0 / m["sampling_rate"],) + (m["corruptor"].spec() if m["corruptor"] is not None else (CORRUPT_NONE, 0.0, 0.0, -np.inf, np.inf))
                 for m in mods]
         if "_obs_noise_seed" not in self.__dict__:
-            base = int(self.seed) if self.seed is not None else int(np.random.SeedSequence().generate_state(1, np.uint64)[0])
             # "OBSN": the observation-noise stream of this seed (Philox keys of the dynamics perturbation take the seed itself)
-            self._obs_noise_seed = int(np.random.SeedSequence([base & (2 ** 64 - 1), 0x4F42534E]).generate_state(1, np.uint64)[0])
+            self._obs_noise_seed = self._tagged_seed(0x4F42534E)
         self.sim.obs_modifiers(row_obs, spec, self._obs_noise_seed)
 
     def check_sim_warnings(self):

@@ -18,9 +18,15 @@ class BatchedDoor(BatchedMujocoEnv):
     maxcon, maxefc = 48, 160
     tier_small = (8, 32)  # small tail tier: see BatchedMujocoEnv.tier_small
 
+    # door.xml's bottom_site z (door.py:32 below), and its top_site z and horizontal_radius_site x, recalled from robosuite v1.5 (no
+    # reference checkout was at hand); only a placement_initializer reads them
+    DOOR_META = dict(radius=0.3, bottom=-0.3, top=0.3)
+
     def __init__(self, *args, door_placement=None, **kwargs):
         # (x, y, yaw) relative to table_offset; sampler ranges x [0.07, 0.09], y [-0.01, 0.01], yaw [-pi/2 - 0.25, -pi/2]
-        self._fixed_door = door_placement is not None or kwargs.get("model") is not None
+        if door_placement is not None and kwargs.get("placement_initializer") is not None:
+            raise ValueError("door_placement pins the door; a placement_initializer samples it: give one of them")
+        self._fixed_door = kwargs.get("placement_initializer") is None and (door_placement is not None or kwargs.get("model") is not None)
         self.door_placement = door_placement if door_placement is not None else (0.08, 0.0, -math.pi / 2 - 0.125)
         self._door_ov = None
         super().__init__(*args, **kwargs)
@@ -75,12 +81,17 @@ class BatchedDoor(BatchedMujocoEnv):
         """(pos [N, 3], quat [N, 4] wxyz) of the door's root body per environment, or None with a pinned placement"""
         return None if self._door_ov is None else self._door_ov[0]
 
+    def _placement_objects(self):
+        """the door's root body, placed through its world-pose override (and Door_frame's, welded to it)"""
+        return {"Door": dict(self.DOOR_META, qpos_adr=-1, body=self.model.names["body"].index("Door_main"))}
+
     def _randomize_model(self, mask):
         """UniformRandomSampler of door.py:303-318: x in [0.07, 0.09], y in [-0.01, 0.01], yaw in [-pi/2 - 0.25, -pi/2] about z,
-        relative to table_offset; z = table height + 0.3 (the door's bottom offset)"""
+        relative to table_offset; z = table height + 0.3 (the door's bottom offset).  A placement_initializer's placement was
+        written by _sample_reset_state instead."""
         import torch
 
-        if self._door_ov is None:
+        if self._door_ov is None or self.placement_initializer is not None:
             return
         n, dev = self.num_envs, self.device
         u = torch.rand((n, 3), generator=self.rng, device=dev, dtype=torch.float64)
@@ -106,7 +117,10 @@ class BatchedDoor(BatchedMujocoEnv):
                 dst.copy_(torch.where(mask.to(dst.device)[:, None], src, dst))
 
     def _sample_reset_state(self, n):
-        return self._robot_reset_qpos(n)  # door closed, latch at rest (qpos0)
+        q = self._robot_reset_qpos(n)  # door closed, latch at rest (qpos0)
+        if self.placement_initializer is not None:
+            self._place_objects(q)  # the door's pose overrides
+        return q
 
     def _check_success(self):
         """hinge opened beyond 0.3 rad (door.py:429-437); qpos after the step, as the reference reads it"""

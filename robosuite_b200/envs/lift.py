@@ -28,6 +28,8 @@ class BatchedLift(BatchedMujocoEnv):
         """per_env_cube_size: every environment draws its own cube half sizes from U[0.020, 0.022]^3 (mass and moments from density
         1000), as the reference does per model build: at construction, and again at each of its resets when hard_reset=True.
         False: every environment keeps the cube of the model (the draw made when the fixture was compiled)."""
+        if per_env_cube_size and kwargs.get("placement_initializer") is not None:
+            raise NotImplementedError("per_env_cube_size with a placement_initializer: the cube's bottom offset would differ per environment")
         self.per_env_cube_size = per_env_cube_size
         self._cube_ov = None
         self._new_cube_size = None  # drawn by _sample_reset_state, written by _randomize_model
@@ -67,12 +69,20 @@ class BatchedLift(BatchedMujocoEnv):
             Ri, Rg = quat2mat(m.body_iquat[b]), quat2mat(m.geom_quat[g])
             self._cube_axis_map = (Ri.T @ Rg) ** 2
 
+    def _placement_objects(self):
+        """the cube as the reference's BoxObject: horizontal radius |half size[:2]|, bottom / top offsets -/+ half size z"""
+        h = self.model.geom_size[self.model.names["geom"].index("cube_g0")]
+        return {"cube": dict(radius=float(np.linalg.norm(h[:2])), bottom=-float(h[2]), top=float(h[2]), qpos_adr=self.cube_qadr, body=-1)}
+
     def _sample_reset_state(self, n):
         """robot: init_qpos + N(0, 0.02^2) (robots/robot.py:247-259); cube: x,y ~ U[-0.03,0.03], yaw ~ U[0,2pi),
-        z = table + 0.01 + half height (lift.py:311-336, placement_samplers.py:221-309)"""
+        z = table + 0.01 + half height (lift.py:311-336, placement_samplers.py:221-309), or the placement_initializer's rules"""
         import torch
 
         q = self._robot_reset_qpos(n)
+        if self.placement_initializer is not None:
+            self._place_objects(q)
+            return q
         u = torch.rand((n, 3), generator=self.rng, device=self.device, dtype=torch.float64)
         a = self.cube_qadr
         q[:, a] = self.table_offset[0] + (u[:, 0] * 2 - 1) * 0.03

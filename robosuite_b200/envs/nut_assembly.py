@@ -6,8 +6,10 @@ import numpy as np
 from .base import (OB_BODY_POS, OB_BODY_QUAT_XYZW, OB_SITE_POS, BatchedMujocoEnv, load_task_model, register_env)
 from .single_object import SingleObjectMixin, parse_mode, reject_fixed
 
-# models/assets/objects/{square,round}-nut.xml: bottom_site z, horizontal_radius_site (x, y)
-NUT_META = {"SquareNut": dict(bottom=-0.05, hradius=math.hypot(0.11, 0.06)), "RoundNut": dict(bottom=-0.05, hradius=math.hypot(0.11, 0.05))}
+# models/assets/objects/{square,round}-nut.xml: bottom_site z, top_site z, horizontal_radius_site (x, y).  top_site (0, 0, 0.05) is
+# recalled from robosuite v1.5 (no reference checkout was at hand); only a placement_initializer's overlap rule reads it
+NUT_META = {"SquareNut": dict(bottom=-0.05, top=0.05, hradius=math.hypot(0.11, 0.06)),
+            "RoundNut": dict(bottom=-0.05, top=0.05, hradius=math.hypot(0.11, 0.05))}
 
 
 class _BatchedNutAssembly(SingleObjectMixin, BatchedMujocoEnv):
@@ -71,6 +73,11 @@ class _BatchedNutAssembly(SingleObjectMixin, BatchedMujocoEnv):
         self.peg_xy = [np.asarray(self.model.body_pos[b][:2], dtype=np.float64) for b in (self.peg1_body_id, self.peg2_body_id)]
         self.table_z = float(self.model.body_pos[self.table_body_id][2])
 
+    def _placement_objects(self):
+        """both nuts (also in the single-object variants, which park the unused one afterwards), in nut_assembly.py's order"""
+        return {n: dict(radius=NUT_META[n]["hradius"], bottom=NUT_META[n]["bottom"], top=NUT_META[n]["top"], qpos_adr=self.obj_qadr[n],
+                        body=-1) for n in self.nut_names}
+
     def _sample_reset_state(self, n):
         """nuts: x ~ U[-0.115, -0.11], y ~ U[0.11, 0.225] (square) / U[-0.225, -0.11] (round), yaw ~ U[0, 2pi),
         z = table + 0.02 - bottom_offset (nut_assembly.py:405-431, placement_samplers.py:255-309)"""
@@ -78,6 +85,10 @@ class _BatchedNutAssembly(SingleObjectMixin, BatchedMujocoEnv):
 
         q = self._robot_reset_qpos(n)
         dev = self.device
+        if self.placement_initializer is not None:
+            self._place_objects(q)
+            self._park_objects(q)
+            return q
         for i, (name, yr) in enumerate(zip(self.nut_names, ((0.11, 0.225), (-0.225, -0.11)))):
             u = torch.rand((n, 3), generator=self.rng, device=dev, dtype=torch.float64)
             x = self.table_offset[0] + (-0.115 + u[:, 0] * 0.005)

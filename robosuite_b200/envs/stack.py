@@ -48,13 +48,23 @@ class BatchedStack(BatchedMujocoEnv):
         self.sim.task_config(self.cubeA_body_id, self.eef_site_id, left, right, self.cubeA_geoms)
         self.sim.task_config2(self.cubeB_body_id, self.cubeB_geoms)
 
+    def _placement_objects(self):
+        """both cubes as the reference's BoxObject (horizontal radius |half size[:2]|, bottom / top offsets -/+ half size z), in
+        stack.py's order"""
+        return {"cube" + k: dict(radius=float(np.linalg.norm(self.half[k][:2])), bottom=-float(self.half[k][2]), top=float(self.half[k][2]),
+                                 qpos_adr=getattr(self, "cube%s_qadr" % k), body=-1) for k in ("A", "B")}
+
     def _sample_reset_state(self, n):
         """robot init pose + noise; cubes: UniformRandomSampler x,y ~ U[-0.08,0.08], yaw ~ U[0,2pi), z = table + 0.01 +
-        half height, cube B re-drawn while it overlaps cube A (placement_samplers.py:255-309, stack.py:357-388)"""
+        half height, cube B re-drawn while it overlaps cube A (placement_samplers.py:255-309, stack.py:357-388), or the
+        placement_initializer's rules"""
         import torch
 
         dev = self.device
         q = self._robot_reset_qpos(n)
+        if self.placement_initializer is not None:
+            self._place_objects(q)
+            return q
 
         def draw(*shape):
             u = torch.rand(shape + (3,), generator=self.rng, device=dev, dtype=torch.float64)
