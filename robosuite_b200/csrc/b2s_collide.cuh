@@ -480,7 +480,7 @@ template <typename R> DEVN void support_w(const Shape<R>& s, R dx, R dy, R dz, R
     }
     case G_MESH: {
       R best = -Lim<R>::big();
-      int bi = 0x7fffffff;
+      int bi = 0;  // vertex 0 when no comparison succeeds (a NaN direction), never an index past the hull
       // generic loads: the work-list convex kernel stages the hull vertices of a pair that needs real GJK / EPA work in shared memory
       const R* vt = s.vert;
       for (int i = lane; i < s.nvert; i += 32) {
@@ -633,6 +633,15 @@ template <typename R> DEVN int closest_tet(R* sx, int& n, R* lam, int lane) {
   return 0;
 }
 
+// the pair's remembered separating direction into cv, or false when there is none: a zero entry, or one that is not a direction -
+// the cache travels in snapshot rows, which may come from a file, and an infinite component would make every support comparison
+// fail (0 * inf).  |c|^2 finite also keeps M^T c and the support products finite.
+template <typename R> DEV bool warm_direction(const R* cache, R* cv) {
+  cv[0] = cache[0]; cv[1] = cache[1]; cv[2] = cache[2];
+  const R c2 = v3dot(cv, cv);
+  return c2 > R(1e-12) && isfinite(c2);
+}
+
 // returns 1 if the cores overlap (simplex valid), else 0 with dist / witnesses.  sx: the warp's simplex area in shared memory (36 reals)
 template <typename R>
 DEVN int gjk(const Shape<R>& A, const Shape<R>& B, R* sx, int& ns, R& dist, R* wa, R* wb, R cutoff, int lane, R* cache = nullptr) {
@@ -642,8 +651,8 @@ DEVN int gjk(const Shape<R>& A, const Shape<R>& B, R* sx, int& ns, R& dist, R* w
   v3sub(v, A.pos, B.pos);
   if (v3dot(v, v) < R(1e-20)) v3set(v, R(1), R(0), R(0));
   if (cache) {  // separating direction found for this pair on the previous substep (temporal coherence)
-    R cv[3] = {cache[0], cache[1], cache[2]};
-    if (v3dot(cv, cv) > R(1e-12)) v3copy(v, cv);
+    R cv[3];
+    if (warm_direction(cache, cv)) v3copy(v, cv);
   }
   int n = 0;
   R lam[4] = {1, 0, 0, 0};
@@ -916,8 +925,8 @@ DEVN int convex_convex(const Shape<R>& A0, const Shape<R>& B0, R* out, int maxn,
     stage += 24; stage_cap -= 24;
     __syncwarp();
     if (cache != nullptr) {  // gjk()'s own first test, made here so that dismissed pairs (the common case) never pay for staging the hulls
-      R cv[3] = {cache[0], cache[1], cache[2]};
-      if (v3dot(cv, cv) > R(1e-12)) {
+      R cv[3];
+      if (warm_direction(cache, cv)) {
         R nv[3] = {-cv[0], -cv[1], -cv[2]};
         SV<R> w0;
         sv_support(A, B, nv, w0, lane);

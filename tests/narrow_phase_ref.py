@@ -1,4 +1,5 @@
-"""Scenes, poses and exact fp64 references for the narrow-phase tests (test_cpu_narrow_phase.py, test_gpu_narrow_phase.py).
+"""Scenes, poses and exact fp64 references for the narrow-phase tests (test_cpu_narrow_phase.py, test_gpu_narrow_phase.py, and the
+warm-start tests test_cpu_narrow_phase_warm.py and test_gpu_narrow_phase_warm.py).
 
 A scene is one geom pair: a plane plus one free body, or two free bodies with one geom each.  The references are functions of the
 geoms' world poses (as the kinematics place them) and sizes only, so they check the collision routines and nothing else:
@@ -42,54 +43,164 @@ def pair_name(pair):
     return "%s-%s" % pair
 
 
+def _fib(n):
+    i = np.arange(n) + 0.5
+    phi = np.arccos(1 - 2 * i / n)
+    th = np.pi * (1 + 5 ** 0.5) * i
+    return np.stack([np.cos(th) * np.sin(phi), np.sin(th) * np.sin(phi), np.cos(phi)], axis=1)
+
+
+def ellipsoid_hull(n, axes, seed, mirror=False):
+    """n points on the ellipsoid with semi-axes `axes` (metres), at jittered Fibonacci directions: every point lies on a strictly
+    convex surface, so every point is a hull vertex.  mirror: the second half is the first mirrored in y (equal support values
+    for directions with no y component: argmax ties between vertices in different lanes of a warp)"""
+    rng = np.random.default_rng(seed)
+    m = n // 2 if mirror else n
+    u = _fib(m) + rng.normal(scale=0.3 / np.sqrt(m), size=(m, 3))
+    if mirror:
+        u[:, 1] = np.maximum(np.abs(u[:, 1]), 0.05)  # strictly one side of y = 0: the mirror images are distinct points
+    u /= np.linalg.norm(u, axis=1, keepdims=True)
+    p = u / np.sqrt(((u / np.asarray(axes)) ** 2).sum(axis=1, keepdims=True))
+    if mirror:
+        p = np.concatenate([p, p * [1.0, -1.0, 1.0]])
+    return p
+
+
+# the convex hulls of the narrow-phase scenes, by mesh name: the 10-vertex probe, and ellipsoidal hulls sized for the mesh support
+# scan (32 lanes: several vertices per lane, ties across lanes) and for the convex kernel's hull staging (see staging_case)
+HULLS = {"probe": _MESH,
+         "hull200": ellipsoid_hull(200, (0.05, 0.035, 0.03), seed=1, mirror=True),
+         "hull2000a": ellipsoid_hull(2000, (0.06, 0.04, 0.03), seed=2),
+         "hull2000b": ellipsoid_hull(2000, (0.035, 0.05, 0.04), seed=3),
+         "hull3000": ellipsoid_hull(3000, (0.07, 0.05, 0.035), seed=4)}
+
 _MESH_DIR = []
 
 
+def _write_obj(path, V):
+    from scipy.spatial import ConvexHull
+
+    hull = ConvexHull(V)
+    faces = []
+    for a, b, c in hull.simplices:  # counter-clockwise seen from outside: the mass properties need outward normals
+        n = np.cross(V[b] - V[a], V[c] - V[a])
+        faces.append((a, b, c) if n @ (V[a] - V.mean(axis=0)) > 0 else (a, c, b))
+    with open(path, "w") as f:
+        f.writelines("v %.17g %.17g %.17g\n" % tuple(v) for v in V)
+        f.writelines("f %d %d %d\n" % tuple(np.array(t) + 1) for t in faces)
+
+
 def _mesh_dir():
-    """a private temporary directory holding the probe mesh as an OBJ file (removed at exit)"""
+    """a private temporary directory holding every hull of HULLS as an OBJ file <name>.obj (removed at exit)"""
     if not _MESH_DIR:
         import atexit
         import shutil
 
-        from scipy.spatial import ConvexHull
-
         d = tempfile.mkdtemp(prefix="b2s_narrow_phase_")
         atexit.register(shutil.rmtree, d, True)
-        hull = ConvexHull(_MESH)
-        faces = []
-        for a, b, c in hull.simplices:  # counter-clockwise seen from outside: the mass properties need outward normals
-            n = np.cross(_MESH[b] - _MESH[a], _MESH[c] - _MESH[a])
-            faces.append((a, b, c) if n @ (_MESH[a] - _MESH.mean(axis=0)) > 0 else (a, c, b))
-        with open(os.path.join(d, "probe.obj"), "w") as f:
-            f.writelines("v %.17g %.17g %.17g\n" % tuple(v) for v in _MESH)
-            f.writelines("f %d %d %d\n" % tuple(np.array(t) + 1) for t in faces)
+        for name, V in HULLS.items():
+            _write_obj(os.path.join(d, name + ".obj"), V)
         _MESH_DIR.append(d)
     return _MESH_DIR[0]
 
 
-def _geom_xml(t, size=None, extra=""):
+def _geom_xml(t, size=None, extra="", mesh="probe"):
     if t == "mesh":
-        return '<geom type="mesh" mesh="probe"%s/>' % extra
+        return '<geom type="mesh" mesh="%s"%s/>' % (mesh, extra)
     sz = " ".join("%.17g" % s for s in (size or SIZES[t]))
     return '<geom type="%s" size="%s"%s/>' % (t, sz, extra)
 
 
-def scene_xml(pair, sizes=(None, None)):
-    """MJCF of one pair: geom 0 is the first type (a world plane, or on free body a), geom 1 the second (on free body b)"""
+def scene_xml(pair, sizes=(None, None), meshes=("probe", "probe"), far=None):
+    """MJCF of one pair: geom 0 is the first type (a world plane, or on free body a), geom 1 the second (on free body b); a mesh
+    geom k uses the hull HULLS[meshes[k]].  far: a third free body far away with the hull HULLS[far], in no pair (collision bits
+    disjoint from the pair's), which only enlarges the model's hulls"""
     t1, t2 = pair
-    asset = '<asset><mesh name="probe" file="probe.obj"/></asset>' if "mesh" in pair else ""
+    used = sorted({meshes[k] for k in range(2) if pair[k] == "mesh"} | ({far} if far else set()))
+    asset = '<asset>%s</asset>' % "".join('<mesh name="%s" file="%s.obj"/>' % (m, m) for m in used) if used else ""
     if t1 == "plane":
-        bodies = '<geom type="plane" size="1 1 0.1"/><body name="b" pos="0 0 0.5"><freejoint/>%s</body>' % _geom_xml(t2, sizes[1])
+        bodies = ('<geom type="plane" size="1 1 0.1"/><body name="b" pos="0 0 0.5"><freejoint/>%s</body>'
+                  % _geom_xml(t2, sizes[1], mesh=meshes[1]))
     else:
         bodies = ('<body name="a" pos="0 0 1"><freejoint/>%s</body><body name="b" pos="0 0 2"><freejoint/>%s</body>'
-                  % (_geom_xml(t1, sizes[0]), _geom_xml(t2, sizes[1])))
+                  % (_geom_xml(t1, sizes[0], mesh=meshes[0]), _geom_xml(t2, sizes[1], mesh=meshes[1])))
+    if far:
+        bodies += '<body name="far" pos="0 0 5"><freejoint/>%s</body>' % _geom_xml("mesh", extra=' contype="2" conaffinity="2"', mesh=far)
     return '<mujoco><option timestep="0.002" cone="elliptic"/>%s<worldbody>%s</worldbody></mujoco>' % (asset, bodies)
+
+
+# mesh-mesh scenes of the hulls above: name -> (meshes of geoms 0 and 1, the far body's hull or None).  Their staging cases per
+# schedule and precision are HULL_STAGING (test_cpu_narrow_phase_warm.py derives them from the capacity formulas)
+HULL_SCENES = {"probe-hull200": (("probe", "hull200"), None), "hull2000a-hull2000b": (("hull2000a", "hull2000b"), None),
+               "hull3000-hull200": (("hull3000", "hull200"), None), "hull3000-hull3000": (("hull3000", "hull3000"), None),
+               "probe-probe": (("probe", "probe"), None), "probe-probe+far200": (("probe", "probe"), "hull200"),
+               "hull200-hull200": (("hull200", "hull200"), None)}
+# the phase pipeline's staging case per scene: (f32, f64)
+HULL_STAGING = {"probe-hull200": ("both", "both"), "hull2000a-hull2000b": ("both", "only A"),
+                "hull3000-hull200": ("both", "only B"), "hull3000-hull3000": ("only A", "neither"),
+                "probe-probe": ("only A", "only A"), "probe-probe+far200": ("same hull", "same hull"),
+                "hull200-hull200": ("only A", "only A")}
+
+
+def hull_poses(meshes, n, seed, tail=()):
+    """(qpos [m, nq], ambiguous flags, names) of a mesh-mesh hull scene: n random poses around contact and a catalogue (coincident
+    centres; unrotated hulls 2 mm into each other along x and deep along z: support directions without a y component, where the
+    mirrored 200-vertex hull has ties); `tail`: the far body's qpos appended to each"""
+    C = np.array([0, 0, 1.0])
+    Q = list(random_poses(("mesh", "mesh"), n, seed, meshes=meshes))
+    amb, names = [False] * n, ["random%d" % i for i in range(n)]
+    A, B = HULLS[meshes[0]], HULLS[meshes[1]]
+    gx = A[:, 0].max() - B[:, 0].min() - 0.002
+    gz = 0.6 * (A[:, 2].max() - B[:, 2].min())
+    for name, q, a in [("concentric", _two(C, I4, C, I4), True), ("concentric_rotated", _two(C, axq([1, 2, 3], 0.7), C, axq([3, -1, 2], 1.1)), True),
+                       ("x_2mm", _two(C, I4, C + [gx, 0, 0], I4), False), ("z_deep", _two(C, I4, C + [0.003, 0, gz], I4), False),
+                       ("deep_offset", _two(C, axq([1, 0, 0], 0.3), C + [0.006, -0.004, 0.008], axq([0, 1, 1], 0.5)), False)]:
+        Q.append(q); amb.append(a); names.append(name)
+    return np.array([np.concatenate([q, tail]) for q in Q]), amb, names
 
 
 def compile_scene(xml):
     from robosuite_b200.mjcf.compiler import compile_mjcf
 
-    return compile_mjcf(xml, mesh_root=_mesh_dir() if 'mesh="probe"' in xml else None)
+    return compile_mjcf(xml, mesh_root=_mesh_dir() if "<mesh " in xml else None)
+
+
+# ------------------------------------------------------------------------------------------------ hull staging
+# The convex narrow phase of the phase pipeline (mode 1) and of the unit queue (mode 2) copies a pair's two poses (24 reals) and, where
+# they fit, its hulls into shared memory before GJK (convex_convex in b2s_collide.cuh).  The pipeline's area holds the model's two
+# largest hulls, at most 56 KB (b2s_capi.cu); the unit queue's is what its per-warp workspace leaves beside the EPA polytope
+# (b2s_unit.cuh), used from 64 reals on.
+EPA_AREA_WORDS = (9 * 96 + 5 * 192 + 64 + 8 + 40 + 3) & ~3
+STAGING_CASES = ("both", "only A", "only B", "neither", "same hull")
+
+
+def _pad4(k):
+    return (k + 3) & ~3
+
+
+def pipeline_stage_cap(vertnums, prec):
+    """the phase pipeline's staging capacity in reals from the model's mesh_vertnum"""
+    n = sorted(vertnums, reverse=True) + [0, 0]
+    return min(24 + _pad4(3 * n[0]) + _pad4(3 * n[1]), 56 * 1024 // (8 if prec == "f64" else 4))
+
+
+def unit_stage_cap(stride_words):
+    """the unit queue's staging capacity in reals from its per-warp workspace stride (0: no staging)"""
+    cap = stride_words - EPA_AREA_WORDS
+    return cap if cap >= 64 else 0
+
+
+def staging_case(nA, nB, same, cap):
+    """which hulls convex_convex stages for hulls of nA and nB vertices (same: two instances of one mesh) in `cap` reals"""
+    if cap <= 0:
+        return "neither"
+    cap -= 24
+    a = 3 * nA <= cap
+    used = _pad4(3 * nA) if a else 0
+    b = used + 3 * nB <= cap
+    if a and b:
+        return "same hull" if same else "both"
+    return "only A" if a else ("only B" if b else "neither")
 
 
 # ------------------------------------------------------------------------------------------------ rotations
@@ -132,13 +243,47 @@ class Geom:
             return s[1] * np.abs(L[:, 2]) + s[0] * np.sqrt(np.maximum(L[:, 0] ** 2 + L[:, 1] ** 2, 0))
         if self.t == "box":
             return (np.abs(L) * s).sum(axis=1)
-        if self.t == "mesh":
-            return (L @ self.vert.T).max(axis=1)
+        if self.t == "mesh":  # in blocks of directions: [n, nvert] at once is gigabytes for the large hulls
+            return np.concatenate([(L[k:k + 2048] @ self.vert.T).max(axis=1) for k in range(0, len(L), 2048)])
+        if self.t == "point":
+            return np.zeros(len(D))
+        if self.t == "segment":
+            return s[1] * np.abs(L[:, 2])
         raise ValueError(self.t)
 
     def support(self, D):
         D = np.atleast_2d(D)
         return self.extent(D) + D @ self.pos
+
+    @property
+    def radius(self):
+        """the radius the narrow phase inflates the core by: spheres and capsules; 0 otherwise"""
+        return float(self.size[0]) if self.t in ("sphere", "capsule") else 0.0
+
+    def core(self):
+        """the shape GJK runs on: a sphere's centre point, a capsule's segment, every other geom itself"""
+        if self.t == "sphere":
+            return Geom("point", self.size, self.pos, self.mat)
+        if self.t == "capsule":
+            return Geom("segment", self.size, self.pos, self.mat)
+        return self
+
+
+def separation_along(A, B, v):
+    """min over a in A of u.a minus max over b in B of u.b, u = v / |v|: positive when the direction separates A from B (a GJK
+    direction v points from B towards A: it is a point of the Minkowski difference A - B)"""
+    u = np.asarray(v, dtype=np.float64) / np.linalg.norm(v)
+    return float(-A.support(-u[None])[0] - B.support(u[None])[0])
+
+
+def core_distance(A, B):
+    """signed distance of the two cores (negative: they overlap by that depth); closed forms for points and segments"""
+    ca, cb = A.core(), B.core()
+    if ca.t in ("point", "segment") and cb.t in ("point", "segment"):
+        ha = ca.size[1] if ca.t == "segment" else 0.0
+        hb = cb.size[1] if cb.t == "segment" else 0.0
+        return seg_seg_dist(ca.pos, ca.mat[:, 2], ha, cb.pos, cb.mat[:, 2], hb)
+    return -mink_depth(ca, cb)
 
 
 def geoms_of(model, o):
@@ -157,13 +302,6 @@ def geoms_of(model, o):
 
 
 # ------------------------------------------------------------------------------------------------ exact signed distances
-def _fib(n):
-    i = np.arange(n) + 0.5
-    phi = np.arccos(1 - 2 * i / n)
-    th = np.pi * (1 + 5 ** 0.5) * i
-    return np.stack([np.cos(th) * np.sin(phi), np.sin(th) * np.sin(phi), np.cos(phi)], axis=1)
-
-
 _DIRS = _fib(20000)
 
 
@@ -276,15 +414,15 @@ def _rand_quat(rng):
     return q / np.linalg.norm(q)
 
 
-def _rbound(t, size):
+def _rbound(t, size, mesh="probe"):
     if t == "mesh":
-        return float(np.linalg.norm(_MESH, axis=1).max())
+        return float(np.linalg.norm(HULLS[mesh], axis=1).max())
     s = np.asarray(size or SIZES[t], dtype=np.float64)
     return {"sphere": s[0], "capsule": s[0] + s[-1], "ellipsoid": s.max(), "cylinder": np.hypot(s[0], s[-1]),
             "box": np.linalg.norm(s)}[t]
 
 
-def random_poses(pair, n, seed, sizes=(None, None)):
+def random_poses(pair, n, seed, sizes=(None, None), meshes=("probe", "probe")):
     """n seeded qpos around contact: geom 2's centre at a random direction from geom 1 (or above the plane), at a distance between
     deep overlap and a little beyond touching"""
     rng = np.random.default_rng(seed)
@@ -294,7 +432,7 @@ def random_poses(pair, n, seed, sizes=(None, None)):
         qb = _rand_quat(rng)
         if t1 == "plane":
             if t2 == "mesh":
-                ext = _rbound(t2, None)
+                ext = _rbound(t2, None, meshes[1])
             else:
                 ext = float(Geom(t2, _pad(sizes[1] or SIZES[t2]), np.zeros(3), quat2mat(qb)).extent(np.array([[0, 0, -1.0]]))[0])
             z = ext * rng.uniform(0.4, 1.15)
@@ -303,7 +441,7 @@ def random_poses(pair, n, seed, sizes=(None, None)):
             qa = _rand_quat(rng)
             d = rng.normal(size=3)
             d /= np.linalg.norm(d)
-            r = (_rbound(t1, sizes[0]) + _rbound(t2, sizes[1])) * rng.uniform(0.15, 0.9)
+            r = (_rbound(t1, sizes[0], meshes[0]) + _rbound(t2, sizes[1], meshes[1])) * rng.uniform(0.15, 0.9)
             pa = np.array([0, 0, 1.0])
             out.append(np.concatenate([pa, qa, pa + r * d, qb]))
     return np.array(out)

@@ -56,7 +56,7 @@ def run_oracle(model, o, qpos):
 def check_pose(pair, model, o, qpos):
     """failures of one pose, and the depth error of its deepest contact (None without a contact)"""
     geoms, cons, ids = run_oracle(model, o, qpos)
-    A, B = geoms
+    A, B = geoms[:2]
     bad = []
     if any(g != (0, 1) for g in ids):
         bad.append("geom ids %s" % ids)
@@ -75,11 +75,11 @@ def _catalogue_cases():
 _MODELS = {}
 
 
-def scene(pair, sizes=(None, None)):
-    key = (pair, sizes)
+def scene(pair, sizes=(None, None), meshes=("probe", "probe"), far=None):
+    key = (pair, sizes, meshes, far)
     if key not in _MODELS:
-        m = npr.compile_scene(npr.scene_xml(pair, sizes))
-        assert m.npair == 1 and m.ngeom == 2
+        m = npr.compile_scene(npr.scene_xml(pair, sizes, meshes, far))
+        assert m.npair == 1 and m.ngeom == (3 if far else 2)
         _MODELS[key] = (m, _oracle(m))
     return _MODELS[key]
 

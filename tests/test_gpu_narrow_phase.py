@@ -68,19 +68,19 @@ def pose_set(pair):
 _REF = {}
 
 
-def oracle_results(pair, Q, sizes_of=lambda i: (None, None)):
-    """per pose: (oracle contacts [(dist, pos, frame, g1, g2)], exact signed distance); cached per pair and size set"""
+def oracle_results(pair, Q, sizes_of=lambda i: (None, None), meshes=("probe", "probe"), far=None):
+    """per pose: (oracle contacts [(dist, pos, frame, g1, g2)], exact signed distance); cached per scene and size set"""
     out = []
     for i, q in enumerate(Q):
         sizes = sizes_of(i)
-        key = (pair, sizes, q.tobytes())
+        key = (pair, sizes, meshes, far, q.tobytes())
         if key not in _REF:
-            model, o = scene(pair, sizes)
+            model, o = scene(pair, sizes, meshes, far)
             o.reset_data()
             o.qpos[:] = q
             o.forward()
             cs = [(c["dist"], c["pos"].copy(), c["frame"].copy(), c["geom1"], c["geom2"]) for c in o.contacts()]
-            A, B = npr.geoms_of(model, o)
+            A, B = npr.geoms_of(model, o)[:2]
             _REF[key] = (cs, npr.signed_distance(A, B, [c[2][0] for c in cs]))
         out.append(_REF[key])
     return out
@@ -110,13 +110,17 @@ def device_contacts(model, Q, prec, sizes=None):
         sim.close()
 
 
-def compare(pair, prec, dev, ref, amb, names):
-    """failures, and the worst (dist, pos, frame) differences"""
+def compare(pair, prec, dev, ref, amb, names, fam=None, tols=None):
+    """failures, and the worst (dist, pos, frame) differences.  fam / tols: the routine family whose gates apply and the exact-geometry
+    tolerances (default family(pair) / tolerances(pair); hulls too large for EPA's polytope to resolve are judged like curved
+    surfaces)"""
     ncon, geom, dist, pos, frame = dev
+    fam = fam or family(pair)
     worst = np.zeros(3)
     bad = []
-    gate = (F64_GATES if prec == "f64" else F32_GATES)[family(pair)]
-    band = tolerances(pair)["band"] if prec == "f64" else F32_BAND
+    gate = (F64_GATES if prec == "f64" else F32_GATES)[fam]
+    tols = tols or tolerances(pair)
+    band = tols["band"] if prec == "f64" else F32_BAND
     for e, (oc, sd) in enumerate(ref):
         n = int(ncon[e])
         if prec == "f32" and names[e] in F32_KNOWN_MISSES.get(pair, ()):
@@ -134,14 +138,14 @@ def compare(pair, prec, dev, ref, amb, names):
             bad.append((names[e], "geom ids"))
         for k, c in enumerate(oc):
             # an ambiguous pose's deep EPA result depends on the polytope's path: its depth is held to the exact reference instead
-            err = np.array([0.0 if amb[e] and family(pair) == "gjk_curved" else abs(dist[e, k] - c[0]), 0.0 if amb[e] else np.abs(pos[e, k] - c[1]).max(),
+            err = np.array([0.0 if amb[e] and fam == "gjk_curved" else abs(dist[e, k] - c[0]), 0.0 if amb[e] else np.abs(pos[e, k] - c[1]).max(),
                             0.0 if amb[e] else np.abs(frame[e, k] - c[2]).max()])
             worst = np.maximum(worst, err)
             if (err > gate).any():
                 bad.append((names[e], "contact %d: |d dist| %.3g |d pos| %.3g |d frame| %.3g" % (k, *err)))
         if n and (prec == "f32" or amb[e]) and pair != ("box", "box"):
             # the deepest contact against exact geometry too (the oracle's own agreement is test_cpu_narrow_phase's)
-            tol = gate[0] + tolerances(pair)["depth"] + tolerances(pair).get("rel", 0.0) * abs(sd)
+            tol = gate[0] + tols["depth"] + tols.get("rel", 0.0) * abs(sd)
             if abs(dist[e, :n].min() - sd) > tol:
                 bad.append((names[e], "deepest dist %.9g vs exact %.9g" % (dist[e, :n].min(), sd)))
     return bad, worst
