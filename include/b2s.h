@@ -143,6 +143,14 @@ int b2s_reset_envs(b2s_sim* sim, const uint8_t* env_mask, const void* qpos_new);
  * replace the constant world pose of that body in every kinematics pass.  Bodies welded to an overridden body keep THEIR constant world
  * pose: override them too (pose = parent pose * local pose).  At most 4 bodies per handle. */
 int b2s_body_pose_override(b2s_sim* sim, int body_id);
+/* The same override (it takes one of the 4 slots and the same arrays, "body_xpos_ov:<id>" / "body_xquat_ov:<id>"), and in addition every
+ * world-welded body below `body_id` that has no override of its own follows it: its pose is (root pose) * (its fixed pose relative to
+ * the root), the relative pose composed from the model's local poses in fp64 on the host once, when the call (or any later override)
+ * is made.  A body follows its nearest overridden ancestor, and only when that ancestor was registered here.  Moving bodies below
+ * such a subtree follow through their parents as always.  Use: a robot's welded root (base, mounts, link0) moved per environment,
+ * e.g. to sit behind a table of per-environment length.  Which bodies follow which root is part of the snapshot signature.  A handle
+ * without a call here runs exactly the code and arithmetic it ran before. */
+int b2s_body_pose_override_tree(b2s_sim* sim, int body_id);
 
 /* Object placement (the reference's UniformRandomSampler / SequentialCompositeSampler.sample, utils/placement_samplers.py, recalled
  * from robosuite v1.5; no reference checkout was available to check it against).  b2s_place_config copies a program of n <= 32

@@ -157,6 +157,9 @@ struct b2s_sim {
   std::vector<char> free_qadr_h;                   // qpos address a is the first of a free joint
   std::vector<int> body_parent_h;
   std::vector<double> body_pos_h, body_quat_h;     // local poses (model constants)
+  // b2s_body_pose_override_tree: the registered roots, and the host copy of the table DState::ov_tree / ov_rel hold (signature)
+  std::vector<int> tree_roots, ov_tree_h;
+  std::vector<double> ov_rel_h;
 };
 
 // Every entry point picks the handle's precision once: f(DModel<R>&, DState<R>&) runs with R = float or double, and
@@ -1380,6 +1383,45 @@ int b2s_reset_envs(b2s_sim* s, const uint8_t* mask, const void* qpos_new) {
 }
 
 }  // extern "C"
+// pose (lp, lq) of body c relative to its ancestor `anc` in fp64: the local poses of the chain below anc composed downwards
+static void chain_pose(const b2s_sim* s, int anc, int c, double* lp, double* lq) {
+  std::vector<int> chain;
+  for (int up = c; up != anc; up = s->body_parent_h[up]) chain.push_back(up);
+  lp[0] = lp[1] = lp[2] = 0; lq[0] = 1; lq[1] = lq[2] = lq[3] = 0;
+  for (auto it = chain.rbegin(); it != chain.rend(); ++it) {  // (lp, lq) <- (lp, lq) * local pose of *it
+    double M[9], q2[4];
+    h_quat2mat(M, lq);
+    const double* bp = &s->body_pos_h[3 * *it];
+    for (int r = 0; r < 3; r++) lp[r] += M[3 * r] * bp[0] + M[3 * r + 1] * bp[1] + M[3 * r + 2] * bp[2];
+    h_qmul(q2, lq, &s->body_quat_h[4 * *it]);
+    for (int r = 0; r < 4; r++) lq[r] = q2[r];
+  }
+}
+
+// the tree-override table (DState::ov_tree / ov_rel) from the registered roots and the handle's overrides: a world-welded body
+// without an override of its own follows its nearest overridden ancestor when that ancestor is a registered root.  Rebuilt whenever
+// an override is added; a handle without roots keeps both pointers null.
+template <typename R> static int rebuild_tree(b2s_sim* s, DState<R>& st) {
+  if (s->tree_roots.empty()) return B2S_OK;
+  const int nb = s->nbody;
+  auto slot_of = [&](int b) { for (int k = 0; k < st.n_ov; k++) if (st.ov_body[k] == b) return k; return -1; };
+  std::vector<int> tree(nb, -1);
+  std::vector<double> rel((size_t)nb * 7, 0.0);
+  for (int b = 1; b < nb; b++) {
+    if (s->body_weldid_h[b] != 0 || slot_of(b) >= 0) continue;
+    int up = s->body_parent_h[b];
+    while (up > 0 && slot_of(up) < 0) up = s->body_parent_h[up];
+    if (up <= 0 || !std::count(s->tree_roots.begin(), s->tree_roots.end(), up)) continue;
+    tree[b] = slot_of(up);
+    chain_pose(s, up, b, &rel[7 * (size_t)b], &rel[7 * (size_t)b + 3]);
+  }
+  try { st.ov_tree = dev_upload(s, tree); st.ov_rel = up_vec<R>(s, rel); } catch (const std::string& e) { return fail(B2S_ERR_CUDA, e); }
+  s->ov_tree_h = tree; s->ov_rel_h = rel;
+  s->dirty = 1;
+  s->layout_version++;
+  return B2S_OK;
+}
+
 template <typename R> static int body_pose_override_t(b2s_sim* s, DState<R>& st, int body) {
   for (int k = 0; k < st.n_ov; k++) if (st.ov_body[k] == body) return B2S_OK;
   if (st.n_ov >= 4) return fail(B2S_ERR_UNSUPPORTED, "b2s_body_pose_override: at most 4 bodies per handle");
@@ -1397,7 +1439,7 @@ template <typename R> static int body_pose_override_t(b2s_sim* s, DState<R>& st,
   s->arrays["body_xquat_ov:" + std::to_string(body)] = ArrayInfo{st.ov_quat[k], code, 2, {s->n_env, 4, 0, 0}};
   s->dirty = 1;
   s->layout_version++;
-  return B2S_OK;
+  return rebuild_tree(s, st);  // a body with an override of its own stops following its root
 }
 // ---- per-environment model values (b2s_model_override) and the set-constants pass
 static bool has_model_overrides(b2s_sim* s) { return with_real(s, [](auto&, auto& st) { return st.dof_iw != nullptr; }); }
@@ -1604,6 +1646,19 @@ int b2s_body_pose_override(b2s_sim* s, int body_id) {
   return with_real(s, [&](auto&, auto& st) { return body_pose_override_t(s, st, body_id); });
 }
 
+int b2s_body_pose_override_tree(b2s_sim* s, int body_id) {
+  if (!s || body_id <= 0 || body_id >= s->nbody) return fail(B2S_ERR_ARG, "b2s_body_pose_override_tree: bad argument");
+  if (s->body_weldid_h[body_id] != 0)
+    return fail(B2S_ERR_UNSUPPORTED, "b2s_body_pose_override_tree: the body is not welded to the world (move it through qpos)");
+  CUDA_TRY(cudaSetDevice(s->device));
+  return with_real(s, [&](auto&, auto& st) {
+    const int rc = body_pose_override_t(s, st, body_id);
+    if (rc != B2S_OK || std::count(s->tree_roots.begin(), s->tree_roots.end(), body_id)) return rc;
+    s->tree_roots.push_back(body_id);
+    return rebuild_tree(s, st);
+  });
+}
+
 int b2s_place_config(b2s_sim* s, const b2s_place* entries, int n) {
   if (!s || n < 0 || n > B2S_PLACE_MAX || (n > 0 && !entries)) return fail(B2S_ERR_ARG, "b2s_place_config: bad argument");
   std::vector<PlaceDev> prog(n);
@@ -1652,18 +1707,10 @@ int b2s_place_config(b2s_sim* s, const b2s_place* entries, int n) {
       add(own, zp, iq);
       for (int k = 0; k < st.n_ov; k++) {
         int c = st.ov_body[k], up = c;
-        std::vector<int> chain;
-        while (up > 0 && up != e.body) { chain.push_back(up); up = s->body_parent_h[up]; }
+        while (up > 0 && up != e.body) up = s->body_parent_h[up];
         if (c == e.body || up != e.body) continue;
-        double lp[3] = {0, 0, 0}, lq[4] = {1, 0, 0, 0};
-        for (auto it = chain.rbegin(); it != chain.rend(); ++it) {  // (lp, lq) <- (lp, lq) * local pose of *it
-          double M[9], q2[4];
-          h_quat2mat(M, lq);
-          const double* bp = &s->body_pos_h[3 * *it];
-          for (int r = 0; r < 3; r++) lp[r] += M[3 * r] * bp[0] + M[3 * r + 1] * bp[1] + M[3 * r + 2] * bp[2];
-          h_qmul(q2, lq, &s->body_quat_h[4 * *it]);
-          for (int r = 0; r < 4; r++) lq[r] = q2[r];
-        }
+        double lp[3], lq[4];
+        chain_pose(s, e.body, c, lp, lq);
         add(k, lp, lq);
       }
       return B2S_OK;
@@ -1968,6 +2015,10 @@ static int ensure_snap(b2s_sim* s) {
   if (s->ctrl.gain) h = fnv1a(h, &s->imp_mode, sizeof(int));  // variable impedance: the action layout (fixed mode hashes nothing new)
   if (s->ctrl.n_sel > 0) {  // the object list (a handle without one hashes what it always did)
     h = fnv1a(h, &s->ctrl.n_sel, sizeof(int)); h = fnv1a(h, s->ctrl.sel_body, sizeof(int) * s->ctrl.n_sel);
+  }
+  if (!s->tree_roots.empty()) {  // tree overrides: which bodies follow which root, and how (a handle without them hashes as before)
+    h = fnv1a(h, s->ov_tree_h.data(), sizeof(int) * s->ov_tree_h.size());
+    h = fnv1a(h, s->ov_rel_h.data(), sizeof(double) * s->ov_rel_h.size());
   }
   CUDA_TRY(cudaSetDevice(s->device));
   if (!s->snap_dev) {

@@ -214,13 +214,24 @@ struct Eng {
       __syncwarp();
     }
     const R* qpos = p(L.qpos);
-    // bodies welded to the world: constant pose
+    // bodies welded to the world: constant pose, the environment's override, or (tree overrides) the override of the root they
+    // follow composed with their fixed pose relative to it
     for (int b = lane; b < m.nbody; b += 32)
       if (m.body_weldid[b] == 0) {
         const R* px = m.body_xpos0 + 3 * b; const R* pq = m.body_xquat0 + 4 * b;
         const DState<R>& st = state();
         for (int k = 0; k < st.n_ov; k++)
           if (st.ov_body[k] == b) { px = st.ov_pos[k] + 3 * (size_t)env; pq = st.ov_quat[k] + 4 * (size_t)env; }
+        R tp[3], tq[4];
+        const int root = st.ov_tree ? st.ov_tree[b] : -1;
+        if (root >= 0) {
+          const R* rp = st.ov_pos[root] + 3 * (size_t)env; const R* rq = st.ov_quat[root] + 4 * (size_t)env;
+          const R* rel = st.ov_rel + 7 * b;
+          qrot(tp, rq, rel);
+          tp[0] += rp[0]; tp[1] += rp[1]; tp[2] += rp[2];
+          qmul(tq, rq, rel + 3);
+          px = tp; pq = tq;
+        }
         R q[4] = {pq[0], pq[1], pq[2], pq[3]};
         xpos[3 * b] = px[0]; xpos[3 * b + 1] = px[1]; xpos[3 * b + 2] = px[2];
         xquat[4 * b] = q[0]; xquat[4 * b + 1] = q[1]; xquat[4 * b + 2] = q[2]; xquat[4 * b + 3] = q[3];

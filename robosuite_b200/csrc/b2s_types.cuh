@@ -108,6 +108,10 @@ struct DState {
   int n_ov, ov_body[4];
   R* ov_pos[4];    // [n_env, 3]
   R* ov_quat[4];   // [n_env, 4]
+  // tree overrides (b2s_body_pose_override_tree): per body, the override slot k of the root whose pose it follows (-1: none; never a
+  // body with an override of its own), and its pose relative to that root [nbody][7] (pos, quat).  Both null without tree overrides
+  const int* ov_tree;
+  const R* ov_rel;
   // per-environment model values (b2s_model_override): up to B2S_MOV colliding primitive geoms (size, friction) and B2S_MOV moving
   // bodies (mass, principal moments).  Slot k of environment e sits at [k * n_env + e].  n_mg == n_mb == 0 and null derived
   // arrays: the handle has no overrides and every lookup (b2s_engine.cuh, *_of) costs one warp-uniform test.

@@ -120,6 +120,7 @@ def lib():
         L.b2s_env_step.argtypes = [C.c_void_p, C.c_void_p, C.c_int]
         L.b2s_reset_envs.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
         L.b2s_body_pose_override.argtypes = [C.c_void_p, C.c_int]
+        L.b2s_body_pose_override_tree.argtypes = [C.c_void_p, C.c_int]
         L.b2s_model_override.argtypes = [C.c_void_p, C.c_char_p, C.c_int]
         L.b2s_set_const.argtypes = [C.c_void_p, C.c_void_p]
         L.b2s_perturb_config.argtypes = [C.c_void_p, C.POINTER(PerturbSpec), C.c_int]
@@ -337,6 +338,12 @@ class BatchedSim:
         """(pos [n_env, 3], quat [n_env, 4]) tensors that replace the constant world pose of a world-welded body per environment
         (b2s_body_pose_override; the reference writes model.body_pos / body_quat per reset, door.py:417-427)"""
         self._check(self._L.b2s_body_pose_override(self._h, int(body_id)))
+        return self.array("body_xpos_ov:%d" % body_id), self.array("body_xquat_ov:%d" % body_id)
+
+    def body_pose_override_tree(self, body_id):
+        """body_pose_override, and every world-welded body below it without an override of its own follows it with its fixed
+        relative pose (b2s_body_pose_override_tree): a robot's welded root moved per environment"""
+        self._check(self._L.b2s_body_pose_override_tree(self._h, int(body_id)))
         return self.array("body_xpos_ov:%d" % body_id), self.array("body_xquat_ov:%d" % body_id)
 
     def model_override(self, field, obj_id=None):

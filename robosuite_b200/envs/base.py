@@ -107,6 +107,50 @@ SIM_WARN_BITS = {1: "singular mass matrix", 2: "non-finite state in the integrat
                        "reference raises RandomizationError"}
 
 
+# The reference's TableArena and robot base placement, recalled from robosuite v1.5 (models/arenas/table_arena.py,
+# models/robots/manipulators/{panda,sawyer}_robot.py base_xpos_offset["table"]); no reference checkout was available.  Pinned by the
+# packaged models, which the reference composer produced with the default arguments (tests/test_cpu_arena.py checks each):
+#   table body pos    = table_offset - (0, 0, table_full_size[2] / 2)        (0.775 in Lift / Stack / Door, 0.795 in NutAssembly)
+#   table_collision   = box, half sizes table_full_size / 2, friction table_friction   (0.4 0.4 0.025; 1 0.005 1e-4)
+#   robot0_base pos x = -0.16 - table_full_size[0] / 2, y and z unchanged     (-0.56 everywhere, Door's 0.8-long table included)
+# Recalled only: that the top of the table stays at table_offset[2] for every thickness, and that the legs are visual (they are
+# not modelled here: no geom of theirs collides).
+TABLE_GEOM, TABLE_BODY, ROBOT_ROOT = "table_collision", "table", "robot0_base"
+
+
+def _arena_value(name, v, num_envs):
+    """a table argument as float64: [3] (batch-wide) or [num_envs, 3] (per environment); ValueError on any other shape, a non-finite
+    or a non-positive value"""
+    import torch
+
+    a = np.array(v.detach().cpu() if torch.is_tensor(v) else v, dtype=np.float64)
+    if a.shape not in ((3,), (num_envs, 3)):
+        raise ValueError("{} must be a length-3 sequence or a [num_envs, 3] = [{}, 3] array, got shape {}".format(name, num_envs, a.shape))
+    if not (np.all(np.isfinite(a)) and np.all(a > 0)):
+        raise ValueError("{} must be finite and > 0, got {}".format(name, v))
+    return a
+
+
+def table_model(model, table_offset, full_size, friction):
+    """a copy of `model` with the reference's table of `full_size` / `friction` and the robot base behind it (the rules above); the
+    table geom's bounding data and the model's derived constants come from the compiler's own code"""
+    import copy
+
+    from ..mjcf.compiler import GEOM_BOX, _set_const, primitive_geom_props
+
+    m = copy.copy(model)
+    for f in ("body_pos", "geom_size", "geom_friction", "geom_rbound", "geom_aabb"):
+        setattr(m, f, np.array(getattr(model, f), dtype=np.float64))
+    g, tb, rb = m.names["geom"].index(TABLE_GEOM), m.names["body"].index(TABLE_BODY), m.names["body"].index(ROBOT_ROOT)
+    m.body_pos[tb] = [table_offset[0], table_offset[1], table_offset[2] - full_size[2] / 2]
+    m.geom_size[g] = np.asarray(full_size, dtype=np.float64) / 2
+    m.geom_friction[g] = friction
+    _, _, m.geom_rbound[g], m.geom_aabb[g] = primitive_geom_props(GEOM_BOX, m.geom_size[g])
+    m.body_pos[rb, 0] = -0.16 - full_size[0] / 2
+    _set_const(m)
+    return m
+
+
 class BatchedMujocoEnv(ContactQueries):
     """N copies of one task on one GPU.  All returned arrays are torch.cuda tensors with leading dim N.
     contact_queries=True switches the contact export on (BatchedSim.set_contact_export) before the first reset, so that
@@ -127,13 +171,21 @@ class BatchedMujocoEnv(ContactQueries):
     # per-environment tensors of the task layer that a snapshot carries besides the engine rows, the episode clocks and `done`
     # (attribute names; [N, ...] device tensors)
     _task_state = ()
+    # the reference's table arguments and their defaults (Lift, Stack, NutAssembly); a task whose table cannot take other values
+    # names the reason in `_table_args_refused`, and non-default values raise NotImplementedError with it
+    table_full_size_default = (0.8, 0.8, 0.05)
+    table_friction_default = (1.0, 5e-3, 1e-4)
+    _table_args_refused = None
 
     def __init__(self, robots="Panda", num_envs=1, device=0, controller_configs=None, control_freq=20, horizon=500,
                  ignore_done=False, reward_scale=1.0, reward_shaping=False, use_object_obs=True, seed=None,
                  initialization_noise="default", precision="f32", xml=None, has_renderer=False,
                  has_offscreen_renderer=False, use_camera_obs=False, hard_reset=False, lite_physics=True, model=None,
                  kernel_mode="pipeline", sim_cls=None, contact_queries=False, data_queries=False,
-                 dynamics_queries=False, placement_initializer=None, **kwargs):
+                 dynamics_queries=False, placement_initializer=None, table_full_size=None, table_friction=None, **kwargs):
+        """table_full_size / table_friction: the reference's TableArena arguments (see table_model), a length-3 sequence for every
+        environment (the model is edited before the engine is created) or a [num_envs, 3] array or tensor, one table per environment
+        (per-environment geom values and a moved table and robot base on the device; set_table changes them later)"""
         import torch
 
         if has_renderer or has_offscreen_renderer or use_camera_obs:
@@ -152,6 +204,8 @@ class BatchedMujocoEnv(ContactQueries):
         self.initialization_noise = {"magnitude": 0.02, "type": "gaussian"} if initialization_noise == "default" \
             else (initialization_noise or {"magnitude": 0.0, "type": "gaussian"})
         self.model = model if model is not None else self._load_model(xml)
+        self.model = self._arena_model(self.model)
+        per_env_table = self._table_arguments(table_full_size, table_friction)
         self.model_timestep = self.model.opt_timestep
         self.control_timestep = 1.0 / control_freq
         if control_freq <= 0:
@@ -176,6 +230,9 @@ class BatchedMujocoEnv(ContactQueries):
         self.obs_dim = len(op)
         self.sim.obs_config(op, a, b)
         self._setup_task()
+        self._table_ov = None
+        if per_env_table:
+            self._setup_table_overrides()
         self.sim.set_export(False)
         self._contact_queries = bool(contact_queries or dynamics_queries)  # contact_force() reads the contact records too
         if self._contact_queries:
@@ -234,6 +291,79 @@ class BatchedMujocoEnv(ContactQueries):
 
     def _setup_task(self):
         pass
+
+    def _arena_model(self, model):
+        """the task's arena arguments other than the table applied to the model (PickPlace's bins); the default: none"""
+        return model
+
+    # ---- the table arguments (TableArena: see table_model)
+    def _table_arguments(self, full_size, friction):
+        """validate table_full_size / table_friction, apply batch-wide values that differ from the defaults to self.model, and
+        return whether any value is per environment.  Default values leave the model untouched."""
+        size = None if full_size is None else _arena_value("table_full_size", full_size, self.num_envs)
+        fric = None if friction is None else _arena_value("table_friction", friction, self.num_envs)
+        default = [v is None or (v.ndim == 1 and np.array_equal(v, d))
+                   for v, d in ((size, self.table_full_size_default), (fric, self.table_friction_default))]
+        if self._table_args_refused is not None and not all(default):
+            raise NotImplementedError("{}: table_full_size / table_friction: {}".format(type(self).__name__, self._table_args_refused))
+        self.table_full_size = np.array(self.table_full_size_default if size is None else size)
+        self.table_friction = np.array(self.table_friction_default if fric is None else fric)
+        batch = [v is not None and v.ndim == 1 and not dflt for v, dflt in zip((size, fric), default)]
+        if any(batch):
+            self.model = table_model(self.model, self.table_offset, self.table_full_size if batch[0] else self.table_full_size_default,
+                                     self.table_friction if batch[1] else self.table_friction_default)
+        return any(v is not None and v.ndim == 2 for v in (size, fric))
+
+    def _setup_table_overrides(self):
+        """per-environment table: size and friction of table_collision through the engine's model overrides, the table body and the
+        robot's welded root through pose overrides (the root's welded subtree follows it), written by set_table"""
+        m, sim = self.model, self.sim
+        g, tb, rb = m.names["geom"].index(TABLE_GEOM), m.names["body"].index(TABLE_BODY), m.names["body"].index(ROBOT_ROOT)
+        self._table_ov = (sim.model_override("geom_size", g), sim.model_override("geom_friction", g),
+                          sim.body_pose_override_tree(tb)[0], sim.body_pose_override_tree(rb)[0])
+        self.set_table(self.table_full_size, self.table_friction)
+
+    def set_table(self, full_size=None, friction=None, mask=None):
+        """Give the masked environments (bool [num_envs] device tensor, None = all) a new table: full_size / friction as a length-3
+        sequence or a [num_envs, 3] array or tensor (rows of unmasked environments are ignored), None = unchanged.  Needs a handle
+        built with per-environment table arguments.  The table, its friction and the robot base move at once and the derived
+        constants are recomputed; meant to be followed by reset(mask=mask).  Called mid-episode, the next step starts from the old
+        state in the new scene: a cube resting on a thinner table falls onto it, and the arm, carried with its base, keeps its joint
+        angles."""
+        import torch
+
+        if self._table_ov is None:
+            raise RuntimeError("set_table needs per-environment table arguments at construction: table_full_size / table_friction "
+                               "as a [num_envs, 3] array")
+        size_ov, fric_ov, table_pos, base_pos = self._table_ov
+        sel = torch.ones(self.num_envs, dtype=torch.bool) if mask is None else mask.detach().to("cpu", torch.bool).reshape(self.num_envs)
+        rows = sel.numpy()
+
+        def per_env(name, v):
+            a = _arena_value(name, v, self.num_envs)
+            return np.broadcast_to(a, (self.num_envs, 3)).copy()
+
+        def put(dst, src):
+            dst[sel.to(dst.device)] = torch.as_tensor(src[rows], device=dst.device, dtype=dst.dtype)
+
+        size = per_env("table_full_size", full_size) if full_size is not None else None
+        fric = per_env("table_friction", friction) if friction is not None else None
+        if size is not None:
+            off = self.table_offset
+            put(size_ov, size / 2)
+            put(table_pos, np.stack([np.full(self.num_envs, float(off[0])), np.full(self.num_envs, float(off[1])),
+                                     off[2] - size[:, 2] / 2], 1))
+            base = base_pos.detach().cpu().numpy().astype(np.float64)
+            base[:, 0] = -0.16 - size[:, 0] / 2
+            put(base_pos, base)
+            self.table_full_size = np.broadcast_to(self.table_full_size, (self.num_envs, 3)).copy()
+            self.table_full_size[rows] = size[rows]
+        if fric is not None:
+            put(fric_ov, fric)
+            self.table_friction = np.broadcast_to(self.table_friction, (self.num_envs, 3)).copy()
+            self.table_friction[rows] = fric[rows]
+        self._table_mask8 = None if mask is None else sel.to(device=self.device, dtype=torch.uint8).contiguous()  # kept alive
+        self.sim.set_const(self._table_mask8)
 
     def _robot_reset_qpos(self, n):
         """[n, nq] float64 qpos0 with the arm at init_qpos + noise and the gripper at its init pose

@@ -23,6 +23,9 @@ class BatchedDoor(BatchedMujocoEnv):
     DOOR_META = dict(radius=0.3, bottom=-0.3, top=0.3)
 
     def __init__(self, *args, door_placement=None, **kwargs):
+        if kwargs.get("table_full_size") is not None or kwargs.get("table_friction") is not None:
+            raise NotImplementedError("Door: table_full_size / table_friction: the reference's Door has a fixed (0.8, 0.3, 0.05) table "
+                                      "and takes no table arguments")
         # (x, y, yaw) relative to table_offset; sampler ranges x [0.07, 0.09], y [-0.01, 0.01], yaw [-pi/2 - 0.25, -pi/2]
         if door_placement is not None and kwargs.get("placement_initializer") is not None:
             raise ValueError("door_placement pins the door; a placement_initializer samples it: give one of them")

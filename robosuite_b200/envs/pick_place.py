@@ -28,11 +28,25 @@ class BatchedPickPlace(SingleObjectMixin, BatchedMujocoEnv):
     tier_small = (12, 56)  # small tail tier: see BatchedMujocoEnv.tier_small
     _task_state = ("objects_in_bins",)  # carried by get_env_state / set_env_state (mode 1's selection: by the engine's snapshot)
 
-    bin1_pos = np.array([0.1, -0.25, 0.8])   # pick_place.py:186-187
+    bin1_pos = np.array([0.1, -0.25, 0.8])   # pick_place.py:186-187 (pinned: the packaged model's bin1 / bin2 bodies)
     bin2_pos = np.array([0.1, 0.28, 0.8])
     bin_size = np.array([0.39, 0.49, 0.82])  # BinsArena table_full_size (pick_place.py:184)
+    table_full_size_default = (0.39, 0.49, 0.82)
+    table_friction_default = (1.0, 5e-3, 1e-4)
+    _table_args_refused = "the bins arena's wall geometry for another table is not known here"
 
-    def __init__(self, *args, single_object_mode=0, object_type=None, **kwargs):
+    def __init__(self, *args, single_object_mode=0, object_type=None, bin1_pos=None, bin2_pos=None, z_offset=0.0, z_rotation=None,
+                 **kwargs):
+        """bin1_pos / bin2_pos: world positions of the two bins (bin 1 holds the objects at reset, bin 2 the targets and the success
+        regions); z_offset: added to every object's placement height; z_rotation: the placement yaw, None = U[0, 2 pi), a number = that
+        angle, a (lo, hi) pair = U[lo, hi) (the reference's UniformRandomSampler `rotation`, recalled from robosuite v1.5).  The bins
+        are moved in the model, for every environment; the robot base stays where the bins arena puts it."""
+        self.bin1_pos = self._position("bin1_pos", bin1_pos, type(self).bin1_pos)
+        self.bin2_pos = self._position("bin2_pos", bin2_pos, type(self).bin2_pos)
+        if not (isinstance(z_offset, (int, float, np.floating, np.integer)) and math.isfinite(float(z_offset))):
+            raise ValueError("z_offset must be a finite number, got {!r}".format(z_offset))
+        self.z_offset = float(z_offset)
+        self.z_rotation = self._rotation(z_rotation)
         self.single_object_mode, self._fixed_object = parse_mode(single_object_mode, object_type, self.object_to_id, "object_type")
         self._object_names = self.obj_names
         if self.single_object_mode:
@@ -41,8 +55,43 @@ class BatchedPickPlace(SingleObjectMixin, BatchedMujocoEnv):
             self.tier_small = (18, 80)
         super().__init__(*args, **kwargs)
 
+    @staticmethod
+    def _position(name, v, default):
+        if v is None:
+            return default
+        a = np.array(v, dtype=np.float64)
+        if a.shape != (3,) or not np.all(np.isfinite(a)):
+            raise ValueError("{} must be 3 finite numbers, got {!r}".format(name, v))
+        return a
+
+    @staticmethod
+    def _rotation(r):
+        """z_rotation as None or a (lo, hi) pair (a number: (a, a))"""
+        if r is None:
+            return None
+        a = np.array(r, dtype=np.float64)
+        if a.shape == ():
+            a = np.array([a, a])
+        if a.shape != (2,) or not np.all(np.isfinite(a)):
+            raise ValueError("z_rotation must be None, a finite number or a (lo, hi) pair, got {!r}".format(r))
+        return float(a.min()), float(a.max())
+
     def _load_model(self, xml):
         return load_task_model("PickPlace", self.robot_name, xml)
+
+    def _arena_model(self, model):
+        """bin1 / bin2 bodies at bin1_pos / bin2_pos (world-welded, children of the world); the defaults leave the model untouched"""
+        import copy
+
+        moved = [(n, p) for n, p, d in (("bin1", self.bin1_pos, type(self).bin1_pos), ("bin2", self.bin2_pos, type(self).bin2_pos))
+                 if not np.array_equal(p, d)]
+        if not moved:
+            return model
+        m = copy.copy(model)
+        m.body_pos = np.array(model.body_pos, dtype=np.float64)
+        for n, p in moved:
+            m.body_pos[m.names["body"].index(n)] = p
+        return m
 
     def _setup_references(self):
         super()._setup_references()
@@ -99,7 +148,7 @@ class BatchedPickPlace(SingleObjectMixin, BatchedMujocoEnv):
         for name in self.obj_names:
             meta = OBJ_META[name]
             r = meta["hradius"]
-            z = float(self.bin1_pos[2] - meta["bottom"])
+            z = float((self.z_offset + self.bin1_pos[2]) - meta["bottom"])
 
             # R candidate positions per environment, the first one that clears every object placed before is taken: the distribution of the
             # reference's sequential rejection loop without a device->host round trip per attempt (no candidate fits: < 1e-12 per reset)
@@ -114,7 +163,12 @@ class BatchedPickPlace(SingleObjectMixin, BatchedMujocoEnv):
             ok[R - 1] = True
             first = torch.argmax(ok.to(torch.uint8), dim=0, keepdim=True)
             x, y = torch.gather(cx, 0, first)[0], torch.gather(cy, 0, first)[0]
-            yaw = torch.rand((n,), generator=self.rng, device=dev, dtype=torch.float64) * 2 * math.pi
+            yaw = torch.rand((n,), generator=self.rng, device=dev, dtype=torch.float64)
+            if self.z_rotation is None:
+                yaw = yaw * 2 * math.pi
+            else:
+                lo, hi = self.z_rotation
+                yaw = lo + yaw * (hi - lo) if hi > lo else torch.full_like(yaw, lo)
             self._place_free_body(q, self.obj_qadr[name], x, y, torch.full((n,), z, device=dev, dtype=torch.float64), yaw)
             placed.append((x, y, z, meta))
         self._park_objects(q)

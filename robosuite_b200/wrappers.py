@@ -252,6 +252,9 @@ class BatchedDomainRandomizationWrapper:
                     spec.append(("body_inertia", b, "scale", a["inertia_perturbation_ratio"], True))
         if geom_on:
             geoms = self.default_geoms(bodies) if a["geom_names"] is None else self._ids("geom", a["geom_names"])
+            if getattr(env, "_table_ov", None) is not None and m.names["geom"].index("table_collision") in geoms:
+                raise ValueError("the task sets the friction of table_collision itself (per-environment table_friction / "
+                                 "table_full_size, set_table): leave it out of geom_names")
             if len(geoms) > _MAX_OBJECTS:
                 raise NotImplementedError("%d geoms selected, the engine holds %d per-environment geoms: pass geom_names"
                                           % (len(geoms), _MAX_OBJECTS))
